@@ -2,7 +2,7 @@
 """bench.py -- forward+backward Mpixels/s of the differentiable Gaussian rasterizer on BASELINE config 3
 (1M synthetic "bicycle-shaped" Gaussians, SH degree 3, 1600x1200), the metric BASELINE.json names.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c3] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one camera: GaussianRasterizer.forward (preprocess + tile-count
 difference array -> R to the host -> depth order -> scan -> ranges -> two radix passes over tile ids (the first
@@ -10,8 +10,8 @@ generates the instances) -> blend, plus output/workspace allocation) + autograd 
 protocol).  The 8 ring cameras of the config are cycled step by step.
 
   value  : W*H*steps / t / 1e6 with every input resident in HBM before the timed region (CUDA events, max over
-           ranks).  Inputs (236 MB of Gaussian parameters + 192 MB of SH gradients written) exceed the 126 MB
-           L2, so no separate L2 flush is needed between iterations.
+           ranks).  Inputs (236 MB of Gaussian parameters + 192 MB of SH gradients written) exceed the 50 MB
+           L2 of an H100, so no separate L2 flush is needed between iterations.
   e2e    : the same step through the public API with HOST buffers: each step copies the camera and the G image
            from pinned host memory (H2D; the 23 MB image on a side stream, overlapping the forward) and reads the
            loss back (D2H into pinned memory) inside the timed region. The read-back is asynchronous and the host
@@ -21,10 +21,14 @@ protocol).  The 8 ring cameras of the config are cycled step by step.
            the path shards over views with no data-path collective ("weak" scaling); value = all ranks' pixels
            / max-over-ranks time.
   --impl reference : the reference's OWN CUDA path (oracle/_ref/libdgr_ref.so = its unmodified .cu files
-           compiled for sm_100a) on the same workload; if that library is absent, the CPU oracle port.
+           compiled for sm_90a) on the same workload; if that library is absent, the CPU oracle port.
 
-  timing : every number is the MEDIAN of 5 back-to-back regions of K steps (each bracketed by barrier + synchronize);
-           the five region times are reported under "timing".
+  timing : the K timed steps are split into up to 5 back-to-back regions (each bracketed by barrier + synchronize);
+           every number is the MEDIAN ms/step over those regions, and the region times are reported under "timing".
+           The e2e leg times its own K steps the same way.
+  --dump-outputs DIR : after the timed steps, write what the last timed step of the headline leg returned to its
+           caller as DIR/<name>.npy (float32): the image and depth in full, radii and the loss, and the gradients of
+           every Gaussian parameter on a fixed seeded sample of 65536 Gaussians (sample_index.npy).
   N > 1 also runs BASELINE config 4 (5M Gaussians, 1920x1080) through the Gaussian-sharded rasterizer over all N
            GPUs (strong scaling) and reports it under "sharded_c4": ms/step, Mpixels/s, ratio to the plain rasterizer
            on one GPU measured in the same run, bit-comparison of the 8 frames, per-phase times, exchange bytes.
@@ -67,12 +71,12 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, not measured)"
 
 
 class ClockSampler:
-    """SM clock + throttle reasons DURING the timed region (B200_PROFILING.md recipe). NVML is polled from a thread every
-    ~4 ms (a timed region of K steps lasts only K x 1.4 ms); if NVML is unavailable, `nvidia-smi -lms 100` is used."""
+    """SM clock + throttle reasons DURING the timed region. NVML is polled from a thread every ~4 ms (a timed region
+    lasts only a few ms per step); if NVML is unavailable, `nvidia-smi -lms 100` is used."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
     BITS = {"sw_power_cap": 0x4, "hw_slowdown": 0x8, "sw_thermal_slowdown": 0x20, "hw_thermal_slowdown": 0x40}
@@ -106,6 +110,7 @@ class ClockSampler:
             phys = int(vis.split(",")[self.gpu]) if vis and all(x.strip().isdigit() for x in vis.split(",")) else self.gpu
             h = nv.nvmlDeviceGetHandleByIndex(phys)
             self.max_mhz = float(nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM))
+            self.power_limit_w = nv.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
             self.nvml = (nv, h)
             self.t = threading.Thread(target=self._nvml_loop, daemon=True)
             self.t.start()
@@ -132,7 +137,7 @@ class ClockSampler:
             sm = [r[0] for r in self.rows]
             reasons = sorted(n for n, b in self.BITS.items() if any(r[1] & b for r in self.rows))
             return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": self.max_mhz, "reasons": reasons,
-                    "samples": len(sm), "source": "nvml"}
+                    "power_limit_w": self.power_limit_w, "samples": len(sm), "source": "nvml"}
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
@@ -186,8 +191,8 @@ class Workload:
         """e2e leg: this step's inputs travel from pinned host memory inside the timed region. The camera (144 B) goes
         on the compute stream; the 23 MB G image is only needed by the loss, so it is copied on a side stream into one
         of two persistent device buffers and overlaps whatever the GPU is doing when the host issues it (the tail of
-        the previous step and this step's forward); the compute stream waits for it right before the loss. The copy
-        takes 0.42 ms at the measured 54 GB/s (`e2e.h2d_GBps_measured`). A buffer is reused only after the backward
+        the previous step and this step's forward); the compute stream waits for it right before the loss (the copy
+        bandwidth is reported as `e2e.h2d_GBps_measured`). A buffer is reused only after the backward
         that read it (two steps earlier) has finished -- an event, not an allocation, guards it: per-step allocation
         of the image on the side stream made the caching allocator stall once the run got longer than ~50 steps."""
         cur = torch.cuda.current_stream(self.dev)
@@ -268,9 +273,17 @@ class OursRunner:
             wl.join_host_inputs()
         loss = (color * G).sum()
         loss.backward()
+        self.last_out = (color, radii, depth, loss)
         if host:
             return wl.read_back(loss)
         return loss
+
+    def outputs(self):
+        """What the caller of the last step received: image, radii, depth, loss and the parameter gradients."""
+        color, radii, depth, loss = self.last_out
+        L = self.leaf
+        return dict(color=color, radii=radii, depth=depth, loss=loss, grad_means2D=self.means2D.grad,
+                    **{"grad_" + k: L[k].grad for k in ("means3D", "opacities", "shs", "scales", "rotations")})
 
     def describe(self):
         from gaussianeditor_b200.rasterizer import _RasterizeGaussians, forward_state_views
@@ -314,9 +327,17 @@ class ReferenceCudaRunner:
         # autograd of loss = (color*G).sum() hands dL/dcolor = G to the rasterizer's backward
         self.g = self.R.backward(dL_dcolor=G, radii=radii, R=R, **common)
         self.last = (radii, R)
+        self.last_out = (color, radii, depth, loss)
         if host:
             return wl.read_back(loss)
         return loss
+
+    def outputs(self):
+        color, radii, depth, loss = self.last_out
+        g = self.g
+        return dict(color=color, radii=radii, depth=depth, loss=loss, grad_means2D=g["dL_dmeans2D"],
+                    grad_means3D=g["dL_dmeans3D"], grad_opacities=g["dL_dopacity"], grad_shs=g["dL_dsh"],
+                    grad_scales=g["dL_dscales"], grad_rotations=g["dL_drotations"])
 
     def describe(self):
         radii, R = self.last
@@ -344,6 +365,42 @@ def cpu_oracle_time(name, P=None, threads=None, budget_s=12.0, max_steps=8):
         n += 1
     dt = (time.perf_counter() - t0) / n
     return dt, cams[0].image_width * cams[0].image_height, cpu_oracle.num_threads(), n
+
+
+DUMP_SAMPLE = 65536   # Gaussians whose radii and gradients --dump-outputs writes (the full SH gradient alone is 192 MB at config 3)
+DUMP_LIMIT = 64 << 20  # bytes --dump-outputs writes at most
+
+
+def dump_outputs(out_dir, outs, P):
+    """Write one step's outputs as .npy files (float32; the sample indices float64), at most DUMP_LIMIT bytes in all, so
+    that two builds can be compared output for output. Per-Gaussian arrays (radii, gradients) are reduced to a fixed
+    seeded sample of DUMP_SAMPLE Gaussians (sample_index.npy). The image and depth are written whole when they fit in
+    what is left of DUMP_LIMIT, otherwise on a fixed seeded sample of pixels (pixel_index.npy, row-major y*W+x)."""
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(P, size=min(P, DUMP_SAMPLE), replace=False))
+    arrays = {"sample_index": idx.astype(np.float64)}
+    images = {}
+    for name, t in outs.items():
+        t = t.detach()
+        if name.startswith("grad_") or name == "radii":
+            t = t.reshape(P, -1)[torch.from_numpy(idx).to(t.device)].reshape((len(idx),) + tuple(t.shape[1:]))
+        elif name in ("color", "depth"):
+            images[name] = t
+            continue
+        arrays[name] = t.float().cpu().numpy()
+    used = sum(a.nbytes for a in arrays.values())
+    if 4 * sum(t.numel() for t in images.values()) > DUMP_LIMIT - used:
+        HW = images["color"].shape[-1] * images["color"].shape[-2]
+        planes = sum(t.numel() // HW for t in images.values())
+        n = min(HW, (DUMP_LIMIT - used) // (4 * planes + 8))   # float32 per plane + the float64 pixel index
+        pix = np.sort(np.random.default_rng(1).choice(HW, size=n, replace=False))
+        arrays["pixel_index"] = pix.astype(np.float64)
+        sel = torch.from_numpy(pix)
+        images = {k: t.reshape(t.numel() // HW, HW)[:, sel.to(t.device)] for k, t in images.items()}
+    arrays.update({k: t.float().cpu().numpy() for k, t in images.items()})
+    assert sum(a.nbytes for a in arrays.values()) <= DUMP_LIMIT
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def alg_bytes(desc, M, Msh, W, H):
@@ -551,7 +608,11 @@ def main():
     ap.add_argument("--option", action="append", default=[], help="library tuning option k=v (A/B measurements only)")
     ap.add_argument("--no-sharded", action="store_true", help="skip the config-4 Gaussian-sharded leg at --gpus N > 1")
     ap.add_argument("--sharded-points", type=int, default=None, help="override config 4's Gaussian count (debug only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -574,11 +635,13 @@ def main():
     config = {"workload": f"BASELINE config 3: 1M synthetic bicycle-shaped Gaussians, SH degree 3, 1600x1200, "
                           f"8 ring cameras cycled, loss=(color*G).sum()" if name == "c3" else f"config {name}",
               "P": args.points or cfg["P"], "sh_degree": cfg["sh_degree"], "image": [cfg["W"], cfg["H"]],
-              "l2": "inputs (236 MB params + 192 MB SH grads) exceed the 126 MB L2; no explicit flush",
+              "l2": "inputs (236 MB params + 192 MB SH grads) exceed the 50 MB L2; no explicit flush",
               "parallelism": f"replicas x{world} (one camera stream per GPU, no data-path collective)"}
 
     if use_cpu_port:
         # reference arm without the compiled reference: the CPU oracle port, rank 0 only
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs needs a GPU path (ours, or the compiled reference)")
         if rank != 0:
             return
         dt, npix, thr, nst = cpu_oracle_time(name, P=args.points, max_steps=max(1, min(args.steps, 8)))
@@ -611,12 +674,12 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
-    def timed_once(n, host):
+    def timed_once(first, n, host):
         barrier()
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         pending, losses = None, []
-        for i in range(n):
+        for i in range(first, first + n):
             cur = runner.step(i + rank * 3, host=host)
             if host:  # consume step i-1's loss on the host while step i runs on the GPU
                 if pending is not None:
@@ -637,32 +700,37 @@ def main():
     REPEATS = 5
 
     def timed(n, host):
-        """The K-step timed region (barrier + synchronize on both sides, CUDA events, max over ranks) is measured
-        REPEATS times back to back and the MEDIAN region is reported: K = 20 steps last 28 ms, so one host hiccup
-        (GC, a page fault, a neighbour rank's launch burst) in a single region used to move the number by 10-20 %.
-        Python's cyclic GC is paused inside the regions for the same reason (it runs between them)."""
+        """The n timed steps are split into up to REPEATS back-to-back regions (barrier + synchronize on both sides,
+        CUDA events, max over ranks) and the MEDIAN ms/step over the regions is returned: one host hiccup (GC, a page
+        fault, a neighbour rank's launch burst) inside a single region then cannot move the number. Python's cyclic
+        GC is paused inside the regions for the same reason (it runs between them). Steps are numbered 0..n-1 across
+        the regions, so the cameras are cycled as in one run of n steps."""
         import gc
-        runs = []
-        for _ in range(REPEATS):
+        sizes = [n // REPEATS + (r < n % REPEATS) for r in range(min(REPEATS, n))]
+        runs, first = [], 0
+        for k in sizes:
             gc.collect()
             gc.disable()
             try:
-                runs.append(timed_once(n, host))
+                runs.append(timed_once(first, k, host))
             finally:
                 gc.enable()
-        return statistics.median(runs), runs
+            first += k
+        return statistics.median(r / k for r, k in zip(runs, sizes)), runs
 
     for i in range(max(args.warmup, 3)):
         runner.step(i + rank * 3)
     launches0 = _lib.launch_count() if args.impl == "ours" else 0
     sampler = ClockSampler(local_rank)
     sampler.start()
-    ms, ms_runs = timed(args.steps, host=False)
+    ms_step, ms_runs = timed(args.steps, host=False)
     clocks = sampler.stop()
     launches = (_lib.launch_count() - launches0) if args.impl == "ours" else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, runner.outputs(), wl.P)
     for i in range(3):
         runner.step(i, host=True).wait()
-    ms_e2e, ms_e2e_runs = timed(args.steps, host=True)
+    ms_e2e_step, ms_e2e_runs = timed(args.steps, host=True)
     desc = runner.describe()
 
     # host->device bandwidth of the G image copy alone (explains the e2e/value gap when the copy is the longer leg)
@@ -675,22 +743,23 @@ def main():
     torch.cuda.synchronize()
     h2d_gbps = 4 * wl.G_host.numel() * 4 / (ca.elapsed_time(cb) * 1e-3) / 1e9
 
-    value = world * npix * args.steps / (ms * 1e-3) / 1e6
-    e2e = world * npix * args.steps / (ms_e2e * 1e-3) / 1e6
+    value = world * npix / (ms_step * 1e-3) / 1e6
+    e2e = world * npix / (ms_e2e_step * 1e-3) / 1e6
     line = {"metric": metric, "value": value, "unit": "Mpixels/s", "n_gpus": world, "steps": args.steps,
-            "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps, "higher_is_better": True,
+            "warmup": max(args.warmup, 3), "ms_per_step": ms_step, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "impl": args.impl,
-            "config": config, "clocks": clocks,
-            "timing": {"protocol": f"median of {REPEATS} back-to-back regions of {args.steps} steps each (every region "
-                                   "bracketed by barrier + synchronize, CUDA events, max over ranks)",
+            "config": config, "device": torch.cuda.get_device_name(dev), "clocks": clocks,
+            "timing": {"protocol": f"{args.steps} timed steps in {len(ms_runs)} back-to-back regions, median ms/step "
+                                   "over the regions (every region bracketed by barrier + synchronize, CUDA events, "
+                                   "max over ranks)",
                        "region_ms": [round(x, 4) for x in ms_runs], "e2e_region_ms": [round(x, 4) for x in ms_e2e_runs]},
-            "e2e": {"value": e2e, "unit": "Mpixels/s", "ms_per_step": ms_e2e / args.steps,
+            "e2e": {"value": e2e, "unit": "Mpixels/s", "ms_per_step": ms_e2e_step,
                     "h2d_bytes_per_step": 3 * npix * 4 + 36 * 4, "d2h_bytes_per_step": 4,
                     "h2d_GBps_measured": round(h2d_gbps, 1)},
             "workload": desc}
 
     if args.impl == "ours":
-        line["gpu_launches"] = int(launches) // REPEATS   # per timed region of `steps` steps
+        line["gpu_launches"] = int(launches)   # over the `steps` timed steps
         # per-stage CUDA-event timing (separate pass so the headline is not perturbed)
         _lib.set_option("profile", 1)
         _lib.profile_read()
@@ -706,26 +775,11 @@ def main():
         dom = max(stages, key=stages.get)
         peak, peak_src = measured_peaks()
         ach = ab[dom] / (stages[dom] * 1e-3) / 1e9
-        traffic, issue = None, None
-        try:  # DRAM bytes and instruction count per launch from the committed ncu --set full capture of the same command
-            tp = os.path.join(ROOT, "profiles", "r02_traffic.json")
-            with open(tp if os.path.exists(tp) else os.path.join(ROOT, "profiles", "r01_traffic.json")) as f:
-                kd = json.load(f)["kernels"][dom]
-            traffic = kd["dram_bytes"]
-            # second lens for the issue-bound render kernels: warp instructions per launch (ncu) / live kernel time,
-            # against 148 SMs x 4 schedulers x 1 instruction per clock at the clock sampled during the timed region
-            sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-            peak_inst = 148 * 4 * sm_mhz * 1e6
-            issue = {"warp_inst_per_launch": kd["warp_inst"], "achieved_Ginst_s": kd["warp_inst"] / (stages[dom] * 1e-3) / 1e9,
-                     "peak_Ginst_s": peak_inst / 1e9, "frac": kd["warp_inst"] / (stages[dom] * 1e-3) / peak_inst,
-                     "ipc_per_sm_under_ncu": kd.get("ipc_per_sm")}
-        except Exception:
-            pass
         line["roofline"] = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
-                            "frac": ach / peak, "traffic": traffic, "peak_source": peak_src,
+                            "frac": ach / peak, "peak_source": peak_src,
                             "note": "the render kernels are FP32-issue bound, not HBM bound (DESIGN.md section 5): "
                                     "frac is the share of the HBM time the algorithmic bytes would need",
-                            "alg_bytes": ab[dom], "kernel_ms": stages[dom], "issue": issue,
+                            "alg_bytes": ab[dom], "kernel_ms": stages[dom],
                             "all": {k: {"ms": round(stages[k], 4), "alg_GB": round(ab[k] / 1e9, 4),
                                         "GBps": round(ab[k] / (stages[k] * 1e-3) / 1e9, 1),
                                         "frac": round(ab[k] / (stages[k] * 1e-3) / 1e9 / peak, 4)}

@@ -1,4 +1,4 @@
-"""gaussianeditor_b200 -- a B200-native (sm_100a) differentiable 3D-Gaussian-splatting rasterizer that drops in
+"""gaussianeditor_b200 -- an H100-native (sm_90a) differentiable 3D-Gaussian-splatting rasterizer that drops in
 behind GaussianEditor's ``gaussiansplatting/gaussian_renderer.render()``.
 
 Only the one hot path is here (see DESIGN.md): ``csrc/`` holds the hand-written CUDA kernels behind a C ABI

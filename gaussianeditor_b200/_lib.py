@@ -105,7 +105,7 @@ _lib = None
 
 
 def build(verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into csrc/libgsr_b200.so (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu for sm_90a into csrc/libgsr_b200.so (nvcc cross-compiles without a GPU)."""
     out = None if verbose else subprocess.DEVNULL
     subprocess.check_call(["make", "-C", os.path.join(_HERE, "csrc"), "-j8"], stdout=out)
     return LIB_PATH

@@ -1,4 +1,4 @@
-// Semantic tracing ("apply_weights") for sm_100a.
+// Semantic tracing ("apply_weights") for sm_90a.
 //
 // Semantics: renderCUDA_apply_weights of GaussianEditor's fork (cuda_rasterizer/apply_weights.cu:240-356):
 // the forward walk of a tile list with the forward's skip / stop rules, but instead of blending, every

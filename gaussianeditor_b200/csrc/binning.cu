@@ -1,4 +1,4 @@
-// Binning for sm_100a: turn per-Gaussian tile rectangles into per-tile, depth-ordered splat lists.
+// Binning for sm_90a: turn per-Gaussian tile rectangles into per-tile, depth-ordered splat lists.
 //
 // The reference (cuda_rasterizer/rasterizer_impl.cu:227-270) emits one 64-bit key  tile<<32 | depth_bits  per
 // (Gaussian, tile) instance in Gaussian-index order and radix-sorts all R instances over 32+bit key bits

@@ -1,4 +1,4 @@
-// Shared declarations of the sm_100a rasterizer kernels (internal; the public surface is include/gsr_b200.h).
+// Shared declarations of the sm_90a rasterizer kernels (internal; the public surface is include/gsr_b200.h).
 #pragma once
 #include <cuda_runtime.h>
 #include <atomic>
@@ -110,6 +110,17 @@ struct StageScope {
   ~StageScope();
 };
 extern Options g_opt;
+
+// SM count of the current device, queried once per device: the grid size cap of the grid-stride kernels.
+inline int device_sm_count() {
+  static std::atomic<int> cached[64];
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  if (dev >= 0 && dev < 64 && (n = cached[dev].load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 1;
+  if (dev >= 0 && dev < 64) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
 extern unsigned long long* g_stats_dev;  // device counters when option "stats" is on (instrumentation only)
 extern std::atomic<long long> g_launches;
 
@@ -178,7 +189,7 @@ int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const Binni
 
 // Reference numerics of one (pixel, splat) evaluation, fixed with explicit round-to-nearest intrinsics so the
 // compiler can neither re-associate nor contract differently. The sequence is what nvcc emits for
-// forward.cu:335-338 / backward.cu:491-494 at sm_100a (SASS of the unmodified reference, see DESIGN.md):
+// forward.cu:335-338 / backward.cu:491-494 at sm_90a (SASS of the unmodified reference, see DESIGN.md):
 //   power = fma( fma(dx, A*dx, (C*dy)*dy), -0.5, -((B*dx)*dy) )
 __device__ __forceinline__ float splat_power(float dx, float dy, float A, float B, float C) {
   float t0 = __fmul_rn(__fmul_rn(dy, C), dy);

@@ -1,4 +1,4 @@
-// Depth order of the P Gaussians and the scan of their tile counts in that order, without CUB (sm_100a).
+// Depth order of the P Gaussians and the scan of their tile counts in that order, without CUB (sm_90a).
 //
 // Contract (binning.cu / tile_binning.cu rely on it; the reference gets the same order from the low 32 bits of its
 // 64-bit keys and the stability of its radix sort, cuda_rasterizer/rasterizer_impl.cu:67-100,253-261):

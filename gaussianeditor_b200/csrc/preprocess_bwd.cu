@@ -1,4 +1,4 @@
-// Backward of the per-Gaussian preprocess for sm_100a: 2-D gradients -> gradients of means3D, scales,
+// Backward of the per-Gaussian preprocess for sm_90a: 2-D gradients -> gradients of means3D, scales,
 // rotations (or cov3D), SH coefficients (or colours) and opacity.
 //
 // Semantics: the reference's two kernels computeCov2DCUDA (cuda_rasterizer/backward.cu:144-274) and

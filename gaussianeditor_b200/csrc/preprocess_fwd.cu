@@ -1,4 +1,4 @@
-// Forward per-Gaussian preprocess for sm_100a: near cull, projection, 3-D covariance, EWA 2-D covariance,
+// Forward per-Gaussian preprocess for sm_90a: near cull, projection, 3-D covariance, EWA 2-D covariance,
 // conic, screen radius, tile rectangle, SH -> RGB; writes one 48-byte splat record per visible Gaussian.
 //
 // Semantics follow the reference kernel preprocessCUDA (cuda_rasterizer/forward.cu:155-256 with its helpers
@@ -7,10 +7,10 @@
 // ill-conditioned for elongated splats, so the projection / covariance chain is pinned with _rn intrinsics to
 // the exact FMA contraction nvcc produces for the reference's expression trees (GLM's column-major mat3 product
 // order, type_mat3x3.inl:486-518; ndc2Pix in fp64), decoded from the SASS of the unmodified reference build.
-// radii, tile counts, means2D, depth, conic and rgb are bit-identical to the reference's CUDA build on the B200
+// radii, tile counts, means2D, depth, conic and rgb are bit-identical to the reference's CUDA build on the same GPU
 // (tests/test_parity_gpu.py).
 //
-// B200-specific structure:
+// Hopper-specific structure:
 //   * the 192-byte SH row of each Gaussian that survives the near-plane test is fetched by the TMA unit
 //     (cp.async.bulk, one 16-byte-aligned row per thread, completion on one CTA mbarrier) into a padded
 //     shared-memory row while the thread does the covariance math; culled Gaussians (39 % of config 3)
@@ -233,7 +233,7 @@ __global__ void __launch_bounds__(PRE_THREADS) preprocess_fwd_kernel(const PreAr
 
     // ---- 3-D covariance (forward.cu:118-152); the quaternion is used as given ----
     // From here to the conic every operation is pinned with _rn intrinsics to the exact sequence nvcc emits for
-    // the reference at sm_100a (decoded from the SASS of the unmodified build, DESIGN.md "Numerics"): every
+    // the reference at sm_90a (decoded from the SASS of the unmodified build, DESIGN.md "Numerics"): every
     // three-term product sum a0*b0 + a1*b1 + a2*b2 is fma(a2,b2, fma(a0,b0, a1*b1)), and the quaternion terms
     // fuse exactly the products noted below. The chain feeds det = a*c - b*b, which cancels catastrophically for
     // elongated splats, so a different (equally valid) contraction changes conics in the 4th digit.

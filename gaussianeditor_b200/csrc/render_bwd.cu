@@ -1,4 +1,4 @@
-// Backward of the alpha blending for sm_100a: per-pixel dL/dcolor -> per-Gaussian 2-D gradients
+// Backward of the alpha blending for sm_90a: per-pixel dL/dcolor -> per-Gaussian 2-D gradients
 // (dL/dcolor, dL/dmean2D, dL/dconic, dL/dopacity), accumulated into the 48-byte-per-Gaussian scratch `acc`.
 //
 // Semantics: renderCUDA (bwd) of the reference (cuda_rasterizer/backward.cu:399-557): walk each tile's list
@@ -12,7 +12,7 @@
 //     three quarters of every list lie behind the last contributor of all 256 pixels and are never loaded;
 //   * warp variants (1/2/3 branchy, 4..9 branch-light, 10/11 skip by sub-block mask, 12..14 register caps; DEFAULT 14 =
 //     one warp per half tile, 96 registers -> 5 CTAs/SM, updates of sub-blocks without a hit skipped warp-uniformly:
-//     0.544 ms at config 3; the A/B of all of them is in DESIGN.md section 3): a
+//     0.627 ms at config 3 on an H100 80GB HBM3; the A/B of all of them is in DESIGN.md section 3): a
 //     warp owns a whole tile, half or a quarter of it, each lane owns one pixel of each of its
 //     8x4 sub-blocks; the nine partial sums are first accumulated over the lane's own pixels in registers,
 //     then summed across the warp with a transposing butterfly (16 shuffles for 9 values instead of 45), and

@@ -1,4 +1,4 @@
-// Sparse exchange of the Gaussian-sharded multi-GPU path (BASELINE config 4, SURVEY.md 8(e)) for sm_100a.
+// Sparse exchange of the Gaussian-sharded multi-GPU path (BASELINE config 4, SURVEY.md 8(e)) for sm_90a.
 //
 // The dense scheme of gsr_shard_* sends every 48-byte splat record to every rank, depth-sorts all P keys on every
 // rank and reduce-scatters all P gradient rows (three P-sized steps that do not shrink with the number of GPUs).
@@ -546,7 +546,7 @@ int gsr_sparse_return(const gsr_sparse_plan* plan, const void* acc_cand, const i
   }
   cudaStream_t st = (cudaStream_t)stream;
   const size_t total = (size_t)plan->world * plan->seg_cap * 3;
-  const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)148 * 16);
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)device_sm_count() * 16);
   sparse_return_kernel<<<blocks, 256, 0, st>>>(a);
   g_launches++;
   return check_launch("sparse_return", false, st);

@@ -1,4 +1,4 @@
-// Tile binning for sm_100a without CUB: per-tile ranges from a 2-D difference array, and the stable sort of the R
+// Tile binning for sm_90a without CUB: per-tile ranges from a 2-D difference array, and the stable sort of the R
 // (Gaussian, tile) instances by tile id as TWO hand-written radix passes with decoupled look-back, the first of which
 // generates its input on the fly (instance emission fused in).
 //

@@ -107,7 +107,7 @@ def make_view(cam: synth.Camera, device):
 def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densification_interval=100, seed=0,
                   log=None, fused_activations=False):
     """Returns a dict with total / render wall times (CUDA-event timed) and the per-step Gaussian counts.
-    ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (B200 rasterizer only)."""
+    ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only)."""
     from . import gaussian_renderer as GR
     cloud, cams = synth.make_config("c5", P=P)
     scene = EditScene(cloud, device)

@@ -2,7 +2,7 @@
 (/root/reference/gaussiansplatting/gaussian_renderer/__init__.py: ``camera2rasterizer`` :21-42, ``render`` :45-150).
 
 Same names, arguments, result dictionary and conventions, so GaussianEditor's edit/add/delete loops that call
-``render(cam, gaussians, pipe, bg)`` work on top of the B200 rasterizer without touching the callers.  The
+``render(cam, gaussians, pipe, bg)`` work on top of this rasterizer without touching the callers.  The
 optional Python-side SH->RGB / covariance paths of the reference (``pipe.convert_SHs_python`` /
 ``pipe.compute_cov3D_python``, both False in every GaussianEditor config, arguments/__init__.py:63-67) are
 supported through the same rasterizer arguments.

@@ -3,7 +3,7 @@
 Same public names, argument meaning, return values and error messages as
 /root/reference/gaussiansplatting/submodules/diff-gaussian-rasterization/diff_gaussian_rasterization/__init__.py
 (``GaussianRasterizationSettings`` :228-240, ``GaussianRasterizer`` :243-364, ``rasterize_gaussians`` :26-47,
-``_RasterizeGaussians`` :50-225), backed by the sm_100a C-ABI library instead of the ``_C`` pybind module.
+``_RasterizeGaussians`` :50-225), backed by the sm_90a C-ABI library instead of the ``_C`` pybind module.
 
 Differences a caller can observe (all documented in DESIGN.md):
   * kernels run on PyTorch's CURRENT stream (the reference always used the legacy default stream);
@@ -126,7 +126,7 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:46-48
     if not means3D.is_cuda:
-        raise RuntimeError("the B200 rasterizer needs CUDA tensors (there is no CPU path)")
+        raise RuntimeError("the rasterizer needs CUDA tensors (there is no CPU path)")
     device = means3D.device
     P = means3D.size(0)
     H, W = int(rs.image_height), int(rs.image_width)

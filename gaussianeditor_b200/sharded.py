@@ -81,8 +81,8 @@ def init_distributed(backend: str = "nccl", device: Optional[torch.device] = Non
     """``init_process_group`` from the torchrun environment with the one setting this path needs.
 
     ProcessGroupNCCL by default calls ``record_stream`` on every tensor a collective touches; the workspaces here are
-    several hundred MB, freed and re-allocated every step, and the deferred frees cost ~0.8 ms per step at config 3
-    (1.98 -> 1.13 ms measured on 2xB200). All collectives of this path are synchronous on the compute stream, so
+    several hundred MB, freed and re-allocated every step, and the deferred frees cost a large share of a step at
+    config 3. All collectives of this path are synchronous on the compute stream, so
     stream recording is not needed: TORCH_NCCL_AVOID_RECORD_STREAMS=1 (must be set before the group is created)."""
     import os
     import torch.distributed as dist
@@ -293,7 +293,7 @@ def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D
     if ws is not None and ws.peer is not None:
         peer = ws.peer
     if not means3D.is_cuda:
-        raise RuntimeError("the B200 rasterizer needs CUDA tensors (there is no CPU path)")
+        raise RuntimeError("the rasterizer needs CUDA tensors (there is no CPU path)")
     if means3D.size(0) != plan.count:
         raise RuntimeError(f"rank {plan.rank} owns {plan.count} Gaussians, got {means3D.size(0)}")
     device = means3D.device
@@ -500,8 +500,7 @@ class ShardedGaussianRasterizer(nn.Module):
             self.sparse_pool = SS.SparsePool(self.plan, dev, int(raster_settings.image_width),
                                              int(raster_settings.image_height), self.exchange, depth=max_in_flight)
         else:
-            # fused preprocess + all-gather through peer-mapped workspaces (measured 2xB200, config 4: 2.15 ms/step vs
-            # ~2.33 with the NCCL all-gather)
+            # fused preprocess + all-gather through peer-mapped workspaces (faster than the NCCL all-gather)
             self.pool = WorkspacePool(self.exchange, _geometry_bytes(_lib.load(), self.plan.P_pad),
                                       bool(can_p2p if p2p is None else p2p))
 

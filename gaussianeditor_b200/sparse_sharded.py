@@ -152,7 +152,7 @@ def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D
     lib = _lib.load()
     plan, device = rk.plan, rk.device
     if not means3D.is_cuda:
-        raise RuntimeError("the B200 rasterizer needs CUDA tensors (there is no CPU path)")
+        raise RuntimeError("the rasterizer needs CUDA tensors (there is no CPU path)")
     if means3D.size(0) != plan.count:
         raise RuntimeError(f"rank {plan.rank} owns {plan.count} Gaussians, got {means3D.size(0)}")
     if not (1 <= cap <= rk.cap_alloc):

@@ -1,4 +1,4 @@
-/* gsr_b200.h -- C ABI of the B200-native (sm_100a) differentiable 3D-Gaussian-splatting rasterizer.
+/* gsr_b200.h -- C ABI of the H100-native (sm_90a) differentiable 3D-Gaussian-splatting rasterizer.
  *
  * This is the drop-in boundary for the ONE hot path of buaacyw/GaussianEditor this repo rebuilds:
  * the `diff_gaussian_rasterization._C` extension behind gaussiansplatting/gaussian_renderer.render().
@@ -21,7 +21,7 @@
  *     default stream and blocked on a cudaMemcpy (rasterizer_impl.cu:237) -- here the only host
  *     synchronisation is the caller waiting for `num_rendered` between the two forward halves.
  *   - return value: 0 = ok, <0 = error (see gsr_last_error()).  There is NO CPU fallback: without a usable
- *     sm_100 device every compute entry point fails with GSR_ERR_CUDA.
+ *     sm_90 device every compute entry point fails with GSR_ERR_CUDA.
  *   - all floating-point data is IEEE binary32, exactly as in the reference.
  */
 #ifndef GSR_B200_H_

@@ -2,7 +2,7 @@
 
 Python front-end of ``oracle/_ref/libdgr_ref.so``: the reference's OWN CUDA rasterizer sources
 (/root/reference/gaussiansplatting/submodules/diff-gaussian-rasterization/cuda_rasterizer/*.cu), compiled
-unmodified for sm_100a by ``oracle/Makefile`` (target ``ref``) behind the thin C shim ``oracle/ref_shim.cu``.
+unmodified for sm_90a by ``oracle/Makefile`` (target ``ref``) behind the thin C shim ``oracle/ref_shim.cu``.
 It restates only the reference's torch glue (rasterize_points.cu:35-157: output allocation, zero-filled
 gradient tensors) so the reference kernels and host orchestration can run on the GPU box without building the
 reference's torch extension.  Used by the GPU parity tests as THE primary oracle and by ``bench.py --impl
@@ -28,7 +28,9 @@ def lib():
     global _lib
     if _lib is None:
         if not available():
-            raise RuntimeError(f"{LIB_PATH} missing: run `make -C oracle ref` where /root/reference exists")
+            raise RuntimeError(f"{LIB_PATH} missing: build() compiles it when the GaussianEditor checkout is present "
+                               "($GSR_REFERENCE; or `make -C oracle ref REF=<checkout>/gaussiansplatting/submodules/"
+                               "diff-gaussian-rasterization`)")
         L = C.CDLL(LIB_PATH)
         L.dgr_create.restype = C.c_void_p
         L.dgr_destroy.argtypes = [C.c_void_p]

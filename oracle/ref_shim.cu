@@ -8,7 +8,7 @@
 // (rasterize_points.cu:35-234) without libtorch: the caller owns inputs/outputs (device
 // pointers), the three opaque byte buffers (rasterize_points.cu:62-69) live in a grow-only
 // cudaMalloc arena per context.  Used to (a) pin our CUDA path and the CPU oracle bit-for-bit
-// against the real reference on the B200, (b) time the reference's CUDA path as the A/B baseline.
+// against the real reference on the GPU, (b) time the reference's CUDA path as the A/B baseline.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>

@@ -30,13 +30,13 @@ def test_library_exports_every_declared_symbol():
     assert lib.gsr_abi_version() == 2
 
 
-def test_library_contains_sm100a_code_and_tma():
+def test_library_contains_sm90a_code_and_tma():
     import shutil
     import subprocess
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert "UBLKCP" in sass  # cp.async.bulk (TMA unit) in the preprocess kernels
 

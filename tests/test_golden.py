@@ -1,5 +1,6 @@
 """Golden vectors produced by the REFERENCE's own CUDA build (oracle/_ref, i.e. the unmodified reference .cu files)
-on a B200 with tools/make_golden.py and committed under tests/golden/.
+with tools/make_golden.py and committed under tests/golden/ (forward outputs are the same on every GPU the reference
+was run on; gradients differ only by the order of its float atomics).
 
   * CPU (no GPU needed): the oracle restatement reproduces them -- integers exactly (up to the documented FMA-contraction
     slack), floats to tolerance. This is what pins the oracle to the real reference when no GPU is at hand.

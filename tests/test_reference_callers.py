@@ -1,261 +1,194 @@
-"""The reference's OWN callers of the hot path, imported unchanged from /root/reference (build container only; the
-GPU box has no reference tree, so these CPU tests skip there).
+"""The reference's OWN callers of the hot path, recorded by tools/make_caller_golden.py into
+tests/golden/callers/reference_callers.npz (the reference's modules imported unchanged, with ``diff_gaussian_rasterization``
+resolving to THIS repository's drop-in package and ``plyfile`` / ``simple_knn`` stubbed):
 
-  * gaussiansplatting/gaussian_renderer/__init__.py and scene/gaussian_model.py are imported with
-    ``diff_gaussian_rasterization`` resolving to THIS repository's drop-in package and the two third-party modules
-    that are absent from the image (``plyfile``, ``simple_knn``) stubbed: every name, positional slot and keyword the
-    reference uses on the rasterizer must exist here (SURVEY 7.3-10 / 8(f-2));
-  * the reference's optimizer surgery (scene/gaussian_model.py:553-641) is RUN on CPU tensors next to
-    gaussianeditor_b200/optim_surgery.py: parameters and Adam state must be equal bit for bit;
-  * the reference's ``save_ply`` (:410-445) is RUN with a capturing ``plyfile`` stub: the structured array it hands to
-    plyfile (field names, order, float32 values) must serialise to exactly the bytes gaussianeditor_b200/ply_io.py
-    writes behind the header (SURVEY 8(f-4)); ``load_ply`` (:447-501) is run on top of our reader.
+  * gaussiansplatting/gaussian_renderer/__init__.py and scene/gaussian_model.py: every name, keyword and positional
+    slot the reference uses on the rasterizer must exist here (SURVEY 7.3-10 / 8(f-2));
+  * the reference's optimizer surgery (scene/gaussian_model.py:553-641) run on CPU tensors: parameters, returned
+    tensors and Adam state of gaussianeditor_b200/optim_surgery.py must equal the recorded ones bit for bit. Inputs and
+    Adam state come from numpy's seeded generator and the surgery only moves data, so the recorded bits do not depend
+    on the CPU's vector unit; the one Adam step afterwards is compared in-process against an Adam rebuilt from the
+    reference's recorded state;
+  * the reference's ``save_ply`` (:410-445): the structured array it hands to plyfile (field names, order, float32
+    values) must serialise to exactly the bytes gaussianeditor_b200/ply_io.py writes behind the header, and our reader
+    must give back every recorded column.
 """
-import ast
-import copy
 import inspect
+import json
 import os
-import sys
-import types
 
 import numpy as np
 import pytest
 import torch
 
-REF = "/root/reference"
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "gaussiansplatting")),
-                                reason="reference tree not present (GPU box)")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-class _Captured:
-    def __init__(self, data, name):
-        self.data, self.name = data, name
-
-
-def _install_stubs():
-    """plyfile: just enough to CAPTURE what the reference hands over / to serve what our reader parsed."""
-    ply = types.ModuleType("plyfile")
-
-    class PlyElement:
-        @staticmethod
-        def describe(data, name):
-            return _Captured(data, name)
-
-    class PlyData:
-        last_written = None
-
-        def __init__(self, elements):
-            self.elements = elements
-
-        def write(self, path):
-            PlyData.last_written = (path, self.elements)
-
-        @staticmethod
-        def read(path):
-            from gaussianeditor_b200 import ply_io
-            cols = ply_io.read_vertex_table(path)
-            names = list(cols)
-
-            class _El:
-                properties = [types.SimpleNamespace(name=n) for n in names]
-
-                def __getitem__(self, k):
-                    return cols[k]
-            return types.SimpleNamespace(elements=[_El()])
-    ply.PlyElement, ply.PlyData = PlyElement, PlyData
-    knn = types.ModuleType("simple_knn")
-    knn_c = types.ModuleType("simple_knn._C")
-    knn_c.distCUDA2 = lambda pts: torch.full((pts.shape[0],), 1e-2)
-    knn._C = knn_c
-    sys.modules.setdefault("plyfile", ply)
-    sys.modules.setdefault("simple_knn", knn)
-    sys.modules.setdefault("simple_knn._C", knn_c)
-    return sys.modules["plyfile"]
+GOLDEN = os.path.join(ROOT, "tests", "golden", "callers", "reference_callers.npz")
+GROUPS = [("xyz", 1.6e-4), ("f_dc", 2.5e-3), ("f_rest", 1.25e-4), ("opacity", 0.05), ("scaling", 5e-3), ("rotation", 1e-3)]
+PLY_DEGREES = [0, 1, 3]
 
 
 @pytest.fixture(scope="module")
-def ref():
-    for p in (ROOT, REF):
-        if p not in sys.path:
-            sys.path.insert(0, p)
-    ply = _install_stubs()
+def gold():
+    z = np.load(GOLDEN)
+    return z, json.loads(str(z["api"]))
+
+
+def _normal(rng, *shape):
+    return torch.from_numpy(rng.standard_normal(shape).astype(np.float32))
+
+
+def bare_model(P=13, deg=2, seed=0):
+    """Parameters and non-trivial Adam state (step 3, seeded moments) of a GaussianModel, from numpy's seeded generator."""
+    rng = np.random.default_rng(seed)
+    K = (deg + 1) ** 2 - 1
+    shapes = {"xyz": (P, 3), "f_dc": (P, 1, 3), "f_rest": (P, K, 3), "opacity": (P, 1), "scaling": (P, 3),
+              "rotation": (P, 4)}
+    params = {n: torch.nn.Parameter(_normal(rng, *shapes[n])) for n, _ in GROUPS}
+    opt = torch.optim.Adam([{"params": [params[n]], "lr": lr, "name": n} for n, lr in GROUPS], lr=0.0, eps=1e-15)
+    for n, _ in GROUPS:
+        opt.state[params[n]] = {"step": torch.tensor(3.0), "exp_avg": _normal(rng, *shapes[n]),
+                                "exp_avg_sq": _normal(rng, *shapes[n]).abs()}
+    return params, opt
+
+
+def surgery_inputs():
+    """Mask, extension tensors and replacement opacity of the surgery test (numpy's seeded generator)."""
+    rng = np.random.default_rng(5)
+    keep = torch.from_numpy(rng.uniform(size=13) > 0.4)
+    ext = {"xyz": _normal(rng, 4, 3), "f_dc": _normal(rng, 4, 1, 3), "f_rest": _normal(rng, 4, 8, 3),
+           "opacity": _normal(rng, 4, 1), "scaling": _normal(rng, 4, 3), "rotation": _normal(rng, 4, 4)}
+    return rng, keep, ext
+
+
+def adam_from(z, tag):
+    """An Adam over fresh parameters holding the state recorded under `tag` (the reference's, after its surgery)."""
+    params = {n: torch.nn.Parameter(torch.from_numpy(z[f"{tag}/{n}/param"].copy())) for n, _ in GROUPS}
+    opt = torch.optim.Adam([{"params": [params[n]], "lr": lr, "name": n} for n, lr in GROUPS], lr=0.0, eps=1e-15)
+    for n, _ in GROUPS:
+        opt.state[params[n]] = {k: torch.from_numpy(z[f"{tag}/{n}/{k}"].copy()) for k in ("step", "exp_avg", "exp_avg_sq")}
+    return opt
+
+
+def adam_step(opt):
+    opt.zero_grad()
+    sum((gr["params"][0] ** 2).sum() for gr in opt.param_groups).backward()
+    opt.step()
+
+
+def snapshot(opt, tag):
+    """{tag/group/param|exp_avg|exp_avg_sq|step: array} of an optimizer."""
+    out = {}
+    for gr in opt.param_groups:
+        p = gr["params"][0]
+        out[f"{tag}/{gr['name']}/param"] = p.detach().numpy().copy()
+        for k, v in opt.state.get(p, {}).items():
+            out[f"{tag}/{gr['name']}/{k}"] = (v.numpy() if torch.is_tensor(v) else np.asarray(v)).copy()
+    return out
+
+
+def returned(d, tag):
+    return {f"{tag}/ret/{k}": v.detach().numpy().copy() for k, v in d.items()}
+
+
+def _assert_recorded(z, got, tag):
+    want = sorted(k for k in z.files if k.startswith(tag + "/"))
+    assert sorted(got) == want, tag
+    for k in want:
+        assert got[k].dtype == z[k].dtype and np.array_equal(got[k], z[k]), k
+
+
+def test_reference_render_uses_only_names_the_drop_in_has(gold):
     import diff_gaussian_rasterization as dgr
-    assert os.path.dirname(dgr.__file__).startswith(ROOT), "the reference must resolve the drop-in, not its own package"
-    import gaussiansplatting.gaussian_renderer as GR
-    import gaussiansplatting.scene.gaussian_model as GM
-    return types.SimpleNamespace(GR=GR, GM=GM, ply=ply, dgr=dgr)
-
-
-def _calls(tree, func_pred):
-    for node in ast.walk(tree):
-        if isinstance(node, ast.Call) and func_pred(node.func):
-            yield node
-
-
-def test_reference_render_uses_only_names_the_drop_in_has(ref):
     import gaussianeditor_b200.rasterizer as RZ
-    # the reference binds the drop-in's classes
-    assert ref.GR.GaussianRasterizer is RZ.GaussianRasterizer
-    assert ref.GR.GaussianRasterizationSettings is RZ.GaussianRasterizationSettings
-    tree = ast.parse(open(os.path.join(REF, "gaussiansplatting/gaussian_renderer/__init__.py")).read())
+    _, api = gold
+    # the reference's renderer imports these names from diff_gaussian_rasterization: they are the drop-in's classes
+    assert {"GaussianRasterizer", "GaussianRasterizationSettings"} <= set(api["renderer_imports"])
+    for name in api["renderer_imports"]:
+        assert getattr(dgr, name) is getattr(RZ, name), name
     # every GaussianRasterizationSettings(...) call: keywords == our NamedTuple fields (order irrelevant, all present)
     fields = set(RZ.GaussianRasterizationSettings._fields)
-    n = 0
-    for c in _calls(tree, lambda f: isinstance(f, ast.Name) and f.id == "GaussianRasterizationSettings"):
-        kws = {k.arg for k in c.keywords}
-        assert not c.args and kws == fields, kws ^ fields
-        n += 1
-    assert n >= 2
+    assert len(api["settings_calls"]) >= 2
+    for c in api["settings_calls"]:
+        assert not c["args"] and set(c["keywords"]) == fields, set(c["keywords"]) ^ fields
     # GaussianRasterizer(raster_settings=...) and the forward call rasterizer(means3D=..., ...)
     assert "raster_settings" in inspect.signature(RZ.GaussianRasterizer.__init__).parameters
     fwd = set(inspect.signature(RZ.GaussianRasterizer.forward).parameters) - {"self"}
-    n = 0
-    for c in _calls(tree, lambda f: isinstance(f, ast.Name) and f.id == "rasterizer"):
-        kws = {k.arg for k in c.keywords}
-        assert kws <= fwd and {"means3D", "means2D", "opacities"} <= kws, kws - fwd
-        n += 1
-    assert n >= 1
+    assert len(api["rasterizer_calls"]) >= 1
+    for kws in api["rasterizer_calls"]:
+        assert set(kws) <= fwd and {"means3D", "means2D", "opacities"} <= set(kws), set(kws) - fwd
     # the reference unpacks exactly three outputs: rendered_image, radii, depth
-    src = open(os.path.join(REF, "gaussiansplatting/gaussian_renderer/__init__.py")).read()
-    assert "rendered_image, radii, depth = rasterizer(" in src
+    assert api["unpacks_image_radii_depth"]
 
 
-def test_reference_scene_model_calls_apply_weights_with_our_slot_order(ref):
+def test_reference_scene_model_calls_apply_weights_with_our_slot_order(gold):
     import gaussianeditor_b200.rasterizer as RZ
-    tree = ast.parse(open(os.path.join(REF, "gaussiansplatting/scene/gaussian_model.py")).read())
-    calls = list(_calls(tree, lambda f: isinstance(f, ast.Attribute) and f.attr == "apply_weights" and
-                        isinstance(f.value, ast.Name) and f.value.id == "rasterizer"))
-    assert len(calls) == 1 and len(calls[0].args) == 10 and not calls[0].keywords
+    from gaussianeditor_b200 import gaussian_renderer as GR
+    _, api = gold
+    assert api["apply_weights_calls"] == [{"args": 10, "keywords": 0}]
     # positional slots of scene/gaussian_model.py:821-832 -> our parameter names
     ours = [p for p in inspect.signature(RZ.GaussianRasterizer.apply_weights).parameters if p != "self"]
     assert ours == ["means3D", "means2D", "opacities", "shs", "weights", "scales", "rotations", "cov3Ds_precomp", "cnt",
                     "image_weights"]
-    # same as the reference package's own signature (DGR/diff_gaussian_rasterization/__init__.py:311-322)
-    dgr_src = open(os.path.join(REF, "gaussiansplatting/submodules/diff-gaussian-rasterization/diff_gaussian_rasterization/"
-                                     "__init__.py")).read()
-    cls = next(n for n in ast.walk(ast.parse(dgr_src)) if isinstance(n, ast.ClassDef) and n.name == "GaussianRasterizer")
-    for fn in (n for n in cls.body if isinstance(n, ast.FunctionDef)):
-        if fn.name.startswith("__"):
-            continue
-        assert hasattr(RZ.GaussianRasterizer, fn.name), fn.name
-        theirs = [a.arg for a in fn.args.args if a.arg != "self"]
-        mine = [p for p in inspect.signature(getattr(RZ.GaussianRasterizer, fn.name)).parameters if p != "self"]
-        assert mine[:len(theirs)] == theirs, (fn.name, mine, theirs)
-    # camera2rasterizer(camera, bg, sh_degree) exists in the reference module the model imports it from
-    assert callable(ref.GR.camera2rasterizer)
+    # same as the reference package's own signatures (DGR/diff_gaussian_rasterization/__init__.py:311-322)
+    assert "apply_weights" in api["rasterizer_methods"]
+    for name, theirs in api["rasterizer_methods"].items():
+        assert hasattr(RZ.GaussianRasterizer, name), name
+        mine = [p for p in inspect.signature(getattr(RZ.GaussianRasterizer, name)).parameters if p != "self"]
+        assert mine[:len(theirs)] == theirs, (name, mine, theirs)
+    # the scene model imports these from the renderer module
+    for name in api["model_imports_from_renderer"]:
+        assert callable(getattr(GR, name)), name
 
 
-def _bare_model(ref, P=13, deg=2, seed=0):
-    """A reference GaussianModel on CPU tensors (its __init__ hard-codes device='cuda': bypassed with __new__)."""
-    g = torch.Generator().manual_seed(seed)
-    m = ref.GM.GaussianModel.__new__(ref.GM.GaussianModel)
-    m.setup_functions()
-    K = (deg + 1) ** 2 - 1
-    r = lambda *s: torch.randn(*s, generator=g)
-    m.active_sh_degree = m.max_sh_degree = deg
-    m._xyz = torch.nn.Parameter(r(P, 3)); m._features_dc = torch.nn.Parameter(r(P, 1, 3))
-    m._features_rest = torch.nn.Parameter(r(P, K, 3)); m._opacity = torch.nn.Parameter(r(P, 1))
-    m._scaling = torch.nn.Parameter(r(P, 3)); m._rotation = torch.nn.Parameter(r(P, 4))
-    groups = [("xyz", m._xyz, 1.6e-4), ("f_dc", m._features_dc, 2.5e-3), ("f_rest", m._features_rest, 1.25e-4),
-              ("opacity", m._opacity, 0.05), ("scaling", m._scaling, 5e-3), ("rotation", m._rotation, 1e-3)]
-    m.optimizer = torch.optim.Adam([{"params": [p], "lr": lr, "name": n} for n, p, lr in groups], lr=0.0, eps=1e-15)
-    for step in range(3):   # build non-trivial Adam state
-        m.optimizer.zero_grad()
-        sum((p * (i + 1 + step)).sum() + (p ** 2).sum() for i, (_, p, _) in enumerate(groups)).backward()
-        m.optimizer.step()
-    return m
-
-
-def _snapshot(opt):
-    out = {}
-    for gr in opt.param_groups:
-        p = gr["params"][0]
-        st = opt.state.get(p, {})
-        out[gr["name"]] = (p.detach().clone(), {k: (v.clone() if torch.is_tensor(v) else v) for k, v in st.items()})
-    return out
-
-
-def _assert_same(a, b):
-    assert a.keys() == b.keys()
-    for name in a:
-        pa, sa = a[name]; pb, sb = b[name]
-        assert torch.equal(pa, pb), name
-        assert sa.keys() == sb.keys(), name
-        for k in sa:
-            if torch.is_tensor(sa[k]):
-                assert torch.equal(sa[k], sb[k]), (name, k)
-            else:
-                assert sa[k] == sb[k], (name, k)
-
-
-def test_optimizer_surgery_equals_the_reference_functions(ref):
+def test_optimizer_surgery_equals_the_reference_functions(gold):
     from gaussianeditor_b200 import optim_surgery as OS
-    g = torch.Generator().manual_seed(5)
-    # prune
-    a, b = _bare_model(ref), _bare_model(ref)
-    keep = torch.rand(13, generator=g) > 0.4
-    ra = a._prune_optimizer(keep)
-    rb = OS.prune_optimizer(b.optimizer, keep)
-    _assert_same(_snapshot(a.optimizer), _snapshot(b.optimizer))
-    assert all(torch.equal(ra[k], rb[k]) and isinstance(rb[k], torch.nn.Parameter) and rb[k].requires_grad for k in ra)
-    # cat (densification_postfix's dictionary, :643-660)
-    ext = {"xyz": torch.randn(4, 3, generator=g), "f_dc": torch.randn(4, 1, 3, generator=g),
-           "f_rest": torch.randn(4, 8, 3, generator=g), "opacity": torch.randn(4, 1, generator=g),
-           "scaling": torch.randn(4, 3, generator=g), "rotation": torch.randn(4, 4, generator=g)}
-    ra = a.cat_tensors_to_optimizer({k: v.clone() for k, v in ext.items()})
-    rb = OS.cat_tensors_to_optimizer(b.optimizer, {k: v.clone() for k, v in ext.items()})
-    _assert_same(_snapshot(a.optimizer), _snapshot(b.optimizer))
-    assert all(torch.equal(ra[k], rb[k]) for k in ra)
-    # replace (reset_opacity path)
-    new_op = torch.randn(a.optimizer.param_groups[3]["params"][0].shape, generator=g)
-    ra = a.replace_tensor_to_optimizer(new_op.clone(), "opacity")
-    rb = OS.replace_tensor_to_optimizer(b.optimizer, new_op.clone(), "opacity")
-    _assert_same(_snapshot(a.optimizer), _snapshot(b.optimizer))
-    assert ra.keys() == rb.keys() == {"opacity"}
-    # and the optimizers keep stepping identically afterwards
-    for m in (a, b):
-        m.optimizer.zero_grad()
-        sum((gr["params"][0] ** 2).sum() for gr in m.optimizer.param_groups).backward()
-        m.optimizer.step()
-    _assert_same(_snapshot(a.optimizer), _snapshot(b.optimizer))
+    z, _ = gold
+    g, keep, ext = surgery_inputs()
+    _, opt = bare_model()
+    r = OS.prune_optimizer(opt, keep)
+    assert all(isinstance(v, torch.nn.Parameter) and v.requires_grad for v in r.values())
+    got = returned(r, "prune")
+    got.update(snapshot(opt, "prune"))
+    _assert_recorded(z, got, "prune")
+    got = returned(OS.cat_tensors_to_optimizer(opt, {k: v.clone() for k, v in ext.items()}), "cat")   # :643-660
+    got.update(snapshot(opt, "cat"))
+    _assert_recorded(z, got, "cat")
+    new_op = _normal(g, *opt.param_groups[3]["params"][0].shape)
+    r = OS.replace_tensor_to_optimizer(opt, new_op.clone(), "opacity")                                 # reset_opacity
+    assert r.keys() == {"opacity"}
+    got = returned(r, "replace")
+    got.update(snapshot(opt, "replace"))
+    _assert_recorded(z, got, "replace")
+    # and the optimizer keeps stepping like the reference's afterwards: one step of ours next to one step of an Adam
+    # holding the reference's recorded state, in this process
+    theirs = adam_from(z, "replace")
+    adam_step(opt)
+    adam_step(theirs)
+    mine, want = snapshot(opt, "step"), snapshot(theirs, "step")
+    assert sorted(mine) == sorted(want)
+    for k in want:
+        assert np.array_equal(mine[k], want[k]), k
 
 
-@pytest.mark.parametrize("deg", [0, 1, 3])
-def test_ply_bytes_equal_what_the_reference_writer_hands_to_plyfile(ref, tmp_path, deg):
+@pytest.mark.parametrize("deg", PLY_DEGREES)
+def test_ply_bytes_equal_what_the_reference_writer_hands_to_plyfile(gold, tmp_path, deg):
     from gaussianeditor_b200 import ply_io
-    m = _bare_model(ref, P=11, deg=deg, seed=deg)
-    ref_path = str(tmp_path / "ref" / "point_cloud.ply")
-    m.save_ply(ref_path)                                   # the REFERENCE's code builds the vertex table
-    path, elements = ref.ply.PlyData.last_written
-    assert path == ref_path and len(elements) == 1 and elements[0].name == "vertex"
-    table = elements[0].data                               # numpy structured array, fields in the reference's order
-    assert all(table.dtype[n] == np.dtype("<f4") for n in table.dtype.names) and table.dtype.itemsize == 4 * len(table.dtype.names)
+    z, api = gold
+    names = api["ply_fields"][str(deg)]
+    table = z[f"ply/{deg}"]                                # the REFERENCE's vertex table, fields in its order
+    assert table.shape[1] == len(names)
+    p, _ = bare_model(P=11, deg=deg, seed=deg)
     ours = str(tmp_path / "ours.ply")
-    ply_io.write_gaussian_ply(ours, xyz=m._xyz.detach().numpy(), features_dc=m._features_dc.detach().numpy(),
-                              features_rest=m._features_rest.detach().numpy(), opacity=m._opacity.detach().numpy(),
-                              scaling=m._scaling.detach().numpy(), rotation=m._rotation.detach().numpy())
+    ply_io.write_gaussian_ply(ours, xyz=p["xyz"].detach().numpy(), features_dc=p["f_dc"].detach().numpy(),
+                              features_rest=p["f_rest"].detach().numpy(), opacity=p["opacity"].detach().numpy(),
+                              scaling=p["scaling"].detach().numpy(), rotation=p["rotation"].detach().numpy())
     raw = open(ours, "rb").read()
     header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % len(table) +
-              "".join(f"property float {n}\n" for n in table.dtype.names) + "end_header\n").encode()   # plyfile's header
+              "".join(f"property float {n}\n" for n in names) + "end_header\n").encode()   # plyfile's header
     assert raw[:len(header)] == header
-    assert raw[len(header):] == table.tobytes()            # body: bit for bit the reference's table
-    # the reference's load_ply (:447-501) on top of our reader reconstructs the same tensors (its .cuda() calls are
-    # redirected to CPU for the duration of the call)
-    m2 = ref.GM.GaussianModel.__new__(ref.GM.GaussianModel)
-    m2.setup_functions()
-    m2.max_sh_degree = deg
-    names = ["tensor", "zeros", "ones", "empty", "full"]
-    orig = {n: getattr(torch, n) for n in names}
-
-    def on_cpu(fn):
-        return lambda *a, **k: fn(*a, **({**k, "device": "cpu"} if k.get("device") == "cuda" else k))
-    try:
-        for n in names:
-            setattr(torch, n, on_cpu(orig[n]))
-        m2.load_ply(ours)
-    finally:
-        for n in names:
-            setattr(torch, n, orig[n])
-    for name in ("_xyz", "_features_dc", "_features_rest", "_opacity", "_scaling", "_rotation"):
-        assert torch.equal(getattr(m2, name).detach(), getattr(m, name).detach()), name
+    assert raw[len(header):] == np.ascontiguousarray(table, "<f4").tobytes()   # body: bit for bit the reference's table
+    # what the reference's load_ply (:447-501) reads by name comes back from our reader unchanged
+    cols = ply_io.read_vertex_table(ours)
+    assert list(cols) == names
+    for i, n in enumerate(names):
+        assert np.array_equal(np.asarray(cols[n], np.float32).ravel(), table[:, i]), n

@@ -351,7 +351,7 @@ def test_sparse_exchange_virtual_ranks_match_single_gpu(world, cap_mode):
 @pytest.mark.parametrize("variant", ["dense-nccl", "dense-p2p", "sparse"])
 def test_two_process_nccl_matches_single_gpu(variant):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     extra = {"dense-nccl": [], "dense-p2p": ["--p2p"], "sparse": ["--mode", "sparse"]}[variant]
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
            "--master-port", str(_free_port()), os.path.join(ROOT, "tools", "sharded_check.py"), "--config", "c3",

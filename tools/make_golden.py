@@ -1,8 +1,15 @@
 """Generate the committed golden vectors under tests/golden/ by running the REFERENCE's own CUDA build
 (oracle/_ref/libdgr_ref.so = the unmodified reference .cu files, see oracle/Makefile) on small seeded scenes.
-Must run on a GPU box:   gpurun -- python tools/make_golden.py   (writes gpurun_out/golden/*.npz; copy them to
+Needs a GPU and the built oracle/_ref:   python tools/make_golden.py OUT_DIR   (writes OUT_DIR/*.npz; copy them to
 tests/golden/ and commit).  The reference has no tests or fixtures of its own (SURVEY.md section 4); these files
-are what pins the CPU oracle and our kernels to the reference's actual outputs when no GPU reference is at hand."""
+are what pins the CPU oracle and our kernels to the reference's actual outputs when no GPU reference is at hand:
+  * <case>.npz                    inputs and full reference outputs of three tiny scenes (tests/test_golden.py);
+  * small_cases_reference.npz     (goes to tests/golden/parity/) for test_parity_gpu's small cases: SHA-256 digests of every forward output and a
+                                  seeded sample of every gradient with its noise floor and max |value|;
+  * reference_outputs.npz         (goes to tests/golden/parity/) every other reference value test_parity_gpu compares
+                                  with: the tests that use test_parity_gpu._Ref are run here against the live reference
+                                  (their assertions included) and what they computed from it is recorded.
+"""
 import os
 import sys
 
@@ -16,8 +23,9 @@ import torch
 from gaussianeditor_b200 import synth
 import test_parity_gpu as T
 
-OUT = os.path.join(ROOT, "gpurun_out", "golden")
+OUT = sys.argv[1]
 os.makedirs(OUT, exist_ok=True)
+assert T.ref_cuda.available(), "oracle/_ref/libdgr_ref.so is not built"
 
 
 def case(name, cloud, cam, bg, colors_precomp=None, scale_modifier=1.0, seed=0):
@@ -54,4 +62,37 @@ c2, _ = synth.make_config("c2", P=300)
 cp = np.random.default_rng(5).uniform(size=(300, 3)).astype(np.float32)
 case("c2_p300_colors_mod07", c2, synth.look_at_camera((0, 0, -3.5), (0, 0, 0), (0, -1, 0), 50, 35, fovy_deg=50.0),
      (1, 1, 1), colors_precomp=cp, scale_modifier=0.7, seed=3)
+small = {}
+for name, cloud, cam, bg in T._small_cases():
+    dL = T._small_case_dL(cam)
+    ref = T._ref_run(cloud, cam, bg, dL=dL)
+    ref2 = T._ref_run(cloud, cam, bg, dL=dL)
+    for k, x in T._ref_forward_fields(ref).items():
+        small[f"{name}/fwd/{k}"] = np.array(T._digest(x))
+    for _, b in T.GRAD_PAIRS:
+        r = ref["grads"][b].cpu().numpy().ravel()
+        small[f"{name}/bwd/{b}"] = r[T._sample_index(r.size)]
+        small[f"{name}/bwd/{b}/noise"] = np.float64(T.rel_l2(ref2["grads"][b].cpu().numpy().ravel(), r))
+        small[f"{name}/bwd/{b}/absmax"] = np.float64(np.abs(r).max())
+np.savez_compressed(os.path.join(OUT, "small_cases_reference.npz"), **small)
+
+
+def parametrizations(fn):
+    marks = [m for m in getattr(fn, "pytestmark", []) if m.name == "parametrize"]
+    if not marks:
+        return [()]
+    return [v if isinstance(v, tuple) else (v,) for v in marks[0].args[1]]
+
+
+T.RECORD = {}
+for fn in (T.test_precomputed_colors_and_scale_modifier, T.test_mark_visible_and_apply_weights_match_reference,
+           T.test_apply_weights_channels_and_float_masks,
+           T.test_alpha_output_matches_reference_accum_alpha_and_is_differentiable,
+           T.test_binning_variants_match_reference_lists, T.test_edit_loop_matches_the_reference_rasterizer_step_by_step,
+           T.test_sh_degrees_and_coefficient_counts, T.test_precomputed_covariance_path,
+           T.test_hd_frame_partial_tile_row_and_debug_flag, T.test_full_size_configs_match_reference_cuda):
+    for args in parametrizations(fn):
+        fn(*args)
+        print("recorded", fn.__name__, args)
+np.savez_compressed(os.path.join(OUT, "reference_outputs.npz"), **T.RECORD)
 print("golden written to", OUT)

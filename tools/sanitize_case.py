@@ -88,7 +88,7 @@ rs_cam = rs._replace(viewmatrix=view, projmatrix=rs.projmatrix.clone().requires_
                      campos=rs.campos.clone().requires_grad_(True))
 # camera gradients + alpha output. initcheck does not track TMA bulk stores (cp.async.bulk shared->global) as writes, so a
 # cudaMemcpy of the dL/dSH tensor they fill (autograd's copy into .grad) is reported as "uninitialized" byte for byte
-# (18006 reports = 576192 B / 32 in profiles/r02_sanitizer.txt). The TMA variant therefore runs with SH detached
+# (one report per 32 bytes of the tensor). The TMA variant therefore runs with SH detached
 # (kernel identical, autograd drops the tensor without a copy) and the plain-store variant runs with SH attached.
 for pv, sh_grad in ((1, False), (0, True)):
     _lib.set_option("preprocess_variant", pv)
