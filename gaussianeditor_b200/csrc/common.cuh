@@ -96,7 +96,7 @@ constexpr int ACC_STRIDE = 12;
 // ---- options -----------------------------------------------------------------------------------------
 struct Options {
   int render_fwd_variant = 3;  // 0 CTA/tile, 1/2/3 = 1/2/4 warps per tile
-  int render_bwd_variant = 14;  // 0 CTA/tile, 1/2/3 branchy, 4..9 branch-light, 10/11 mask-skip, 12..14 register caps (14: 96 regs + hit-skip)
+  int render_bwd_variant = 15;  // 0 CTA/tile, 1/2/3 branchy, 4..9 branch-light, 10/11 mask-skip, 12..14 register caps (14: 96 regs + hit-skip), 15: 14 + the moment reduction batched through shared memory
   int preprocess_variant = 1;
   int profile = 0;
   int tile_key_bits = 16;

@@ -10,13 +10,15 @@
 // from its very end.  Here:
 //   * the walk starts at tile_last = max n_contrib of the tile (written by the forward): on a saturated scene
 //     three quarters of every list lie behind the last contributor of all 256 pixels and are never loaded;
-//   * warp variants (1/2/3 branchy, 4..9 branch-light, 10/11 skip by sub-block mask, 12..14 register caps; DEFAULT 14 =
+//   * warp variants (1/2/3 branchy, 4..9 branch-light, 10/11 skip by sub-block mask, 12..14 register caps; 14 =
 //     one warp per half tile, 96 registers -> 5 CTAs/SM, updates of sub-blocks without a hit skipped warp-uniformly:
 //     0.627 ms at config 3 on an H100 80GB HBM3; the A/B of all of them is in DESIGN.md section 3): a
 //     warp owns a whole tile, half or a quarter of it, each lane owns one pixel of each of its
 //     8x4 sub-blocks; the nine partial sums are first accumulated over the lane's own pixels in registers,
 //     then summed across the warp with a transposing butterfly (16 shuffles for 9 values instead of 45), and
 //     only then added to global memory: 9 atomics per (tile, splat) instead of 9 per (pixel, splat);
+//   * DEFAULT 15 = variant 14 with that warp reduction deferred: the moments of 4 splats are summed at once through
+//     shared memory (flush_moments), 0.553 instead of 0.646 ms at config 3 on an H100 80GB HBM3 at a 400 W power limit;
 //   * the same opacity-aware sub-block culling as the forward (render_fwd.cu) removes splats whose
 //     alpha>=1/255 ellipse misses the sub-block before any pixel looks at them.
 // Variant 0: the reference's CTA-per-tile structure with a plain warp-shuffle reduction before the atomics.
@@ -309,8 +311,78 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false>
+// ------------------------------------------------------------------------------------------------------
+// Variant 15: variant 14 with the per-splat warp reduction deferred and batched through shared memory.
+// Every staged splat with a hit costs variant 14 a warp_sum9 + finish_and_add (~90 instructions: 15 SHFL, the FSEL of
+// the transposing butterfly, two REDG behind divergent writer branches) in its critical path. Here each lane instead
+// stores its nine moments as one column of a per-warp buffer  part[slot][moment][lane]  (9 STS.32), and every
+// BATCH_NB splats the warp sums the 9*BATCH_NB rows at once: lane l owns the row (slot l>>3, moment l&7) and sums its
+// 32 entries with 8 LDS.128 + 31 FADD; the BATCH_NB moment-8 rows (sum w) are split over the 8 lanes of a slot
+// (1 LDS.128 + 3 FADD each) and completed with a 3-level butterfly. The row owners then issue the nine atomics of a
+// slot (moments 0..7 from 8 lanes, opacity from the first of them) into one 48-byte acc row: 2 REDG per batch.
+// A slot records the stage index j of its splat (5 bits of the warp-uniform register jpack, behind a leading 1 that
+// also counts the slots), so the batch is also flushed before the stage is refilled.
+// Banks (4-byte words, 32 banks). A row is 32 words plus 4 of padding (BATCH_ROW = 36), so row r starts on bank 4r mod 32:
+//   * column write of moment i by lane l: word (slot*9 + i)*36 + l -> bank (4*(slot*9 + i) + l) mod 32, a different
+//     bank for each of the 32 lanes: conflict-free;
+//   * row read: an LDS.128 is served per quarter warp (8 lanes, 128 bytes). At step k lane l reads chunk k of row
+//     slot*9 + (l&7) = banks 4*(slot*9 + (l&7) + k) mod 32 .. +3; the 8 lanes of a quarter warp share the slot and have
+//     distinct l&7, so distinct bank quads. The padding is what lets every lane read its chunks at the same immediate
+//     offsets (no per-load address arithmetic);
+//   * moment-8 read: the 8 lanes of a quarter warp are the 8 lanes of one slot and read chunks 0..7 of its row.
+// Static SASS (nvcc 12.9, sm_90a): the per-splat loop is 388 instructions against 362 for variant 14, but 110 of them
+// are the flush, run once per 4 splats, and 42 the rare expf re-check. A splat with hits in all four sub-blocks costs
+// 236 + 110/4 = 264 instead of ~320: 14 for the write (9 STS) and 28 for its share of the flush, against ~90 for the
+// warp reduction. 96 registers, 0 spills, 27392 B of shared memory per CTA (5 CTAs/SM).
+// Gradients differ from variant 14 only in the order of the fp32 sums.
+// ------------------------------------------------------------------------------------------------------
+constexpr int BATCH_NB = 4;    // slots per flush (8 slots, 43 KB per CTA, measured no faster)
+constexpr int BATCH_ROW = 36;  // floats per row: 32 lanes + 4 of padding; 4 * 9 * 36 * 4 B = 5 KB per warp
+
+// Sums the nslot filled slots (warp-uniform; all lanes call it) and adds them to acc. The slots refer to the stage:
+// call it before the stage is refilled.
+__device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpack, int nslot, const float4 (*stg)[32],
+                                              const uint32_t* sid, float* acc, int lane, float ddelx_dx,
+                                              float ddely_dy) {
+  const unsigned F = 0xffffffffu;
+  const int s = lane >> 3, m = lane & 7;  // this lane's slot and moment row
+  const float4* row = part4 + (s * 9 + m) * (BATCH_ROW / 4);
+  float4 t = row[0];
+#pragma unroll
+  for (int k = 1; k < 8; k++) {
+    const float4 v = row[k];
+    t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
+  }
+  const float tot = (t.x + t.y) + (t.z + t.w);
+  const float4 v8 = part4[(s * 9 + 8) * (BATCH_ROW / 4) + m];  // chunk m of the slot's moment-8 row
+  float sw = (v8.x + v8.y) + (v8.z + v8.w);
+  sw += __shfl_xor_sync(F, sw, 1);
+  sw += __shfl_xor_sync(F, sw, 2);
+  sw += __shfl_xor_sync(F, sw, 4);
+  const float other = __shfl_xor_sync(F, tot, 7);  // s_x <-> s_y between moments 3 and 4
+  if (s < nslot) {
+    const int j = (jpack >> (5 * (nslot - 1 - s))) & 31u;
+    const float4 s0 = stg[0][j];  // x, y, A, B
+    const float4 s1 = stg[1][j];  // C, o
+    float* dst = acc + (size_t)sid[j] * ACC_STRIDE;
+    // as finish_and_add: m<3 tot | 3: -(A*s_x + B*s_y)*0.5W | 4: -(C*s_y + B*s_x)*0.5H | 5..7: -0.5*tot | opacity sw / o
+    const bool is_x = m == 3, is_y = m == 4;
+    const float nAx = -s0.z * ddelx_dx, nCy = -s1.x * ddely_dy, nBx = -s0.w * ddelx_dx, nBy = -s0.w * ddely_dy;
+    const float ka = is_x ? nAx : (is_y ? nCy : (m < 3 ? 1.0f : -0.5f));
+    const float kb = is_x ? nBx : (is_y ? nBy : 0.0f);
+    atomicAdd(dst + m, fmaf(kb, other, ka * tot));
+    if (m == 0) {
+      float rcp;  // o >= 1/255 for every staged splat (splat_subblock_mask): __fdividef(sw, o) without its denormal guard
+      asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(s1.y));
+      atomicAdd(dst + 8, sw * rcp);
+    }
+  }
+}
+
+// BATCHED (variant 15): the per-splat reduction is deferred and batched through shared memory (flush_moments)
+template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false>
 __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgs a, const int ntiles) {
+  static_assert(!BATCHED || (NSB == 4 && SKIP && !MASKSKIP), "the batched reduction is written for variant 15");
   __shared__ float4 s_stage[BW_WARPS][3][32];
   __shared__ uint32_t s_id[BW_WARPS][32];
   constexpr int PARTS = 8 / NSB;
@@ -321,6 +393,14 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
   const int tile = owned_tile(gw / PARTS, a.gx, a.own_stride, a.own_phase);  // ntiles counts the OWNED tiles
   float4(*stg)[32] = s_stage[warp];
   uint32_t* sid = s_id[warp];
+  float4* bpart = nullptr;  // BATCHED: part[slot][moment][BATCH_ROW] of this warp
+  if constexpr (BATCHED) {
+    __shared__ float4 s_part[BW_WARPS][BATCH_NB * 9 * (BATCH_ROW / 4)];
+    bpart = s_part[warp];
+  }
+  // BATCHED: a 1 followed by the stage index j (< 32) of each filled slot in 5 bits, the latest slot lowest; warp-uniform
+  uint32_t jpack = 1;
+  float* col = reinterpret_cast<float*>(bpart) + lane;  // BATCHED: this lane's column in the next free slot
 
   const int tx = tile % a.gx, ty = tile / a.gx;
   const int lx = lane & 7, ly = lane >> 3;
@@ -452,9 +532,31 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
         if (MASKSKIP && !((m >> k) & 1u)) continue;
         hit_update(ps[k], g, dxv[k & 1], dyv[k >> 1], G[k], al[k], s1.y, s2.x, s2.y, s2.z);
       }
-      float m8;
-      const float tot = warp_sum9(g, lane, m8);
-      finish_and_add(a.acc + (size_t)sid[j] * ACC_STRIDE, tot, m8, role, s0.z, s0.w, s1.x, s1.y, ddelx_dx, ddely_dy);
+      if constexpr (!BATCHED) {
+        float m8;
+        const float tot = warp_sum9(g, lane, m8);
+        finish_and_add(a.acc + (size_t)sid[j] * ACC_STRIDE, tot, m8, role, s0.z, s0.w, s1.x, s1.y, ddelx_dx, ddely_dy);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 9; i++) col[BATCH_ROW * i] = g[i];
+        col += 9 * BATCH_ROW;
+        jpack = (jpack << 5) | (uint32_t)j;
+        if (jpack >= 1u << (5 * BATCH_NB)) {  // all slots filled
+          __syncwarp();
+          flush_moments(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
+          __syncwarp();  // the next splat overwrites slot 0
+          jpack = 1;
+          col -= BATCH_NB * 9 * BATCH_ROW;
+        }
+      }
+    }
+    if constexpr (BATCHED) {
+      if (jpack > 1) {  // before the stage is refilled
+        __syncwarp();
+        flush_moments(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
+        col = reinterpret_cast<float*>(bpart) + lane;
+        jpack = 1;
+      }
     }
     __syncwarp();
   }
@@ -570,6 +672,8 @@ int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningW
     render_bwd_flat_kernel<4, 6, true><<<(ntiles * 2 + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(a, ntiles);
   } else if (v == 14) {
     render_bwd_flat_kernel<4, 5, true><<<(ntiles * 2 + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(a, ntiles);
+  } else if (v == 15) {  // variant 14 with the per-splat reduction batched through shared memory
+    render_bwd_flat_kernel<4, 5, true, false, true><<<(ntiles * 2 + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(a, ntiles);
   } else if (v == 10) {  // variant 4 + sub-blocks outside the splat's mask skipped with warp-uniform branches
     render_bwd_flat_kernel<4, 1, false, true><<<(ntiles * 2 + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(a, ntiles);
   } else if (v == 11) {  // the same for the quarter-tile mapping

@@ -16,7 +16,7 @@ import bench  # noqa: E402
 from gaussianeditor_b200 import _lib  # noqa: E402
 
 SWEEP = {"render_fwd_variant": ([0, 1, 2, 3, 4, 5], ["render_fwd"]),
-         "render_bwd_variant": (list(range(15)), ["render_bwd"]),
+         "render_bwd_variant": (list(range(16)), ["render_bwd"]),
          "preprocess_variant": ([0, 1], ["preprocess_fwd", "preprocess_bwd"]),
          "binning_variant": ([0, 1], ["emit_instances", "tile_sort", "tile_ranges"]),
          "depth_sort_variant": ([0, 1], ["depth_order_scan"])}
