@@ -91,6 +91,7 @@ void carve_image(void* base, int W, int H, ImageWS& ws);
 
 // Backward scratch: per-Gaussian accumulators of the nine 2-D gradients (+3 pad -> 48 B, 16-B aligned):
 //   [0..2] dL/dcolor  [3..4] dL/dmean2D  [5..7] dL/dconic (a,b,c)  [8] dL/dopacity
+//   [9] dL/dz (view depth) when the depth image has an upstream gradient, else 0; [10..11] padding
 constexpr int ACC_STRIDE = 12;
 
 // ---- options -----------------------------------------------------------------------------------------
@@ -160,9 +161,10 @@ int clear_tile_counts(const GeometryWS& g, int gx, int gy, cudaStream_t st);
 int launch_tile_count(const GeometryWS& g, int gx, int gy, const TileOwner& own, cudaStream_t st);
 int launch_render_fwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       float* out_color, float* out_depth, cudaStream_t st, const TileOwner& own = TileOwner());
+// dL_ddepth != nullptr: also the depth image's upstream [H*W]; dL/dz of each splat goes to acc slot 9 (variant 15 only)
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own = TileOwner(),
-                      const float* dL_dalpha_img = nullptr);
+                      const float* dL_dalpha_img = nullptr, const float* dL_ddepth = nullptr);
 // raw != nullptr: RAW variant -- gradients w.r.t. the raw parameters (gr.dL_dsh = d features_dc, raw->dL_dfeatures_rest)
 struct RawBackward {
   const float* features_rest;
@@ -176,9 +178,10 @@ struct CameraBackward {
   float* scratch;
 };
 size_t camera_scratch_bytes(int P);
+// depth: acc slot 9 holds dL/dz (launch_render_bwd with dL_ddepth) and enters the mean (and view-matrix) gradient
 int launch_preprocess_bwd(const gsr_settings& s, const gsr_cloud& c, const GeometryWS& g, const int32_t* radii,
                           const float* acc, const gsr_grads& gr, cudaStream_t st, const RawBackward* raw = nullptr,
-                          const CameraBackward* cam = nullptr);
+                          const CameraBackward* cam = nullptr, bool depth = false);
 // out_alpha[i] = 1 - final_T[i]  (the reference keeps final_T as ImageState::accum_alpha, rasterizer_impl.h:50)
 int launch_alpha_image(const float* final_T, size_t n, float* out_alpha, cudaStream_t st);
 int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t st);

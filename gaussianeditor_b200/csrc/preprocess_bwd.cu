@@ -91,7 +91,9 @@ __device__ __forceinline__ M3 quat_to_R(float r, float x, float y, float z) {
 //   [24 + c]      dL/dcampos[c]
 constexpr int CAM_N = 27, CAM_STRIDE = 32;
 
-template <bool BULK, bool RAW = false, bool CAM = false>
+// DEPTH: the accumulators carry dL/dz in slot 9 (acc2.y; the depth image's gradient, render_bwd.cu). z = t.z is the view
+// depth the forward blends, not clamped, so dL/dt.z gains it, and with it the mean and, under CAM, view row 2.
+template <bool BULK, bool RAW = false, bool CAM = false, bool DEPTH = false>
 __global__ void __launch_bounds__(PB_THREADS) preprocess_bwd_kernel(const PbArgs a) {
   static_assert(!(BULK && RAW), "the RAW variant stages its SH block itself");
   float cg[CAM ? CAM_N : 1];
@@ -153,7 +155,7 @@ __global__ void __launch_bounds__(PB_THREADS) preprocess_bwd_kernel(const PbArgs
     const float4* ap = reinterpret_cast<const float4*>(a.acc + (size_t)idx * ACC_STRIDE);
     acc0 = __ldg(ap);      // dcolor.rgb, dmean2D.x
     acc1 = __ldg(ap + 1);  // dmean2D.y, dconic.a, dconic.b, dconic.c
-    acc2 = __ldg(ap + 2);  // dopacity
+    acc2 = __ldg(ap + 2);  // dopacity, dL/dz (DEPTH)
     mean = make_float3(a.means3D[3 * idx], a.means3D[3 * idx + 1], a.means3D[3 * idx + 2]);
 
     // ---- 3-D covariance (recomputed; forward.cu:118-152) ----
@@ -249,8 +251,9 @@ __global__ void __launch_bounds__(PB_THREADS) preprocess_bwd_kernel(const PbArgs
       const float tz = 1.f / t.z, tz2 = tz * tz, tz3 = tz2 * tz;
       const float dL_dtx = x_grad_mul * -a.h_x * tz2 * dL_dJ02;
       const float dL_dty = y_grad_mul * -a.h_y * tz2 * dL_dJ12;
-      const float dL_dtz = -a.h_x * tz2 * dL_dJ00 - a.h_y * tz2 * dL_dJ11 + (2 * a.h_x * t.x) * tz3 * dL_dJ02 +
-                           (2 * a.h_y * t.y) * tz3 * dL_dJ12;
+      float dL_dtz = -a.h_x * tz2 * dL_dJ00 - a.h_y * tz2 * dL_dJ11 + (2 * a.h_x * t.x) * tz3 * dL_dJ02 +
+                     (2 * a.h_y * t.y) * tz3 * dL_dJ12;
+      if constexpr (DEPTH) dL_dtz += acc2.y;  // dL/dz of the depth image
       // transformVec4x3Transpose (auxiliary.h:89-97)
       dmean[0] = vm[0] * dL_dtx + vm[1] * dL_dty + vm[2] * dL_dtz;
       dmean[1] = vm[4] * dL_dtx + vm[5] * dL_dty + vm[6] * dL_dtz;
@@ -545,7 +548,7 @@ size_t camera_scratch_bytes(int P) { return align_up((size_t)((P + PB_THREADS - 
 
 int launch_preprocess_bwd(const gsr_settings& s, const gsr_cloud& c, const GeometryWS& g, const int32_t* radii,
                           const float* acc, const gsr_grads& gr, cudaStream_t st, const RawBackward* raw,
-                          const CameraBackward* cam) {
+                          const CameraBackward* cam, bool depth) {
   PbArgs a;
   a.cam_partial = cam ? cam->scratch : nullptr;
   a.opacities = c.opacities;
@@ -568,20 +571,34 @@ int launch_preprocess_bwd(const gsr_settings& s, const gsr_cloud& c, const Geome
                     (reinterpret_cast<uintptr_t>(c.shs) % 16) == 0 && (reinterpret_cast<uintptr_t>(gr.dL_dsh) % 16) == 0;
   if (cam) {  // opt-in camera gradients (never together with the RAW entry point)
     if (raw) { set_error("camera gradients are not available on the fused-activation entry point"); return GSR_ERR_INVALID; }
-    if (bulk)
+    if (depth) {
+      if (bulk)
+        preprocess_bwd_kernel<true, false, true, true><<<grid, PB_THREADS, 0, st>>>(a);
+      else
+        preprocess_bwd_kernel<false, false, true, true><<<grid, PB_THREADS, 0, st>>>(a);
+    } else if (bulk) {
       preprocess_bwd_kernel<true, false, true><<<grid, PB_THREADS, 0, st>>>(a);
-    else
+    } else {
       preprocess_bwd_kernel<false, false, true><<<grid, PB_THREADS, 0, st>>>(a);
+    }
     camera_reduce_kernel<<<1, 1024, 0, st>>>(cam->scratch, grid, cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos);
     g_launches += 2;
     return check_launch("preprocess_bwd (camera)", s.debug != 0, st);
   }
-  if (raw)
+  if (depth) {
+    if (raw)
+      preprocess_bwd_kernel<false, true, false, true><<<grid, PB_THREADS, 0, st>>>(a);
+    else if (bulk)
+      preprocess_bwd_kernel<true, false, false, true><<<grid, PB_THREADS, 0, st>>>(a);
+    else
+      preprocess_bwd_kernel<false, false, false, true><<<grid, PB_THREADS, 0, st>>>(a);
+  } else if (raw) {
     preprocess_bwd_kernel<false, true><<<grid, PB_THREADS, 0, st>>>(a);
-  else if (bulk)
+  } else if (bulk) {
     preprocess_bwd_kernel<true><<<grid, PB_THREADS, 0, st>>>(a);
-  else
+  } else {
     preprocess_bwd_kernel<false><<<grid, PB_THREADS, 0, st>>>(a);
+  }
   g_launches++;
   return check_launch("preprocess_bwd", s.debug != 0, st);
 }

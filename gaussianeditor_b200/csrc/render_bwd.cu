@@ -25,6 +25,8 @@
 //
 // Gradients are sums of floats in a different order than the reference's atomics (which are themselves
 // non-deterministic), so parity is to tolerance (tests: rel L2 <= 1e-4), not bit-exact.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace gsr {
@@ -45,6 +47,12 @@ struct BwdArgs {
   float* acc;  // [P, ACC_STRIDE]
   int own_stride, own_phase;  // tile-row ownership (1, 0 = all tiles)
 };
+// Arguments of the depth instantiation: a separate type, so that the parameter block of every other kernel keeps its
+// size and layout (and those kernels their code).
+struct BwdDepthArgs : BwdArgs {
+  const float* dL_ddepth;  // [H*W] gradient of the depth image (gsr_backward_depth)
+};
+template <bool DEPTH> using BwdArgsT = std::conditional_t<DEPTH, BwdDepthArgs, BwdArgs>;
 
 // One (pixel, splat) hit. `ar` tracks the reference's accum_rec (backward.cu:515) dotted with dL_dpixel, updated
 // eagerly; `bgT` = T_final * (bg . dL_dpixel).
@@ -54,8 +62,12 @@ struct BwdArgs {
 // and turned into the reference's quantities once per (tile, splat) by finish_sums() -- the per-splat factors
 // (conic, opacity, 0.5*W, 0.5*H) are constant over the pixels, so this is the same sum with the common factor
 // pulled out (8 instead of 17 operations per hit).
+//
+// The depth image D = sum z*alpha*T (no background term) is a fourth channel with colour z, so with a depth upstream
+// dD = dL/dD the DEPTH kernels add z*dD to that dot product and keep a tenth moment g[9] = sum alpha*T*dD = dL/dz.
 struct PixState {
   float T, ar, d0, d1, d2, bgT;   // ar = accum_rec . dL_dpixel (scalar; see hit_update)
+  float dD;                       // DEPTH only: dL/dD of the pixel
 };
 
 // What multiplies dT_final/dalpha_i = -T_final/(1-alpha_i) in dL/dalpha_i: the background term of the colour
@@ -66,8 +78,9 @@ __device__ __forceinline__ float bg_term(const BwdArgs& a, size_t pix_id, float 
   return t;
 }
 
+template <bool DEPTH = false>
 __device__ __forceinline__ void hit_update(PixState& p, float* g, float dx, float dy, float G, float alpha, float o,
-                                           float c0, float c1, float c2) {
+                                           float c0, float c1, float c2, float z = 0.f) {
   const float oma = 1.f - alpha;
   float rcp;  // 1-alpha is in [0.01, 1]: the bare MUFU.RCP (<= 1 ulp here) needs no range fix-up
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(oma));
@@ -78,11 +91,13 @@ __device__ __forceinline__ void hit_update(PixState& p, float* g, float dx, floa
   // sum_ch (c_ch - accum_rec_ch) * dL_dpixel_ch. Only that dot product is ever used, and the recurrence
   // accum_rec' = alpha*c + (1-alpha)*accum_rec is linear, so the scalar ar = accum_rec . dL_dpixel obeys
   // ar' = ar + alpha*(c.dL_dpixel - ar): one state variable and 5 operations instead of three and 9.
-  const float s = fmaf(c2, p.d2, fmaf(c1, p.d1, c0 * p.d0));
+  float s = fmaf(c2, p.d2, fmaf(c1, p.d1, c0 * p.d0));
+  if constexpr (DEPTH) s = fmaf(z, p.dD, s);  // the depth channel: colour z, upstream dL/dD
   float dL_dalpha = s - p.ar;
   g[0] = fmaf(dchannel_dcolor, p.d0, g[0]);
   g[1] = fmaf(dchannel_dcolor, p.d1, g[1]);
   g[2] = fmaf(dchannel_dcolor, p.d2, g[2]);
+  if constexpr (DEPTH) g[9] = fmaf(dchannel_dcolor, p.dD, g[9]);
   p.ar = fmaf(alpha, dL_dalpha, p.ar);
   dL_dalpha = fmaf(dL_dalpha, p.T, -p.bgT * rcp);
   const float w = (o * dL_dalpha) * G;  // dL_dG * G
@@ -336,17 +351,23 @@ __device__ __forceinline__ float ex2_approx(float x) {
 // warp reduction. 96 registers, 0 spills, 27392 B of shared memory per CTA (5 CTAs/SM).
 // Gradients differ from variant 14 only in the order of the fp32 sums.
 // ------------------------------------------------------------------------------------------------------
+// DEPTH (the depth-gradient instantiation): part[slot][10][BATCH_ROW]; the moment-9 rows (sum alpha*T*dL/dD) are summed
+// like the moment-8 rows, split over the 8 lanes of a slot, and go to acc slot 9 in the same REDG as the opacity.
+// Rows start on bank 4*(slot*10 + i) mod 32, so the column writes and row reads stay conflict-free by the argument above.
 constexpr int BATCH_NB = 4;    // slots per flush (8 slots, 43 KB per CTA, measured no faster)
 constexpr int BATCH_ROW = 36;  // floats per row: 32 lanes + 4 of padding; 4 * 9 * 36 * 4 B = 5 KB per warp
+template <bool DEPTH> constexpr int batch_moments() { return DEPTH ? 10 : 9; }
 
 // Sums the nslot filled slots (warp-uniform; all lanes call it) and adds them to acc. The slots refer to the stage:
 // call it before the stage is refilled.
+template <bool DEPTH = false>
 __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpack, int nslot, const float4 (*stg)[32],
                                               const uint32_t* sid, float* acc, int lane, float ddelx_dx,
                                               float ddely_dy) {
+  constexpr int NM = batch_moments<DEPTH>();
   const unsigned F = 0xffffffffu;
   const int s = lane >> 3, m = lane & 7;  // this lane's slot and moment row
-  const float4* row = part4 + (s * 9 + m) * (BATCH_ROW / 4);
+  const float4* row = part4 + (s * NM + m) * (BATCH_ROW / 4);
   float4 t = row[0];
 #pragma unroll
   for (int k = 1; k < 8; k++) {
@@ -354,11 +375,19 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
     t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
   }
   const float tot = (t.x + t.y) + (t.z + t.w);
-  const float4 v8 = part4[(s * 9 + 8) * (BATCH_ROW / 4) + m];  // chunk m of the slot's moment-8 row
+  const float4 v8 = part4[(s * NM + 8) * (BATCH_ROW / 4) + m];  // chunk m of the slot's moment-8 row
   float sw = (v8.x + v8.y) + (v8.z + v8.w);
   sw += __shfl_xor_sync(F, sw, 1);
   sw += __shfl_xor_sync(F, sw, 2);
   sw += __shfl_xor_sync(F, sw, 4);
+  float sz = 0.f;  // DEPTH: the slot's sum alpha*T*dL/dD = dL/dz
+  if constexpr (DEPTH) {
+    const float4 v9 = part4[(s * NM + 9) * (BATCH_ROW / 4) + m];
+    sz = (v9.x + v9.y) + (v9.z + v9.w);
+    sz += __shfl_xor_sync(F, sz, 1);
+    sz += __shfl_xor_sync(F, sz, 2);
+    sz += __shfl_xor_sync(F, sz, 4);
+  }
   const float other = __shfl_xor_sync(F, tot, 7);  // s_x <-> s_y between moments 3 and 4
   if (s < nslot) {
     const int j = (jpack >> (5 * (nslot - 1 - s))) & 31u;
@@ -371,7 +400,13 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
     const float ka = is_x ? nAx : (is_y ? nCy : (m < 3 ? 1.0f : -0.5f));
     const float kb = is_x ? nBx : (is_y ? nBy : 0.0f);
     atomicAdd(dst + m, fmaf(kb, other, ka * tot));
-    if (m == 0) {
+    if constexpr (DEPTH) {
+      if (m < 2) {  // lane m = 0: opacity into slot 8, lane m = 1: dL/dz into slot 9
+        float rcp;
+        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(s1.y));
+        atomicAdd(dst + 8 + m, m == 0 ? sw * rcp : sz);
+      }
+    } else if (m == 0) {
       float rcp;  // o >= 1/255 for every staged splat (splat_subblock_mask): __fdividef(sw, o) without its denormal guard
       asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(s1.y));
       atomicAdd(dst + 8, sw * rcp);
@@ -380,9 +415,12 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
 }
 
 // BATCHED (variant 15): the per-splat reduction is deferred and batched through shared memory (flush_moments)
-template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false>
-__global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgs a, const int ntiles) {
+// DEPTH: variant 15 with the depth channel (a.dL_ddepth, tenth moment -> acc slot 9)
+template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false, bool DEPTH = false>
+__global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgsT<DEPTH> a, const int ntiles) {
   static_assert(!BATCHED || (NSB == 4 && SKIP && !MASKSKIP), "the batched reduction is written for variant 15");
+  static_assert(!DEPTH || BATCHED, "the depth channel is written for variant 15");
+  constexpr int NM = batch_moments<DEPTH>();
   __shared__ float4 s_stage[BW_WARPS][3][32];
   __shared__ uint32_t s_id[BW_WARPS][32];
   constexpr int PARTS = 8 / NSB;
@@ -395,7 +433,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
   uint32_t* sid = s_id[warp];
   float4* bpart = nullptr;  // BATCHED: part[slot][moment][BATCH_ROW] of this warp
   if constexpr (BATCHED) {
-    __shared__ float4 s_part[BW_WARPS][BATCH_NB * 9 * (BATCH_ROW / 4)];
+    __shared__ float4 s_part[BW_WARPS][BATCH_NB * NM * (BATCH_ROW / 4)];
     bpart = s_part[warp];
   }
   // BATCHED: a 1 followed by the stage index j (< 32) of each filled slot in 5 bits, the latest slot lowest; warp-uniform
@@ -422,6 +460,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
     const int px = tx * TILE + 8 * (kg & 1) + lx, py = ty * TILE + 4 * (kg >> 1) + ly;
     PixState p;
     p.T = 0.f; p.ar = 0.f; p.d0 = p.d1 = p.d2 = 0.f; p.bgT = 0.f;
+    if constexpr (DEPTH) p.dD = 0.f;
     nc[k] = 0;
     if (px < a.W && py < a.H) {
       const size_t pix_id = (size_t)a.W * py + px;
@@ -430,6 +469,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
       p.d0 = a.dL_dpix[pix_id];
       p.d1 = a.dL_dpix[HW + pix_id];
       p.d2 = a.dL_dpix[2 * HW + pix_id];
+      if constexpr (DEPTH) p.dD = a.dL_ddepth[pix_id];
       p.bgT = Tf * bg_term(a, pix_id, bg0, bg1, bg2, p);
       nc[k] = a.n_contrib[pix_id];
     }
@@ -522,15 +562,15 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
         if (SKIP && __any_sync(0xffffffffu, ok)) hitk |= 1u << k;
       }
       if (SKIP ? hitk == 0 : !__any_sync(0xffffffffu, anyhit)) continue;
-      float g[9];
+      float g[NM];
 #pragma unroll
-      for (int i = 0; i < 9; i++) g[i] = 0.f;
+      for (int i = 0; i < NM; i++) g[i] = 0.f;
 #pragma unroll
       for (int k = 0; k < NSB; k++) {
         // (alpha, G) = (0, 0) makes every update below an exact no-op: 1/(1-0) = 1, +0 contributions
         if (SKIP && !((hitk >> k) & 1u)) continue;
         if (MASKSKIP && !((m >> k) & 1u)) continue;
-        hit_update(ps[k], g, dxv[k & 1], dyv[k >> 1], G[k], al[k], s1.y, s2.x, s2.y, s2.z);
+        hit_update<DEPTH>(ps[k], g, dxv[k & 1], dyv[k >> 1], G[k], al[k], s1.y, s2.x, s2.y, s2.z, s1.z);
       }
       if constexpr (!BATCHED) {
         float m8;
@@ -538,22 +578,22 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
         finish_and_add(a.acc + (size_t)sid[j] * ACC_STRIDE, tot, m8, role, s0.z, s0.w, s1.x, s1.y, ddelx_dx, ddely_dy);
       } else {
 #pragma unroll
-        for (int i = 0; i < 9; i++) col[BATCH_ROW * i] = g[i];
-        col += 9 * BATCH_ROW;
+        for (int i = 0; i < NM; i++) col[BATCH_ROW * i] = g[i];
+        col += NM * BATCH_ROW;
         jpack = (jpack << 5) | (uint32_t)j;
         if (jpack >= 1u << (5 * BATCH_NB)) {  // all slots filled
           __syncwarp();
-          flush_moments(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
+          flush_moments<DEPTH>(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
           __syncwarp();  // the next splat overwrites slot 0
           jpack = 1;
-          col -= BATCH_NB * 9 * BATCH_ROW;
+          col -= BATCH_NB * NM * BATCH_ROW;
         }
       }
     }
     if constexpr (BATCHED) {
       if (jpack > 1) {  // before the stage is refilled
         __syncwarp();
-        flush_moments(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
+        flush_moments<DEPTH>(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
         col = reinterpret_cast<float*>(bpart) + lane;
         jpack = 1;
       }
@@ -634,7 +674,7 @@ __global__ void __launch_bounds__(TILE_PIX) render_bwd_cta_kernel(const BwdArgs 
 
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own,
-                      const float* dL_dalpha_img) {
+                      const float* dL_dalpha_img, const float* dL_ddepth) {
   BwdArgs a;
   a.dL_dalpha_img = dL_dalpha_img;
   a.own_stride = own.stride; a.own_phase = own.phase;
@@ -646,7 +686,13 @@ int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningW
   if (ntiles == 0) return GSR_OK;
   int v = g_opt.render_bwd_variant;
   if (v == 0 && own.stride != 1) v = 4;  // the CTA-per-tile kernel maps blockIdx to tiles directly: single-GPU only
-  if (v == 0) {
+  if (dL_ddepth != nullptr) {  // the depth channel exists only in variant 15, whatever the option says. At 5 CTAs/SM
+    // (96 registers) it spills 20 bytes; at 4 CTAs/SM it does not.
+    BwdDepthArgs da;
+    static_cast<BwdArgs&>(da) = a;
+    da.dL_ddepth = dL_ddepth;
+    render_bwd_flat_kernel<4, 4, true, false, true, true><<<(ntiles * 2 + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(da, ntiles);
+  } else if (v == 0) {
     render_bwd_cta_kernel<<<dim3(a.gx, a.gy), dim3(TILE, TILE), 0, st>>>(a);
   } else if (v == 2) {
     const int warps = ntiles * 2;

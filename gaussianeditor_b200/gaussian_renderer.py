@@ -63,9 +63,13 @@ def _python_sh_colors(pc, camera_center) -> torch.Tensor:
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           fused_activations: bool = False):
+           fused_activations: bool = False, depth_grad: bool = False):
     """Render the scene; background tensor must be on the GPU. Returns the reference's dictionary:
     render [3,H,W], viewspace_points [P,3] (grad sink for densification), visibility_filter, radii, depth_3dgs.
+
+    ``depth_grad=True`` (opt-in, not in the reference) makes ``depth_3dgs`` differentiable, so that a depth term in the
+    loss (e.g. against a monocular depth estimate) trains the Gaussians; by default its gradient is dropped, as in the
+    reference. Works on both the plain and the fused-activation path.
 
     ``fused_activations=True`` (opt-in, not in the reference; SURVEY 8(f-3)) hands the scene model's RAW parameters
     (``pc._opacity, pc._features_dc, pc._features_rest, pc._scaling, pc._rotation``) to the rasterizer, which applies
@@ -79,8 +83,11 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         screenspace_points.retain_grad()
     except Exception:
         pass
+    # depth_grad is passed only when asked for: by default the rasterizer is constructed exactly as the reference's
+    # render() does, so any class with the reference's constructor (raster_settings only) can stand in for it
+    opt = {"depth_grad": True} if depth_grad else {}
     rasterizer = GaussianRasterizer(
-        raster_settings=_settings_for(viewpoint_camera, bg_color, scaling_modifier, pc.active_sh_degree))
+        raster_settings=_settings_for(viewpoint_camera, bg_color, scaling_modifier, pc.active_sh_degree), **opt)
     python_sh = getattr(pipe, "convert_SHs_python", False)
     python_cov = getattr(pipe, "compute_cov3D_python", False)
 

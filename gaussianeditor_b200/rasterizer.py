@@ -209,9 +209,13 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, return_alpha=False, camera_grad=False):
+                        raster_settings, return_alpha=False, camera_grad=False, depth_grad=False):
+    rs = raster_settings
+    if depth_grad:    # the depth output's gradient is used (gsr_backward_depth); without it, it is dropped as in the reference
+        cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if camera_grad else (None, None, None)
+        return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                         cov3Ds_precomp, rs, return_alpha, *cam, True)
     if camera_grad:   # the camera arrays become autograd inputs of the node (they are read from the settings as usual)
-        rs = raster_settings
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                          cov3Ds_precomp, rs, return_alpha, rs.viewmatrix, rs.projmatrix, rs.campos)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
@@ -231,12 +235,17 @@ def _alpha_image(lib, state, device):
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, return_alpha=False, viewmatrix=None, projmatrix=None, campos=None):
+                raster_settings, return_alpha=False, viewmatrix=None, projmatrix=None, campos=None, depth_grad=False):
         color, depth, state, inputs = _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations,
                                                     cov3Ds_precomp, raster_settings)
         ctx.raster_settings = raster_settings
         ctx.camera_grad = viewmatrix is not None
+        ctx.depth_grad = bool(depth_grad)
         ctx.n_inputs = 10 + (3 if ctx.camera_grad else 0)
+        if ctx.depth_grad:
+            # outputs without a gradient arrive as None: no depth gradient -> the ordinary backward, and a loss on the
+            # depth alone leaves the colour gradient None (treated as zeros)
+            ctx.set_materialize_grads(False)
         ctx.state = state
         ctx.save_for_backward(*inputs, state.radii, state.geom, state.binning, state.img)
         ctx.mark_non_differentiable(state.radii)
@@ -256,6 +265,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         device = means3D.device
         P, M, W, H = state.P, state.M, state.W, state.H
         with torch.cuda.device(device):
+            if grad_out_color is None:   # depth_grad: only the depth and/or alpha outputs carry a loss
+                grad_out_color = torch.zeros(3, H, W, dtype=torch.float32, device=device)
             grad_out_color = _f32c(grad_out_color, device)
             f32 = dict(dtype=torch.float32, device=device)
             dL_dmeans3D = torch.empty(P, 3, **f32); dL_dmeans2D = torch.empty(P, 3, **f32)
@@ -271,7 +282,23 @@ class _RasterizeGaussians(torch.autograd.Function):
                 gr = _lib.Grads(_ptr(dL_dmeans3D), _ptr(dL_dmeans2D), _ptr(dL_dcolors), _ptr(dL_dopacity),
                                 _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations))
                 st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-                if ctx.camera_grad:
+                if ctx.depth_grad and grad_depth is not None:
+                    gd = _f32c(grad_depth, device)
+                    ga = None if grad_alpha is None else _f32c(grad_alpha, device)
+                    cam = None
+                    if ctx.camera_grad:
+                        d_view = torch.empty(16, **f32); d_proj = torch.empty(16, **f32); d_cam = torch.empty(3, **f32)
+                        cbytes = lib.gsr_camera_scratch_bytes(P)
+                        cscratch = torch.empty(cbytes, dtype=torch.uint8, device=device)
+                        cam = _lib.CameraGrads(_ptr(d_view), _ptr(d_proj), _ptr(d_cam), _ptr(cscratch), cbytes)
+                        cam_grads = (d_view.view(rs.viewmatrix.shape), d_proj.view(rs.projmatrix.shape),
+                                     d_cam.view(rs.campos.shape))
+                    _lib.check(lib.gsr_backward_depth(C.byref(s), C.byref(c), state.cap, _ptr(geom), geom.numel(),
+                                                      _ptr(binning), binning.numel(), _ptr(img), img.numel(),
+                                                      _ptr(radii), _ptr(grad_out_color), _ptr(ga), _ptr(gd),
+                                                      _ptr(scratch), sbytes, C.byref(gr),
+                                                      None if cam is None else C.byref(cam), st), "gsr_backward_depth")
+                elif ctx.camera_grad:
                     d_view = torch.empty(16, **f32); d_proj = torch.empty(16, **f32); d_cam = torch.empty(3, **f32)
                     cbytes = lib.gsr_camera_scratch_bytes(P)
                     cscratch = torch.empty(cbytes, dtype=torch.uint8, device=device)
@@ -304,6 +331,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 z = lambda t: torch.zeros_like(t, dtype=torch.float32)
                 cam_grads = (z(rs.viewmatrix), z(rs.projmatrix), z(rs.campos))
             grads = grads + cam_grads
+        if ctx.depth_grad:
+            grads = grads + ((None, None, None) if not ctx.camera_grad else ()) + (None,)
         return grads
 
 
@@ -313,12 +342,15 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
-                raster_settings):
+                raster_settings, depth_grad=False):
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         color, depth, state, inputs = _forward_impl(means3D, features_dc, empty, opacity_logits, log_scales,
                                                     raw_rotations, empty, raster_settings, raw_rest=features_rest)
         ctx.raster_settings = raster_settings
         ctx.state = state
+        ctx.depth_grad = bool(depth_grad)
+        if ctx.depth_grad:   # as _RasterizeGaussians: None = no gradient for that output
+            ctx.set_materialize_grads(False)
         (m3, dc, _, op, sc, ro, _, rest) = inputs
         ctx.save_for_backward(m3, dc, rest, op, sc, ro, state.radii, state.geom, state.binning, state.img)
         ctx.mark_non_differentiable(state.radii)
@@ -333,6 +365,8 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
         device = means3D.device
         P, M = state.P, state.M
         with torch.cuda.device(device):
+            if grad_out_color is None:   # depth_grad: a loss on the depth alone
+                grad_out_color = torch.zeros(3, state.H, state.W, dtype=torch.float32, device=device)
             grad_out_color = _f32c(grad_out_color, device)
             f32 = dict(dtype=torch.float32, device=device)
             d_m3 = torch.empty(P, 3, **f32); d_m2 = torch.empty(P, 3, **f32); d_op = torch.empty(P, 1, **f32)
@@ -346,30 +380,46 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                 sbytes = lib.gsr_backward_scratch_bytes(P)
                 scratch = torch.empty(sbytes, dtype=torch.uint8, device=device)
                 st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-                _lib.check(lib.gsr_backward_raw(C.byref(s), C.byref(rc), state.cap, _ptr(geom), geom.numel(),
-                                                _ptr(binning), binning.numel(), _ptr(img), img.numel(), _ptr(radii),
-                                                _ptr(grad_out_color), _ptr(scratch), sbytes, C.byref(gr), st),
-                           "gsr_backward_raw")
+                if ctx.depth_grad and grad_depth is not None:
+                    gd = _f32c(grad_depth, device)
+                    _lib.check(lib.gsr_backward_raw_depth(C.byref(s), C.byref(rc), state.cap, _ptr(geom), geom.numel(),
+                                                          _ptr(binning), binning.numel(), _ptr(img), img.numel(),
+                                                          _ptr(radii), _ptr(grad_out_color), _ptr(gd),
+                                                          _ptr(scratch), sbytes, C.byref(gr), st), "gsr_backward_raw_depth")
+                else:
+                    _lib.check(lib.gsr_backward_raw(C.byref(s), C.byref(rc), state.cap, _ptr(geom), geom.numel(),
+                                                    _ptr(binning), binning.numel(), _ptr(img), img.numel(), _ptr(radii),
+                                                    _ptr(grad_out_color), _ptr(scratch), sbytes, C.byref(gr), st),
+                               "gsr_backward_raw")
+        if ctx.depth_grad:
+            return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None
         return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False):
+    def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False):
         """``return_alpha=True`` (opt-in, not in the reference) appends a fourth output to ``forward``: the alpha image
         ``1 - final_T`` [1,H,W] (the reference keeps final_T as ``accum_alpha`` but never returns it); it is
         differentiable like the colour.
         ``camera_grad=True`` (opt-in, not in the reference): ``raster_settings.viewmatrix / projmatrix / campos`` become
         differentiable inputs -- their ``.grad`` is filled by the backward (gsr_backward_camera), each array treated as an
-        independent input exactly as the forward reads it."""
+        independent input exactly as the forward reads it.
+        ``depth_grad=True`` (opt-in, for ``forward`` and ``forward_raw``): the depth output becomes differentiable
+        (gsr_backward_depth). By default its gradient is dropped, as in the reference. When the depth receives no
+        gradient the ordinary backward runs; a loss on the depth alone works too."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_alpha = bool(return_alpha)
         self.camera_grad = bool(camera_grad)
+        self.depth_grad = bool(depth_grad)
 
     def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations):
         """Opt-in fused-activation call (not part of the reference API): the arguments are the scene model's raw
         parameters (``_xyz, _opacity, _features_dc, _features_rest, _scaling, _rotation``); sigmoid / exp / normalize
         and the SH concatenation happen inside the preprocess kernels. Same return tuple as ``forward``."""
+        if self.depth_grad:
+            return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
+                                                raw_rotations, self.raster_settings, True)
         return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
                                             raw_rotations, self.raster_settings)
 
@@ -415,7 +465,7 @@ class GaussianRasterizer(nn.Module):
             cov3D_precomp = empty
 
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                   cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad)
+                                   cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad, self.depth_grad)
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):

@@ -177,6 +177,23 @@ GSR_API int gsr_backward_camera(const gsr_settings* s, const gsr_cloud* c, int32
                         const float* dL_dout_alpha /* may be NULL */, void* scratch, size_t scratch_bytes,
                         const gsr_grads* grads, const gsr_camera_grads* camera, void* stream);
 
+/* ---- depth gradients (north-star output "RGB / depth / alpha"; opt-in, the reference drops dL/ddepth) -----------
+ * The forward's depth image is D = sum_i z_i alpha_i T_i with the view depth z_i = (view * mean).z and no background
+ * term. gsr_backward_depth is gsr_backward with the additional upstream gradient dL_dout_depth [H*W] (must not be NULL):
+ * depth enters the blending backward as a fourth colour channel with colour z_i and background 0, so it reaches
+ * dL/dmean2D, dL/dconic and dL/dopacity through dL/dalpha_i, and dL/dz_i = sum_pixels alpha_i T_i dL/dD reaches
+ * dL/dmeans3D through z_i (and dL/dviewmatrix row 2 when `camera` is given). One call covers every combination:
+ * dL_dout_alpha may be NULL (as gsr_backward_alpha), `camera` may be NULL (as gsr_backward_camera). Pass a zero
+ * dL_dout_color for a loss on the depth alone. The blending backward always runs render_bwd variant 15 here.
+ * gsr_backward_raw_depth is the same for gsr_backward_raw (fused activations, below).
+ * Single-GPU only: the Gaussian-sharded entry points take no depth gradient. */
+GSR_API int gsr_backward_depth(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered, const void* geometry,
+                       size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
+                       size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                       const float* dL_dout_alpha /* may be NULL */, const float* dL_dout_depth, void* scratch,
+                       size_t scratch_bytes, const gsr_grads* grads, const gsr_camera_grads* camera /* may be NULL */,
+                       void* stream);
+
 /* ---- markVisible: present[i] = view-space z > 0.2 (auxiliary.h:139-164) ------------------------------- */
 GSR_API int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);
@@ -247,6 +264,12 @@ GSR_API int gsr_backward_raw(const gsr_settings* s, const gsr_raw_cloud* c, int3
                      size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                      size_t image_bytes, const int32_t* radii, const float* dL_dout_color, void* scratch,
                      size_t scratch_bytes, const gsr_raw_grads* grads, void* stream);
+/* gsr_backward_raw with the depth image's upstream gradient dL_dout_depth [H*W] (see gsr_backward_depth). */
+GSR_API int gsr_backward_raw_depth(const gsr_settings* s, const gsr_raw_cloud* c, int32_t num_rendered,
+                           const void* geometry, size_t geometry_bytes, const void* binning, size_t binning_bytes,
+                           const void* image, size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                           const float* dL_dout_depth, void* scratch, size_t scratch_bytes, const gsr_raw_grads* grads,
+                           void* stream);
 
 /* ---- Gaussian-sharded multi-GPU path (BASELINE config 4; SURVEY.md 8(e)) ----------------------------------
  * The reference has no multi-GPU rasterizer; these entry points split the single-GPU pipeline at the two places
