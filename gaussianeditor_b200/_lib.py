@@ -29,6 +29,8 @@ SYMBOLS = [
     "gsr_sparse_local_bytes", "gsr_sparse_candidate_bytes", "gsr_sparse_view", "gsr_sparse_preprocess", "gsr_sparse_order",
     "gsr_sparse_return", "gsr_sparse_backward_preprocess", "gsr_frame_broadcast", "gsr_peer_barrier",
     "gsr_backward_depth", "gsr_backward_raw_depth",
+    "gsr_deterministic_scratch_bytes", "gsr_backward_deterministic", "gsr_backward_raw_deterministic",
+    "gsr_apply_weights_deterministic",
 ]
 
 
@@ -150,6 +152,11 @@ def load():
     lib.gsr_backward_depth.restype = C.c_int
     lib.gsr_backward_depth.argtypes = [C.POINTER(Settings), C.POINTER(Cloud), i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp,
                                        vp, sz, C.POINTER(Grads), C.POINTER(CameraGrads), vp]
+    lib.gsr_deterministic_scratch_bytes.restype = sz
+    lib.gsr_deterministic_scratch_bytes.argtypes = [i32, i64, i32]
+    lib.gsr_backward_deterministic.restype = C.c_int
+    lib.gsr_backward_deterministic.argtypes = [C.POINTER(Settings), C.POINTER(Cloud), i32, vp, sz, vp, sz, vp, sz, vp, vp,
+                                               vp, vp, vp, sz, C.POINTER(Grads), C.POINTER(CameraGrads), vp, sz, vp]
     lib.gsr_alpha_image.restype = C.c_int
     lib.gsr_alpha_image.argtypes = [vp, sz, i32, i32, vp, vp]
     lib.gsr_mark_visible.restype = C.c_int
@@ -157,6 +164,9 @@ def load():
     lib.gsr_apply_weights.restype = C.c_int
     lib.gsr_apply_weights.argtypes = [C.POINTER(Settings), C.POINTER(Cloud), i32, vp, sz, vp, sz, vp, sz, vp, vp, i32,
                                       vp, vp, vp]
+    lib.gsr_apply_weights_deterministic.restype = C.c_int
+    lib.gsr_apply_weights_deterministic.argtypes = [C.POINTER(Settings), C.POINTER(Cloud), i32, vp, sz, vp, sz, vp, sz,
+                                                    vp, vp, i32, vp, vp, vp, sz, vp]
     lib.gsr_view_geometry.restype = C.c_int; lib.gsr_view_geometry.argtypes = [vp, i32, C.POINTER(GeometryView)]
     lib.gsr_view_binning.restype = C.c_int
     lib.gsr_view_binning.argtypes = [vp, i32, i64, i32, i32, C.POINTER(BinningView)]
@@ -196,6 +206,9 @@ def load():
     lib.gsr_backward_raw_depth.restype = C.c_int
     lib.gsr_backward_raw_depth.argtypes = [S, C.POINTER(RawCloud), i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, sz,
                                            C.POINTER(RawGrads), vp]
+    lib.gsr_backward_raw_deterministic.restype = C.c_int
+    lib.gsr_backward_raw_deterministic.argtypes = [S, C.POINTER(RawCloud), i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp,
+                                                   sz, C.POINTER(RawGrads), vp, sz, vp]
     SP = C.POINTER(SparsePlan)
     lib.gsr_sparse_local_bytes.restype = sz; lib.gsr_sparse_local_bytes.argtypes = [i32]
     lib.gsr_sparse_candidate_bytes.restype = sz; lib.gsr_sparse_candidate_bytes.argtypes = [i32, i32]

@@ -107,6 +107,25 @@ size_t gsr_binning_bytes(int32_t P, int64_t R, int32_t W, int32_t H) {
   return ws.total;
 }
 size_t gsr_backward_scratch_bytes(int32_t P) { return align_up((size_t)(P > 0 ? P : 1) * ACC_STRIDE * sizeof(float)); }
+size_t gsr_deterministic_scratch_bytes(int32_t P, int64_t num_rendered, int32_t num_channels) {
+  DetWS d;
+  if (!carve_det(nullptr, P, num_rendered, num_channels, d)) return 0;
+  return d.total;
+}
+
+// the deterministic-mode scratch of one call (gsr_*_deterministic), checked against P and R
+struct DetScratch {
+  void* ptr;
+  size_t bytes;
+};
+static int carve_det_checked(const DetScratch& ds, int P, int64_t R, int CH, DetWS& d) {
+  if (!carve_det(ds.ptr, P, R, CH, d)) { set_error("deterministic scratch: bad sizes"); return GSR_ERR_INVALID; }
+  if (!ds.ptr || ds.bytes < d.total) {
+    set_error("deterministic scratch too small: %zu < %zu", ds.bytes, d.total);
+    return GSR_ERR_WORKSPACE;
+  }
+  return GSR_OK;
+}
 
 // First forward half on a carved workspace: preprocess, depth order, tile-count scan, and the copy of num_rendered to
 // the host. With the tile-binning path (tile_binning.cu) the preprocess kernel accumulates the count itself, so the copy
@@ -199,7 +218,7 @@ static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, c
                          const void* binning, size_t binning_bytes, const void* image, size_t image_bytes,
                          const int32_t* radii, const float* dL_dout_color, const float* dL_dout_alpha, void* scratch,
                          size_t scratch_bytes, const gsr_grads* gr, void* stream, const gsr_camera_grads* cam = nullptr,
-                         const float* dL_dout_depth = nullptr) {
+                         const float* dL_dout_depth = nullptr, const DetScratch* ds = nullptr) {
   int rc = validate_cloud(s, c);
   if (rc) return rc;
   if (!gr || !dL_dout_color) { set_error("grads / dL_dout_color is null"); return GSR_ERR_INVALID; }
@@ -217,12 +236,17 @@ static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, c
   if (rc) return rc;
   const size_t need = gsr_backward_scratch_bytes(c->P);
   if (!scratch || scratch_bytes < need) { set_error("backward scratch too small: %zu < %zu", scratch_bytes, need); return GSR_ERR_WORKSPACE; }
+  DetWS det;
+  if (ds && (rc = carve_det_checked(*ds, c->P, R, 0, det))) return rc;
   {
-    StageScope t(ST_RENDER_BWD, st);  // includes zeroing the accumulators
-    cudaError_t e = cudaMemsetAsync(scratch, 0, (size_t)c->P * ACC_STRIDE * sizeof(float), st);
-    if (e != cudaSuccess) return check_cuda(e, "scratch memset");
+    StageScope t(ST_RENDER_BWD, st);  // includes zeroing the accumulators (deterministic mode: the reduction)
+    if (!ds || R <= 0) {  // the deterministic reduction writes every accumulator itself
+      cudaError_t e = cudaMemsetAsync(scratch, 0, (size_t)c->P * ACC_STRIDE * sizeof(float), st);
+      if (e != cudaSuccess) return check_cuda(e, "scratch memset");
+    }
     if (R > 0) {
-      rc = launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)scratch, st, TileOwner(), dL_dout_alpha, dL_dout_depth);
+      rc = launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)scratch, st, TileOwner(), dL_dout_alpha, dL_dout_depth,
+                             ds ? &det : nullptr, c->P, R);
       if (rc) return rc;
     }
   }
@@ -246,7 +270,8 @@ static int camera_backward(const gsr_settings* s, const gsr_cloud* c, int32_t R,
                            size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                            size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
                            const float* dL_dout_alpha, void* scratch, size_t scratch_bytes, const gsr_grads* gr,
-                           const gsr_camera_grads* cam, void* stream, const float* dL_dout_depth) {
+                           const gsr_camera_grads* cam, void* stream, const float* dL_dout_depth,
+                           const DetScratch* ds = nullptr) {
   if (!cam) { set_error("camera gradients: null struct"); return GSR_ERR_INVALID; }
   if (c && c->P == 0) {  // nothing contributes: the gradients are zero
     cudaStream_t st = (cudaStream_t)stream;
@@ -257,7 +282,7 @@ static int camera_backward(const gsr_settings* s, const gsr_cloud* c, int32_t R,
     if (e != cudaSuccess) return check_cuda(e, "camera gradient memset");
   }
   return backward_impl(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
-                       dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, stream, cam, dL_dout_depth);
+                       dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, stream, cam, dL_dout_depth, ds);
 }
 
 int gsr_backward_camera(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry, size_t geometry_bytes,
@@ -279,6 +304,20 @@ int gsr_backward_depth(const gsr_settings* s, const gsr_cloud* c, int32_t R, con
                            dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, cam, stream, dL_dout_depth);
   return backward_impl(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
                        dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, stream, nullptr, dL_dout_depth);
+}
+
+int gsr_backward_deterministic(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry,
+                               size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
+                               size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                               const float* dL_dout_alpha, const float* dL_dout_depth, void* scratch,
+                               size_t scratch_bytes, const gsr_grads* gr, const gsr_camera_grads* cam,
+                               void* det_scratch, size_t det_scratch_bytes, void* stream) {
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  if (cam)
+    return camera_backward(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                           dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, cam, stream, dL_dout_depth, &ds);
+  return backward_impl(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                       dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, stream, nullptr, dL_dout_depth, &ds);
 }
 
 int gsr_backward(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry, size_t geometry_bytes,
@@ -315,9 +354,10 @@ int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, c
   return launch_mark_visible(P, means3D, viewmatrix, present, (cudaStream_t)stream);
 }
 
-int gsr_apply_weights(const gsr_settings* s, const gsr_cloud* c, int32_t R, void* geometry, size_t geometry_bytes,
-                      void* binning, size_t binning_bytes, void* image, size_t image_bytes, const int32_t* radii,
-                      const float* image_weights, int32_t CH, float* weights, int32_t* cnt, void* stream) {
+static int apply_weights_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, void* geometry,
+                              size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                              size_t image_bytes, const int32_t* radii, const float* image_weights, int32_t CH,
+                              float* weights, int32_t* cnt, void* stream, const DetScratch* ds) {
   int rc = validate_cloud(s, c);
   if (rc) return rc;
   if (!image_weights || !weights || !cnt) { set_error("apply_weights: null buffer"); return GSR_ERR_INVALID; }
@@ -326,10 +366,29 @@ int gsr_apply_weights(const gsr_settings* s, const gsr_cloud* c, int32_t R, void
   GeometryWS g; BinningWS b; ImageWS im;
   rc = carve_all(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, g, b, im);
   if (rc) return rc;
+  DetWS det;
+  if (ds && (rc = carve_det_checked(*ds, c->P, R, CH, det))) return rc;
   rc = run_binning(*s, *c, R, false, g, b, im, radii, st);
   if (rc) return rc;
-  StageScope t(ST_APPLY_W, st);
-  return launch_apply_weights(*s, g, b, im, image_weights, CH, weights, cnt, st);
+  StageScope t(ST_APPLY_W, st);  // deterministic mode: includes the reduction
+  return launch_apply_weights(*s, g, b, im, image_weights, CH, weights, cnt, st, ds ? &det : nullptr, c->P, R);
+}
+
+int gsr_apply_weights(const gsr_settings* s, const gsr_cloud* c, int32_t R, void* geometry, size_t geometry_bytes,
+                      void* binning, size_t binning_bytes, void* image, size_t image_bytes, const int32_t* radii,
+                      const float* image_weights, int32_t CH, float* weights, int32_t* cnt, void* stream) {
+  return apply_weights_impl(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                            image_weights, CH, weights, cnt, stream, nullptr);
+}
+
+int gsr_apply_weights_deterministic(const gsr_settings* s, const gsr_cloud* c, int32_t R, void* geometry,
+                                    size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                                    size_t image_bytes, const int32_t* radii, const float* image_weights, int32_t CH,
+                                    float* weights, int32_t* cnt, void* det_scratch, size_t det_scratch_bytes,
+                                    void* stream) {
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  return apply_weights_impl(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                            image_weights, CH, weights, cnt, stream, &ds);
 }
 
 // ---- fused activations (raw parameters) --------------------------------------------------------------------
@@ -364,7 +423,7 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
                              size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                              size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
                              const float* dL_dout_depth, void* scratch, size_t scratch_bytes, const gsr_raw_grads* gr,
-                             void* stream) {
+                             void* stream, const DetScratch* ds = nullptr) {
   gsr_cloud c;
   int rc = raw_to_cloud(s, r, c);
   if (rc) return rc;
@@ -386,12 +445,17 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
   if (rc) return rc;
   const size_t need = gsr_backward_scratch_bytes(c.P);
   if (!scratch || scratch_bytes < need) { set_error("backward scratch too small: %zu < %zu", scratch_bytes, need); return GSR_ERR_WORKSPACE; }
+  DetWS det;
+  if (ds && (rc = carve_det_checked(*ds, c.P, R, 0, det))) return rc;
   {
     StageScope t(ST_RENDER_BWD, st);
-    cudaError_t e = cudaMemsetAsync(scratch, 0, (size_t)c.P * ACC_STRIDE * sizeof(float), st);
-    if (e != cudaSuccess) return check_cuda(e, "scratch memset");
+    if (!ds || R <= 0) {  // the deterministic reduction writes every accumulator itself
+      cudaError_t e = cudaMemsetAsync(scratch, 0, (size_t)c.P * ACC_STRIDE * sizeof(float), st);
+      if (e != cudaSuccess) return check_cuda(e, "scratch memset");
+    }
     if (R > 0) {
-      rc = launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)scratch, st, TileOwner(), nullptr, dL_dout_depth);
+      rc = launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)scratch, st, TileOwner(), nullptr, dL_dout_depth,
+                             ds ? &det : nullptr, c.P, R);
       if (rc) return rc;
     }
   }
@@ -419,6 +483,16 @@ int gsr_backward_raw_depth(const gsr_settings* s, const gsr_raw_cloud* r, int32_
   if (!dL_dout_depth) { set_error("dL_dout_depth is null"); return GSR_ERR_INVALID; }
   return raw_backward_impl(s, r, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
                            dL_dout_color, dL_dout_depth, scratch, scratch_bytes, gr, stream);
+}
+
+int gsr_backward_raw_deterministic(const gsr_settings* s, const gsr_raw_cloud* r, int32_t R, const void* geometry,
+                                   size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
+                                   size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                                   const float* dL_dout_depth, void* scratch, size_t scratch_bytes,
+                                   const gsr_raw_grads* gr, void* det_scratch, size_t det_scratch_bytes, void* stream) {
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  return raw_backward_impl(s, r, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                           dL_dout_color, dL_dout_depth, scratch, scratch_bytes, gr, stream, &ds);
 }
 
 // ---- Gaussian-sharded multi-GPU path ---------------------------------------------------------------------

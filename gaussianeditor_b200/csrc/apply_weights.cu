@@ -92,10 +92,121 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_kernel(const AwArgs a)
   }
 }
 
+
+// Deterministic mode (DetWS, deterministic.cu): the same walk, but the per-warp sums of a 256-splat round go to shared
+// memory [8 warps][256][CH]. At the round boundary (where __syncthreads_count already synchronises, and so also before
+// the early break) thread t adds the 8 warp entries of splat t in warp order and stores the row at that instance's
+// emission slot, with its flag; the reduction kernel adds each Gaussian's rows to `weights`. `cnt` keeps its integer
+// atomics, which are exact.
+struct AwDetArgs : AwArgs {
+  const uint32_t* excl;
+  float* rows;     // [R, CH]
+  uint8_t* flags;  // [R]
+};
+
+template <int CH>
+__global__ void __launch_bounds__(TILE_PIX) apply_weights_det_kernel(const AwDetArgs a) {
+  constexpr int NW = TILE_PIX / 32;
+  __shared__ float4 s_q0[TILE_PIX], s_q1[TILE_PIX];
+  __shared__ uint32_t s_ids[TILE_PIX];
+  __shared__ uint32_t s_slot[TILE_PIX];
+  __shared__ float s_w[NW][TILE_PIX][CH];
+  const int tile = blockIdx.y * a.gx + blockIdx.x;
+  const int tid = threadIdx.y * TILE + threadIdx.x;
+  const int lane = tid & 31, warp = tid >> 5;
+  const uint2 pix = make_uint2(blockIdx.x * TILE + threadIdx.x, blockIdx.y * TILE + threadIdx.y);
+  const bool inside = pix.x < (unsigned)a.W && pix.y < (unsigned)a.H;
+  const size_t pix_id = (size_t)a.W * pix.y + pix.x;
+  const float2 pixf = make_float2((float)pix.x, (float)pix.y);
+  const uint2 range = a.ranges[tile];
+  const int rounds = ((range.y - range.x + TILE_PIX - 1) / TILE_PIX);
+  int toDo = range.y - range.x;
+  bool done = !inside;
+  float T = 1.0f;
+  float Cw[CH];
+#pragma unroll
+  for (int ch = 0; ch < CH; ch++) Cw[ch] = inside ? a.image_weights[(size_t)ch * a.H * a.W + pix_id] : 0.f;
+  // row of splat t of the round just finished (block-uniform count n)
+  auto flush = [&](int n) {
+    if (tid < n) {
+      const size_t slot = s_slot[tid];
+#pragma unroll
+      for (int ch = 0; ch < CH; ch++) {
+        float v = s_w[0][tid][ch];
+#pragma unroll
+        for (int w = 1; w < NW; w++) v += s_w[w][tid][ch];
+        a.rows[slot * CH + ch] = v;
+      }
+      a.flags[slot] = 1;
+    }
+  };
+
+  int prev_n = 0;
+  for (int i = 0; i < rounds; i++, toDo -= TILE_PIX) {
+    int num_done = __syncthreads_count(done);
+    flush(prev_n);
+    prev_n = 0;
+    if (num_done == TILE_PIX) break;
+    int progress = i * TILE_PIX + tid;
+    if (range.x + progress < range.y) {
+      const uint32_t id = a.point_list[range.x + progress];
+      const float4* r = reinterpret_cast<const float4*>(a.records + id);
+      const uint32_t ex = __ldg(a.excl + id);
+      const float4 q0 = __ldg(r);
+      s_q0[tid] = q0;
+      s_q1[tid] = __ldg(r + 1);
+      s_ids[tid] = id;
+      s_slot[tid] = emission_slot(ex, q0.x, q0.y, __float_as_int(__ldg(r + 2).w), a.gx, a.gy, blockIdx.x, blockIdx.y);
+    }
+    __syncthreads();
+    const int n = min(TILE_PIX, toDo);
+    for (int j = 0; j < n; j++) {
+      bool hit = false;
+      if (!done) {
+        const float4 q0 = s_q0[j], q1 = s_q1[j];
+        const float dx = q0.x - pixf.x, dy = q0.y - pixf.y;
+        const float power = splat_power(dx, dy, q0.z, q0.w, q1.x);
+        if (!(power > 0.0f)) {
+          const float alpha = fminf(0.99f, __fmul_rn(q1.y, expf(power)));
+          if (!(alpha < 1.0f / 255.0f)) {
+            const float test_T = __fmul_rn(T, __fadd_rn(1.0f, -alpha));
+            if (test_T < 0.0001f) {
+              done = true;
+            } else {
+              hit = true;
+              T = test_T;
+            }
+          }
+        }
+      }
+      const unsigned hits = __ballot_sync(0xffffffffu, hit);
+      if (hits) {
+#pragma unroll
+        for (int ch = 0; ch < CH; ch++) {
+          float v = hit ? Cw[ch] : 0.f;
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+          if (lane == 0) s_w[warp][j][ch] = v;
+        }
+        if (lane == 0) atomicAdd(a.cnt + s_ids[j], CH * __popc(hits));
+      } else if (lane == 0) {
+#pragma unroll
+        for (int ch = 0; ch < CH; ch++) s_w[warp][j][ch] = 0.f;
+      }
+    }
+    prev_n = n;
+  }
+  if (prev_n > 0) {  // block-uniform: the last round ran to its end
+    __syncthreads();
+    flush(prev_n);
+  }
+}
+
 }  // namespace
 
 int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
-                         const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st) {
+                         const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st,
+                         const DetWS* det, int P, int64_t R) {
   AwArgs a;
   a.ranges = im.ranges; a.point_list = b.point_list; a.records = g.records;
   a.W = s.image_width; a.H = s.image_height;
@@ -103,6 +214,19 @@ int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const Binni
   a.image_weights = image_weights; a.weights = weights; a.cnt = cnt;
   if (a.gx * a.gy == 0) return GSR_OK;
   dim3 grid(a.gx, a.gy), block(TILE, TILE);
+  if (det != nullptr && CH >= 1 && CH <= 3) {
+    int rc = launch_det_prepare(P, R, 1, g, *det, st);
+    if (rc) return rc;
+    AwDetArgs da;
+    static_cast<AwArgs&>(da) = a;
+    da.excl = det->excl; da.rows = det->rows; da.flags = det->flags;
+    if (CH == 1) apply_weights_det_kernel<1><<<grid, block, 0, st>>>(da);
+    else if (CH == 2) apply_weights_det_kernel<2><<<grid, block, 0, st>>>(da);
+    else apply_weights_det_kernel<3><<<grid, block, 0, st>>>(da);
+    g_launches++;
+    if ((rc = check_launch("apply_weights", s.debug != 0, st))) return rc;
+    return launch_det_reduce_weights(P, CH, g, *det, weights, st);
+  }
   if (CH == 1) apply_weights_kernel<1><<<grid, block, 0, st>>>(a);
   else if (CH == 2) apply_weights_kernel<2><<<grid, block, 0, st>>>(a);
   else if (CH == 3) apply_weights_kernel<3><<<grid, block, 0, st>>>(a);

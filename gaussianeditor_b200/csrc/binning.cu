@@ -46,14 +46,6 @@ struct GatherTilesOp {
   __host__ __device__ __forceinline__ uint32_t operator()(uint32_t rank) const { return tiles[order[rank]]; }
 };
 
-__device__ __forceinline__ void tile_rect(float px, float py, int radius, int gx, int gy, uint2& rmin, uint2& rmax) {
-  // auxiliary.h:46-56
-  rmin.x = (unsigned)min(gx, max((int)0, (int)((px - radius) / TILE)));
-  rmin.y = (unsigned)min(gy, max((int)0, (int)((py - radius) / TILE)));
-  rmax.x = (unsigned)min(gx, max((int)0, (int)((px + radius + TILE - 1) / TILE)));
-  rmax.y = (unsigned)min(gy, max((int)0, (int)((py + radius + TILE - 1) / TILE)));
-}
-
 // Rows of the rectangle [rmin.y, rmax.y) this rank owns (ty % stride == phase): first owned row and their number.
 __device__ __forceinline__ void owned_rows(uint32_t ymin, uint32_t ymax, int stride, int phase, uint32_t& y0, uint32_t& ny) {
   if (stride == 1) { y0 = ymin; ny = ymax - ymin; return; }

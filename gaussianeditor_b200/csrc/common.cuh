@@ -94,6 +94,27 @@ void carve_image(void* base, int W, int H, ImageWS& ws);
 //   [9] dL/dz (view depth) when the depth image has an upstream gradient, else 0; [10..11] padding
 constexpr int ACC_STRIDE = 12;
 
+// Deterministic mode (deterministic.cu): the float atomics of render_bwd and apply_weights are replaced by plain stores
+// of one row per (instance, tile half) -- per instance for apply_weights -- at the instance's EMISSION SLOT, the
+// position binning gave it before the tile sort:
+//   slot(g, tile) = excl[g] + (ty - rmin.y) * (rmax.x - rmin.x) + (tx - rmin.x)
+// with excl[g] the exclusive prefix of the tile counts in depth order and [rmin, rmax) the tile rectangle (tile_rect).
+// The slots of Gaussian g are [excl[g], excl[g] + tiles_touched[g]), so one reduction kernel adds each Gaussian's
+// flagged rows in a fixed order: the result depends on the data only, never on timing.
+struct DetWS {
+  uint32_t* excl;   // [P]
+  uint8_t* flags;   // [2R]: row written this call
+  float* rows;      // [2R, ACC_STRIDE] (render_bwd) or [R, CH] (apply_weights)
+  size_t total;
+};
+bool carve_det(void* base, int P, int64_t R, int CH, DetWS& ws);
+// clears the flags of R instances x `rows_per` rows and computes excl[] from the forward's depth order and offsets
+int launch_det_prepare(int P, int64_t R, int rows_per, const GeometryWS& g, const DetWS& d, cudaStream_t st);
+// acc[g] = sum of g's flagged rows (all ACC_STRIDE words written, zeros for a Gaussian without any)
+int launch_det_reduce_acc(int P, bool depth, const GeometryWS& g, const DetWS& d, float* acc, cudaStream_t st);
+// weights[g*CH + ch] += sum of g's flagged rows (untouched when there is none)
+int launch_det_reduce_weights(int P, int CH, const GeometryWS& g, const DetWS& d, float* weights, cudaStream_t st);
+
 // ---- options -----------------------------------------------------------------------------------------
 struct Options {
   int render_fwd_variant = 3;  // 0 CTA/tile, 1/2/3 = 1/2/4 warps per tile
@@ -162,9 +183,11 @@ int launch_tile_count(const GeometryWS& g, int gx, int gy, const TileOwner& own,
 int launch_render_fwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       float* out_color, float* out_depth, cudaStream_t st, const TileOwner& own = TileOwner());
 // dL_ddepth != nullptr: also the depth image's upstream [H*W]; dL/dz of each splat goes to acc slot 9 (variant 15 only)
+// det != nullptr: deterministic mode (single-GPU only): rows + reduction instead of atomics; acc needs no memset
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own = TileOwner(),
-                      const float* dL_dalpha_img = nullptr, const float* dL_ddepth = nullptr);
+                      const float* dL_dalpha_img = nullptr, const float* dL_ddepth = nullptr,
+                      const DetWS* det = nullptr, int P = 0, int64_t R = 0);
 // raw != nullptr: RAW variant -- gradients w.r.t. the raw parameters (gr.dL_dsh = d features_dc, raw->dL_dfeatures_rest)
 struct RawBackward {
   const float* features_rest;
@@ -186,7 +209,8 @@ int launch_preprocess_bwd(const gsr_settings& s, const gsr_cloud& c, const Geome
 int launch_alpha_image(const float* final_T, size_t n, float* out_alpha, cudaStream_t st);
 int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t st);
 int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
-                         const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st);
+                         const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st,
+                         const DetWS* det = nullptr, int P = 0, int64_t R = 0);
 
 // ---- host + device helpers ----------------------------------------------------------------------------
 // The per-pixel hit test and the sub-block culling predicate compile for the host too (oracle/subblock_check.cpp
@@ -291,6 +315,21 @@ __host__ __device__ __forceinline__ uint32_t splat_subblock_mask(const float4 q0
 __device__ __forceinline__ int owned_tile(int n, int gx, int stride, int phase) {
   const int r = n / gx;
   return (phase + r * stride) * gx + (n - r * gx);
+}
+
+// tile rectangle [rmin, rmax) of a splat (auxiliary.h:46-56); binning and the deterministic backward share it
+__device__ __forceinline__ void tile_rect(float px, float py, int radius, int gx, int gy, uint2& rmin, uint2& rmax) {
+  rmin.x = (unsigned)min(gx, max((int)0, (int)((px - radius) / TILE)));
+  rmin.y = (unsigned)min(gy, max((int)0, (int)((py - radius) / TILE)));
+  rmax.x = (unsigned)min(gx, max((int)0, (int)((px + radius + TILE - 1) / TILE)));
+  rmax.y = (unsigned)min(gy, max((int)0, (int)((py + radius + TILE - 1) / TILE)));
+}
+// emission slot of the instance (Gaussian with exclusive prefix `excl` and radius `radius` at (px, py), tile (tx, ty))
+__device__ __forceinline__ uint32_t emission_slot(uint32_t excl, float px, float py, int radius, int gx, int gy, int tx,
+                                                  int ty) {
+  uint2 rmin, rmax;
+  tile_rect(px, py, radius, gx, gy, rmin, rmax);
+  return excl + ((uint32_t)ty - rmin.y) * (rmax.x - rmin.x) + ((uint32_t)tx - rmin.x);
 }
 
 // the four corners of a tile rectangle [rmin, rmax) in replica (idx & (copies-1)) of the (gy+1) x (gx+1) difference array

@@ -52,7 +52,16 @@ struct BwdArgs {
 struct BwdDepthArgs : BwdArgs {
   const float* dL_ddepth;  // [H*W] gradient of the depth image (gsr_backward_depth)
 };
-template <bool DEPTH> using BwdArgsT = std::conditional_t<DEPTH, BwdDepthArgs, BwdArgs>;
+// Arguments of the deterministic instantiations (DET): the finished rows go to rows[2*slot + part] with a flag instead
+// of atomics into acc (common.cuh: DetWS); again a separate type, so the other kernels keep their parameter block.
+template <class Base> struct BwdDetArgs : Base {
+  const uint32_t* excl;  // [P] exclusive prefix of the tile counts in depth order
+  float* rows;           // [2R, ACC_STRIDE]
+  uint8_t* flags;        // [2R]
+};
+template <bool DEPTH, bool DET = false>
+using BwdArgsT = std::conditional_t<DET, BwdDetArgs<std::conditional_t<DEPTH, BwdDepthArgs, BwdArgs>>,
+                                    std::conditional_t<DEPTH, BwdDepthArgs, BwdArgs>>;
 
 // One (pixel, splat) hit. `ar` tracks the reference's accum_rec (backward.cu:515) dotted with dL_dpixel, updated
 // eagerly; `bgT` = T_final * (bg . dL_dpixel).
@@ -360,10 +369,14 @@ template <bool DEPTH> constexpr int batch_moments() { return DEPTH ? 10 : 9; }
 
 // Sums the nslot filled slots (warp-uniform; all lanes call it) and adds them to acc. The slots refer to the stage:
 // call it before the stage is refilled.
-template <bool DEPTH = false>
+// DET: sid[j] holds the instance's emission slot instead of the Gaussian index; the finished row of stage entry j is
+// stored, not added, at rows[2*sid[j] + part] and its flag is set; the reduction kernel (deterministic.cu) adds the rows
+// of each Gaussian.
+template <bool DEPTH = false, bool DET = false>
 __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpack, int nslot, const float4 (*stg)[32],
                                               const uint32_t* sid, float* acc, int lane, float ddelx_dx,
-                                              float ddely_dy) {
+                                              float ddely_dy, float* rows = nullptr, uint8_t* flags = nullptr,
+                                              int part = 0) {
   constexpr int NM = batch_moments<DEPTH>();
   const unsigned F = 0xffffffffu;
   const int s = lane >> 3, m = lane & 7;  // this lane's slot and moment row
@@ -393,33 +406,46 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
     const int j = (jpack >> (5 * (nslot - 1 - s))) & 31u;
     const float4 s0 = stg[0][j];  // x, y, A, B
     const float4 s1 = stg[1][j];  // C, o
-    float* dst = acc + (size_t)sid[j] * ACC_STRIDE;
+    size_t row = 0;
+    if constexpr (DET) row = (size_t)2 * sid[j] + (size_t)part;
+    float* dst = DET ? rows + row * ACC_STRIDE : acc + (size_t)sid[j] * ACC_STRIDE;
     // as finish_and_add: m<3 tot | 3: -(A*s_x + B*s_y)*0.5W | 4: -(C*s_y + B*s_x)*0.5H | 5..7: -0.5*tot | opacity sw / o
     const bool is_x = m == 3, is_y = m == 4;
     const float nAx = -s0.z * ddelx_dx, nCy = -s1.x * ddely_dy, nBx = -s0.w * ddelx_dx, nBy = -s0.w * ddely_dy;
     const float ka = is_x ? nAx : (is_y ? nCy : (m < 3 ? 1.0f : -0.5f));
     const float kb = is_x ? nBx : (is_y ? nBy : 0.0f);
-    atomicAdd(dst + m, fmaf(kb, other, ka * tot));
+    if constexpr (DET) dst[m] = fmaf(kb, other, ka * tot);
+    else atomicAdd(dst + m, fmaf(kb, other, ka * tot));
     if constexpr (DEPTH) {
       if (m < 2) {  // lane m = 0: opacity into slot 8, lane m = 1: dL/dz into slot 9
         float rcp;
         asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(s1.y));
-        atomicAdd(dst + 8 + m, m == 0 ? sw * rcp : sz);
+        if constexpr (DET) dst[8 + m] = m == 0 ? sw * rcp : sz;
+        else atomicAdd(dst + 8 + m, m == 0 ? sw * rcp : sz);
       }
     } else if (m == 0) {
       float rcp;  // o >= 1/255 for every staged splat (splat_subblock_mask): __fdividef(sw, o) without its denormal guard
       asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(s1.y));
-      atomicAdd(dst + 8, sw * rcp);
+      if constexpr (DET) dst[8] = sw * rcp;
+      else atomicAdd(dst + 8, sw * rcp);
+    }
+    if constexpr (DET) {
+      if (m == 0) flags[row] = 1;
     }
   }
 }
 
 // BATCHED (variant 15): the per-splat reduction is deferred and batched through shared memory (flush_moments)
 // DEPTH: variant 15 with the depth channel (a.dL_ddepth, tenth moment -> acc slot 9)
-template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false, bool DEPTH = false>
-__global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgsT<DEPTH> a, const int ntiles) {
+// DET: variant 15 (or its DEPTH form) in deterministic mode. Mapping, staging, evaluation, skip decisions and the
+// batched sum are unchanged; the staging lane computes the instance's emission slot and keeps it in sid in place of the
+// Gaussian index, and the flush stores the finished row at that slot instead of adding it to acc.
+template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false, bool DEPTH = false,
+          bool DET = false>
+__global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgsT<DEPTH, DET> a, const int ntiles) {
   static_assert(!BATCHED || (NSB == 4 && SKIP && !MASKSKIP), "the batched reduction is written for variant 15");
   static_assert(!DEPTH || BATCHED, "the depth channel is written for variant 15");
+  static_assert(!DET || BATCHED, "deterministic mode is written for variant 15");
   constexpr int NM = batch_moments<DEPTH>();
   __shared__ float4 s_stage[BW_WARPS][3][32];
   __shared__ uint32_t s_id[BW_WARPS][32];
@@ -480,7 +506,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
 
   for (int hi = (int)my_last; hi > 0; hi -= 32) {
     const int pos = hi - lane;
-    uint32_t mask = 0, id = 0;
+    uint32_t mask = 0, id = 0, ex = 0;
     float4 q0, q1, q2;
     if (pos >= 1) {
       id = a.point_list[range.x + pos - 1];
@@ -489,17 +515,22 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
       q1 = __ldg(r + 1);
       q2 = __ldg(r + 2);
       mask = splat_subblock_mask<NSB>(q0, q1, X0, Y0, part);
+      if constexpr (DET) {  // after the mask: one register less across splat_subblock_mask (no spill at 5 CTAs/SM)
+        if (mask != 0) ex = __ldg(a.excl + id);
+      }
     }
     const uint32_t keep = __ballot_sync(0xffffffffu, mask != 0);
     const int cnt = __popc(keep);
     if (mask != 0) {
       const int slot = __popc(keep & ((1u << lane) - 1u));
+      uint32_t es = 0;  // DET: the instance's emission slot, kept in sid (the flush needs no Gaussian index then)
+      if constexpr (DET) es = emission_slot(ex, q0.x, q0.y, __float_as_int(q2.w), a.gx, a.gy, tx, ty);
       q1.w = __uint_as_float(mask);
       q2.w = __uint_as_float((uint32_t)pos);
       stg[0][slot] = q0;
       stg[1][slot] = q1;
       stg[2][slot] = q2;
-      sid[slot] = id;
+      sid[slot] = DET ? es : id;
     }
     __syncwarp();
     const uint32_t lo = (uint32_t)max(hi - 31, 1);
@@ -583,7 +614,11 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
         jpack = (jpack << 5) | (uint32_t)j;
         if (jpack >= 1u << (5 * BATCH_NB)) {  // all slots filled
           __syncwarp();
-          flush_moments<DEPTH>(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
+          if constexpr (DET)
+            flush_moments<DEPTH, true>(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy, a.rows, a.flags,
+                                       part);
+          else
+            flush_moments<DEPTH>(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
           __syncwarp();  // the next splat overwrites slot 0
           jpack = 1;
           col -= BATCH_NB * NM * BATCH_ROW;
@@ -593,7 +628,11 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
     if constexpr (BATCHED) {
       if (jpack > 1) {  // before the stage is refilled
         __syncwarp();
-        flush_moments<DEPTH>(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
+        if constexpr (DET)
+          flush_moments<DEPTH, true>(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy,
+                                     a.rows, a.flags, part);
+        else
+          flush_moments<DEPTH>(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
         col = reinterpret_cast<float*>(bpart) + lane;
         jpack = 1;
       }
@@ -674,7 +713,7 @@ __global__ void __launch_bounds__(TILE_PIX) render_bwd_cta_kernel(const BwdArgs 
 
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own,
-                      const float* dL_dalpha_img, const float* dL_ddepth) {
+                      const float* dL_dalpha_img, const float* dL_ddepth, const DetWS* det, int P, int64_t R) {
   BwdArgs a;
   a.dL_dalpha_img = dL_dalpha_img;
   a.own_stride = own.stride; a.own_phase = own.phase;
@@ -684,6 +723,28 @@ int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningW
   a.bg = s.bg; a.final_T = im.final_T; a.n_contrib = im.n_contrib; a.dL_dpix = dL_dpix; a.acc = acc;
   const int ntiles = a.gx * own.owned_rows(a.gy);  // tiles this rank walks (all of them when own = {1,0})
   if (ntiles == 0) return GSR_OK;
+  if (det != nullptr) {  // deterministic mode: variant 15 (or its depth form) writes rows, one kernel reduces them
+    if (own.stride != 1) { set_error("render_bwd: deterministic mode is single-GPU only"); return GSR_ERR_INVALID; }
+    int rc = launch_det_prepare(P, R, 2, g, *det, st);
+    if (rc) return rc;
+    const int blocks = (ntiles * 2 + BW_WARPS - 1) / BW_WARPS;
+    // 4 CTAs/SM for both: at 5 (96 registers) the colour-only DET kernel spills 8 bytes, as the depth kernel did 20
+    if (dL_ddepth != nullptr) {
+      BwdDetArgs<BwdDepthArgs> da;
+      static_cast<BwdArgs&>(da) = a;
+      da.dL_ddepth = dL_ddepth;
+      da.excl = det->excl; da.rows = det->rows; da.flags = det->flags;
+      render_bwd_flat_kernel<4, 4, true, false, true, true, true><<<blocks, BW_WARPS * 32, 0, st>>>(da, ntiles);
+    } else {
+      BwdDetArgs<BwdArgs> da;
+      static_cast<BwdArgs&>(da) = a;
+      da.excl = det->excl; da.rows = det->rows; da.flags = det->flags;
+      render_bwd_flat_kernel<4, 4, true, false, true, false, true><<<blocks, BW_WARPS * 32, 0, st>>>(da, ntiles);
+    }
+    g_launches++;
+    if ((rc = check_launch("render_bwd", s.debug != 0, st))) return rc;
+    return launch_det_reduce_acc(P, dL_ddepth != nullptr, g, *det, acc, st);
+  }
   int v = g_opt.render_bwd_variant;
   if (v == 0 && own.stride != 1) v = 4;  // the CTA-per-tile kernel maps blockIdx to tiles directly: single-GPU only
   if (dL_ddepth != nullptr) {  // the depth channel exists only in variant 15, whatever the option says. At 5 CTAs/SM

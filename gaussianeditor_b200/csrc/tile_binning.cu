@@ -47,13 +47,6 @@ uint32_t higher_msb(uint32_t n) {
   return msb;
 }
 
-__device__ __forceinline__ void tile_rect(float px, float py, int radius, int gx, int gy, uint2& rmin, uint2& rmax) {
-  // auxiliary.h:46-56
-  rmin.x = (unsigned)min(gx, max((int)0, (int)((px - radius) / TILE)));
-  rmin.y = (unsigned)min(gy, max((int)0, (int)((py - radius) / TILE)));
-  rmax.x = (unsigned)min(gx, max((int)0, (int)((px + radius + TILE - 1) / TILE)));
-  rmax.y = (unsigned)min(gy, max((int)0, (int)((py + radius + TILE - 1) / TILE)));
-}
 __device__ __forceinline__ void owned_rows(uint32_t ymin, uint32_t ymax, int stride, int phase, uint32_t& y0, uint32_t& ny) {
   if (stride == 1) { y0 = ymin; ny = ymax - ymin; return; }
   int d = (phase - (int)ymin) % stride;

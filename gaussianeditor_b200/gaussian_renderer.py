@@ -63,7 +63,7 @@ def _python_sh_colors(pc, camera_center) -> torch.Tensor:
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           fused_activations: bool = False, depth_grad: bool = False):
+           fused_activations: bool = False, depth_grad: bool = False, deterministic=None):
     """Render the scene; background tensor must be on the GPU. Returns the reference's dictionary:
     render [3,H,W], viewspace_points [P,3] (grad sink for densification), visibility_filter, radii, depth_3dgs.
 
@@ -75,7 +75,11 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     (``pc._opacity, pc._features_dc, pc._features_rest, pc._scaling, pc._rotation``) to the rasterizer, which applies
     sigmoid / exp / normalize and reads the SH row from the two feature arrays inside its preprocess kernels: the
     per-render PyTorch prologue (five elementwise kernels, a [P,16,3] ``torch.cat``) and its autograd epilogue go away.
-    Only valid for the plain SH path (no override colour, no Python-side SH / covariance)."""
+    Only valid for the plain SH path (no override colour, no Python-side SH / covariance).
+
+    ``deterministic`` (opt-in, not in the reference): ``True`` / ``False`` selects the rasterizer's bit-reproducible /
+    default backward; ``None`` (default) leaves the choice to the rasterizer, which follows
+    ``torch.are_deterministic_algorithms_enabled()``."""
     xyz = pc.get_xyz
     # gradient sink for the 2-D means: densification reads its .grad (gaussian_renderer/__init__.py:60-69)
     screenspace_points = torch.zeros_like(xyz, requires_grad=True) + 0
@@ -83,9 +87,11 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         screenspace_points.retain_grad()
     except Exception:
         pass
-    # depth_grad is passed only when asked for: by default the rasterizer is constructed exactly as the reference's
-    # render() does, so any class with the reference's constructor (raster_settings only) can stand in for it
+    # depth_grad / deterministic are passed only when asked for: by default the rasterizer is constructed exactly as the
+    # reference's render() does, so any class with the reference's constructor (raster_settings only) can stand in for it
     opt = {"depth_grad": True} if depth_grad else {}
+    if deterministic is not None:
+        opt["deterministic"] = bool(deterministic)
     rasterizer = GaussianRasterizer(
         raster_settings=_settings_for(viewpoint_camera, bg_color, scaling_modifier, pc.active_sh_degree), **opt)
     python_sh = getattr(pipe, "convert_SHs_python", False)

@@ -209,12 +209,14 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, return_alpha=False, camera_grad=False, depth_grad=False):
+                        raster_settings, return_alpha=False, camera_grad=False, depth_grad=False, deterministic=False):
     rs = raster_settings
-    if depth_grad:    # the depth output's gradient is used (gsr_backward_depth); without it, it is dropped as in the reference
+    if depth_grad or deterministic:
+        # depth_grad: the depth output's gradient is used (gsr_backward_depth); without it, it is dropped as in the
+        # reference. deterministic: bit-reproducible backward (gsr_backward_deterministic).
         cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if camera_grad else (None, None, None)
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                         cov3Ds_precomp, rs, return_alpha, *cam, True)
+                                         cov3Ds_precomp, rs, return_alpha, *cam, bool(depth_grad), bool(deterministic))
     if camera_grad:   # the camera arrays become autograd inputs of the node (they are read from the settings as usual)
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                          cov3Ds_precomp, rs, return_alpha, rs.viewmatrix, rs.projmatrix, rs.campos)
@@ -235,12 +237,15 @@ def _alpha_image(lib, state, device):
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, return_alpha=False, viewmatrix=None, projmatrix=None, campos=None, depth_grad=False):
+                raster_settings, return_alpha=False, viewmatrix=None, projmatrix=None, campos=None, depth_grad=False,
+                deterministic=None):
         color, depth, state, inputs = _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations,
                                                     cov3Ds_precomp, raster_settings)
         ctx.raster_settings = raster_settings
         ctx.camera_grad = viewmatrix is not None
         ctx.depth_grad = bool(depth_grad)
+        ctx.long_form = deterministic is not None   # called with depth_grad and deterministic given
+        ctx.deterministic = bool(deterministic)
         ctx.n_inputs = 10 + (3 if ctx.camera_grad else 0)
         if ctx.depth_grad:
             # outputs without a gradient arrive as None: no depth gradient -> the ordinary backward, and a loss on the
@@ -282,7 +287,26 @@ class _RasterizeGaussians(torch.autograd.Function):
                 gr = _lib.Grads(_ptr(dL_dmeans3D), _ptr(dL_dmeans2D), _ptr(dL_dcolors), _ptr(dL_dopacity),
                                 _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations))
                 st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-                if ctx.depth_grad and grad_depth is not None:
+                if ctx.deterministic:   # one entry point for every combination of alpha, camera and depth gradients
+                    gd = _f32c(grad_depth, device) if ctx.depth_grad and grad_depth is not None else None
+                    ga = None if grad_alpha is None else _f32c(grad_alpha, device)
+                    cam = None
+                    if ctx.camera_grad:
+                        d_view = torch.empty(16, **f32); d_proj = torch.empty(16, **f32); d_cam = torch.empty(3, **f32)
+                        cbytes = lib.gsr_camera_scratch_bytes(P)
+                        cscratch = torch.empty(cbytes, dtype=torch.uint8, device=device)
+                        cam = _lib.CameraGrads(_ptr(d_view), _ptr(d_proj), _ptr(d_cam), _ptr(cscratch), cbytes)
+                        cam_grads = (d_view.view(rs.viewmatrix.shape), d_proj.view(rs.projmatrix.shape),
+                                     d_cam.view(rs.campos.shape))
+                    dbytes = lib.gsr_deterministic_scratch_bytes(P, state.cap, 0)
+                    dscratch = torch.empty(dbytes, dtype=torch.uint8, device=device)
+                    _lib.check(lib.gsr_backward_deterministic(C.byref(s), C.byref(c), state.cap, _ptr(geom), geom.numel(),
+                                                              _ptr(binning), binning.numel(), _ptr(img), img.numel(),
+                                                              _ptr(radii), _ptr(grad_out_color), _ptr(ga), _ptr(gd),
+                                                              _ptr(scratch), sbytes, C.byref(gr),
+                                                              None if cam is None else C.byref(cam), _ptr(dscratch),
+                                                              dbytes, st), "gsr_backward_deterministic")
+                elif ctx.depth_grad and grad_depth is not None:
                     gd = _f32c(grad_depth, device)
                     ga = None if grad_alpha is None else _f32c(grad_alpha, device)
                     cam = None
@@ -331,8 +355,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                 z = lambda t: torch.zeros_like(t, dtype=torch.float32)
                 cam_grads = (z(rs.viewmatrix), z(rs.projmatrix), z(rs.campos))
             grads = grads + cam_grads
-        if ctx.depth_grad:
-            grads = grads + ((None, None, None) if not ctx.camera_grad else ()) + (None,)
+        if ctx.long_form:   # depth_grad, deterministic
+            grads = grads + ((None, None, None) if not ctx.camera_grad else ()) + (None, None)
         return grads
 
 
@@ -342,13 +366,15 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
-                raster_settings, depth_grad=False):
+                raster_settings, depth_grad=False, deterministic=None):
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         color, depth, state, inputs = _forward_impl(means3D, features_dc, empty, opacity_logits, log_scales,
                                                     raw_rotations, empty, raster_settings, raw_rest=features_rest)
         ctx.raster_settings = raster_settings
         ctx.state = state
         ctx.depth_grad = bool(depth_grad)
+        ctx.long_form = deterministic is not None   # called with depth_grad and deterministic given
+        ctx.deterministic = bool(deterministic)
         if ctx.depth_grad:   # as _RasterizeGaussians: None = no gradient for that output
             ctx.set_materialize_grads(False)
         (m3, dc, _, op, sc, ro, _, rest) = inputs
@@ -380,7 +406,17 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                 sbytes = lib.gsr_backward_scratch_bytes(P)
                 scratch = torch.empty(sbytes, dtype=torch.uint8, device=device)
                 st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-                if ctx.depth_grad and grad_depth is not None:
+                if ctx.deterministic:
+                    gd = _f32c(grad_depth, device) if ctx.depth_grad and grad_depth is not None else None
+                    dbytes = lib.gsr_deterministic_scratch_bytes(P, state.cap, 0)
+                    dscratch = torch.empty(dbytes, dtype=torch.uint8, device=device)
+                    _lib.check(lib.gsr_backward_raw_deterministic(C.byref(s), C.byref(rc), state.cap, _ptr(geom),
+                                                                  geom.numel(), _ptr(binning), binning.numel(), _ptr(img),
+                                                                  img.numel(), _ptr(radii), _ptr(grad_out_color),
+                                                                  _ptr(gd), _ptr(scratch), sbytes, C.byref(gr),
+                                                                  _ptr(dscratch), dbytes, st),
+                               "gsr_backward_raw_deterministic")
+                elif ctx.depth_grad and grad_depth is not None:
                     gd = _f32c(grad_depth, device)
                     _lib.check(lib.gsr_backward_raw_depth(C.byref(s), C.byref(rc), state.cap, _ptr(geom), geom.numel(),
                                                           _ptr(binning), binning.numel(), _ptr(img), img.numel(),
@@ -391,13 +427,16 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                                                     _ptr(binning), binning.numel(), _ptr(img), img.numel(), _ptr(radii),
                                                     _ptr(grad_out_color), _ptr(scratch), sbytes, C.byref(gr), st),
                                "gsr_backward_raw")
+        if ctx.long_form:   # depth_grad, deterministic
+            return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None
         if ctx.depth_grad:
             return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None
         return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None
 
 
 class GaussianRasterizer(nn.Module):
-    def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False):
+    def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False,
+                 deterministic=None):
         """``return_alpha=True`` (opt-in, not in the reference) appends a fourth output to ``forward``: the alpha image
         ``1 - final_T`` [1,H,W] (the reference keeps final_T as ``accum_alpha`` but never returns it); it is
         differentiable like the colour.
@@ -406,20 +445,33 @@ class GaussianRasterizer(nn.Module):
         independent input exactly as the forward reads it.
         ``depth_grad=True`` (opt-in, for ``forward`` and ``forward_raw``): the depth output becomes differentiable
         (gsr_backward_depth). By default its gradient is dropped, as in the reference. When the depth receives no
-        gradient the ordinary backward runs; a loss on the depth alone works too."""
+        gradient the ordinary backward runs; a loss on the depth alone works too.
+        ``deterministic`` (for ``forward``, ``forward_raw`` and ``apply_weights``): ``True`` computes the backward and
+        ``apply_weights`` without float atomics (gsr_backward_deterministic), so two calls on the same inputs give the
+        same bits; ``False`` keeps the faster default. ``None`` (default) follows
+        ``torch.are_deterministic_algorithms_enabled()`` at the time of the call, so ``torch.use_deterministic_algorithms
+        (True)`` (Lightning's ``trainer.deterministic=true``) selects it without other changes. Forward outputs are the
+        same in both modes."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_alpha = bool(return_alpha)
         self.camera_grad = bool(camera_grad)
         self.depth_grad = bool(depth_grad)
+        self.deterministic = None if deterministic is None else bool(deterministic)
+
+    def _deterministic(self) -> bool:
+        if self.deterministic is None:
+            return torch.are_deterministic_algorithms_enabled()
+        return self.deterministic
 
     def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations):
         """Opt-in fused-activation call (not part of the reference API): the arguments are the scene model's raw
         parameters (``_xyz, _opacity, _features_dc, _features_rest, _scaling, _rotation``); sigmoid / exp / normalize
         and the SH concatenation happen inside the preprocess kernels. Same return tuple as ``forward``."""
-        if self.depth_grad:
+        det = self._deterministic()
+        if self.depth_grad or det:
             return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
-                                                raw_rotations, self.raster_settings, True)
+                                                raw_rotations, self.raster_settings, self.depth_grad, det)
         return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
                                             raw_rotations, self.raster_settings)
 
@@ -465,7 +517,8 @@ class GaussianRasterizer(nn.Module):
             cov3D_precomp = empty
 
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                   cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad, self.depth_grad)
+                                   cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad, self.depth_grad,
+                                   self._deterministic())
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):
@@ -483,6 +536,7 @@ class GaussianRasterizer(nn.Module):
         if not (cnt.is_cuda and cnt.dtype == torch.int32 and cnt.is_contiguous()):
             raise RuntimeError("cnt must be a contiguous int32 CUDA tensor (it is updated in place)")
         CH = int(image_weights.size(0))
+        det = self._deterministic()
         with torch.no_grad():
             # the reference passes `weights` in the colors_precomp slot (rasterize_points.cu:223), so SH
             # evaluation is skipped; the forward's colours are never used
@@ -500,6 +554,15 @@ class GaussianRasterizer(nn.Module):
                 c = _make_cloud(state.P, m3, op_, sh_, cp_, sc_, ro_, cv_)
                 iw = _f32c(image_weights, device)
                 st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+                if det:   # bit-identical weights on every call (gsr_apply_weights_deterministic)
+                    dbytes = lib.gsr_deterministic_scratch_bytes(state.P, state.num_rendered, CH)
+                    dscratch = torch.empty(dbytes, dtype=torch.uint8, device=device)
+                    _lib.check(lib.gsr_apply_weights_deterministic(
+                        C.byref(s), C.byref(c), state.num_rendered, _ptr(state.geom), state.geom.numel(),
+                        _ptr(state.binning), state.binning.numel(), _ptr(state.img), state.img.numel(), _ptr(state.radii),
+                        _ptr(iw), CH, _ptr(weights), _ptr(cnt), _ptr(dscratch), dbytes, st),
+                        "gsr_apply_weights_deterministic")
+                    return
                 _lib.check(lib.gsr_apply_weights(C.byref(s), C.byref(c), state.num_rendered, _ptr(state.geom),
                                                  state.geom.numel(), _ptr(state.binning), state.binning.numel(),
                                                  _ptr(state.img), state.img.numel(), _ptr(state.radii), _ptr(iw), CH,

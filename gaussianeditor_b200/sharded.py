@@ -25,6 +25,7 @@ from __future__ import annotations
 
 import ctypes as C
 import weakref
+import warnings
 from typing import NamedTuple, Optional
 
 import torch
@@ -464,6 +465,21 @@ def p2p_available(exchange: "Exchange") -> bool:
     return bool(int(flag[0]))
 
 
+def _check_deterministic_flag():
+    """The sharded backward adds gradient rows with float atomics, whose order changes from call to call. Under
+    ``torch.use_deterministic_algorithms(True)`` that is an error (a warning with ``warn_only=True``), as for any PyTorch op
+    without a deterministic implementation; the single-GPU ``GaussianRasterizer`` has one."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = ("ShardedGaussianRasterizer does not have a deterministic implementation: its backward adds gradients with "
+           "float atomics. Use the single-GPU GaussianRasterizer (deterministic mode) or turn the flag off with "
+           "torch.use_deterministic_algorithms(False).")
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
+
+
 class ShardedGaussianRasterizer(nn.Module):
     """``GaussianRasterizer`` for a cloud sharded by Gaussian index over the ranks of a process group.
 
@@ -513,6 +529,7 @@ class ShardedGaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
+        _check_deterministic_flag()
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
         if ((scales is None or rotations is None) and cov3D_precomp is None) or (

@@ -194,6 +194,28 @@ GSR_API int gsr_backward_depth(const gsr_settings* s, const gsr_cloud* c, int32_
                        size_t scratch_bytes, const gsr_grads* grads, const gsr_camera_grads* camera /* may be NULL */,
                        void* stream);
 
+/* ---- deterministic mode (opt-in; bit-reproducible gradients and apply_weights) ---------------------------
+ * The default blending backward and apply_weights add per-Gaussian partial sums with float atomics, so their results
+ * change in the last bits from call to call. The *_deterministic entry points compute the same quantities without
+ * float atomics: each (instance, tile half) -- each instance for apply_weights -- stores its partial sum as a row at
+ * the instance's position in the binning's emission order, and one kernel adds every Gaussian's rows in a fixed
+ * order. Two calls on the same inputs give the same bits; the values differ from the default path only in the order
+ * of the fp32 sums. Forward outputs are the same in both modes.
+ * det_scratch: at least gsr_deterministic_scratch_bytes(P, num_rendered, num_channels) bytes (num_channels: the CH
+ * of apply_weights, 0 for the backward), device memory, contents irrelevant (nothing of it needs clearing).
+ * gsr_backward_deterministic takes the arguments of gsr_backward_depth, with dL_dout_depth allowed to be NULL (no
+ * depth gradient), so it covers the plain, alpha, camera and depth combinations; gsr_backward_raw_deterministic is
+ * the same for gsr_backward_raw_depth (fused activations, below). cnt of apply_weights is integer and was already
+ * exact. Single-GPU only: the Gaussian-sharded entry points keep their atomics. */
+GSR_API size_t gsr_deterministic_scratch_bytes(int32_t P, int64_t num_rendered, int32_t num_channels);
+GSR_API int gsr_backward_deterministic(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered,
+                               const void* geometry, size_t geometry_bytes, const void* binning,
+                               size_t binning_bytes, const void* image, size_t image_bytes, const int32_t* radii,
+                               const float* dL_dout_color, const float* dL_dout_alpha /* may be NULL */,
+                               const float* dL_dout_depth /* may be NULL */, void* scratch, size_t scratch_bytes,
+                               const gsr_grads* grads, const gsr_camera_grads* camera /* may be NULL */,
+                               void* det_scratch, size_t det_scratch_bytes, void* stream);
+
 /* ---- markVisible: present[i] = view-space z > 0.2 (auxiliary.h:139-164) ------------------------------- */
 GSR_API int gsr_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);
@@ -207,6 +229,12 @@ GSR_API int gsr_apply_weights(const gsr_settings* s, const gsr_cloud* c, int32_t
                       size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
                       const int32_t* radii, const float* image_weights, int32_t num_channels, float* weights,
                       int32_t* cnt, void* stream);
+/* gsr_apply_weights in deterministic mode (see gsr_backward_deterministic): bit-identical weights on every call. */
+GSR_API int gsr_apply_weights_deterministic(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered,
+                                    void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes,
+                                    void* image, size_t image_bytes, const int32_t* radii,
+                                    const float* image_weights, int32_t num_channels, float* weights, int32_t* cnt,
+                                    void* det_scratch, size_t det_scratch_bytes, void* stream);
 
 /* ---- introspection for parity tests: device pointers into the opaque workspaces ----------------------- */
 typedef struct gsr_geometry_view {
@@ -270,6 +298,13 @@ GSR_API int gsr_backward_raw_depth(const gsr_settings* s, const gsr_raw_cloud* c
                            const void* image, size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
                            const float* dL_dout_depth, void* scratch, size_t scratch_bytes, const gsr_raw_grads* grads,
                            void* stream);
+/* gsr_backward_raw_depth in deterministic mode (see gsr_backward_deterministic); dL_dout_depth may be NULL. */
+GSR_API int gsr_backward_raw_deterministic(const gsr_settings* s, const gsr_raw_cloud* c, int32_t num_rendered,
+                                   const void* geometry, size_t geometry_bytes, const void* binning,
+                                   size_t binning_bytes, const void* image, size_t image_bytes, const int32_t* radii,
+                                   const float* dL_dout_color, const float* dL_dout_depth /* may be NULL */,
+                                   void* scratch, size_t scratch_bytes, const gsr_raw_grads* grads, void* det_scratch,
+                                   size_t det_scratch_bytes, void* stream);
 
 /* ---- Gaussian-sharded multi-GPU path (BASELINE config 4; SURVEY.md 8(e)) ----------------------------------
  * The reference has no multi-GPU rasterizer; these entry points split the single-GPU pipeline at the two places
