@@ -31,6 +31,7 @@ SYMBOLS = [
     "gsr_backward_depth", "gsr_backward_raw_depth",
     "gsr_deterministic_scratch_bytes", "gsr_backward_deterministic", "gsr_backward_raw_deterministic",
     "gsr_apply_weights_deterministic",
+    "gsr_shard_apply_weights", "gsr_sparse_apply_weights_gather",
 ]
 
 
@@ -192,6 +193,8 @@ def load():
     lib.gsr_shard_backward_render.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, sz, vp]
     lib.gsr_shard_backward_preprocess.restype = C.c_int
     lib.gsr_shard_backward_preprocess.argtypes = [S, Cl, i32, i32, vp, sz, vp, vp, C.POINTER(Grads), vp]
+    lib.gsr_shard_apply_weights.restype = C.c_int
+    lib.gsr_shard_apply_weights.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, i32, vp, i64, vp, i64, vp]
     lib.gsr_peer_alloc.restype = C.c_int; lib.gsr_peer_alloc.argtypes = [sz, C.POINTER(vp), vp]
     lib.gsr_peer_open.restype = C.c_int; lib.gsr_peer_open.argtypes = [vp, C.POINTER(vp)]
     lib.gsr_peer_close.restype = C.c_int; lib.gsr_peer_close.argtypes = [vp]
@@ -221,6 +224,8 @@ def load():
     lib.gsr_sparse_return.argtypes = [SP, vp, vp, C.POINTER(vp), vp]
     lib.gsr_sparse_backward_preprocess.restype = C.c_int
     lib.gsr_sparse_backward_preprocess.argtypes = [S, Cl, SP, vp, sz, vp, vp, sz, vp, sz, C.POINTER(Grads), vp]
+    lib.gsr_sparse_apply_weights_gather.restype = C.c_int
+    lib.gsr_sparse_apply_weights_gather.argtypes = [SP, vp, sz, vp, sz, i32, i32, vp, vp, vp]
     lib.gsr_peer_barrier.restype = C.c_int
     lib.gsr_peer_barrier.argtypes = [i32, i32, C.POINTER(vp), C.c_uint32, i32, vp]
     lib.gsr_frame_broadcast.restype = C.c_int

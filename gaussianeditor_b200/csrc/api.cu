@@ -687,6 +687,39 @@ int gsr_shard_backward_render(const gsr_settings* s, const gsr_tile_owner* owner
   return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own);
 }
 
+int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                            void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                            size_t image_bytes, const int32_t* radii_total, const float* image_weights, int32_t CH,
+                            float* weights_total, int64_t weights_stride, int32_t* cnt_total, int64_t cnt_stride,
+                            void* stream) {
+  int rc = check_settings(s);
+  if (rc) return rc;
+  TileOwner own;
+  rc = check_owner(owner, own);
+  if (rc) return rc;
+  if (CH < 1 || CH > 3) { set_error("shard_apply_weights: num_channels %d outside 1..3", CH); return GSR_ERR_INVALID; }
+  if (P_total <= 0 || R < 0 || !radii_total || !image_weights || !weights_total || !cnt_total) {
+    set_error("shard_apply_weights: bad arguments");
+    return GSR_ERR_INVALID;
+  }
+  if (weights_stride < CH || cnt_stride < 1) {
+    set_error("shard_apply_weights: need weights_stride >= num_channels and cnt_stride >= 1");
+    return GSR_ERR_INVALID;
+  }
+  if (R == 0) return GSR_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  gsr_cloud c{};
+  c.P = P_total;
+  GeometryWS g; BinningWS b; ImageWS im;
+  rc = carve_all(s, &c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, g, b, im);
+  if (rc) return rc;
+  rc = run_binning(*s, c, R, false, g, b, im, radii_total, st, own);
+  if (rc) return rc;
+  StageScope t(ST_APPLY_W, st);
+  return launch_apply_weights_owner(*s, g, b, im, image_weights, CH, weights_total, weights_stride, cnt_total, cnt_stride,
+                                    own, st);
+}
+
 int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
                                   const void* geometry, size_t geometry_bytes, const int32_t* radii_total,
                                   const void* acc_slice, const gsr_grads* gr, void* stream) {

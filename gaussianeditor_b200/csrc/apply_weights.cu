@@ -24,14 +24,16 @@ struct AwArgs {
   int32_t* cnt;
 };
 
+// The walk of tile (blockIdx.x, ty). Splat id's hits go to weights[id*w_stride + ch] and cnt[id*c_stride].
 template <int CH>
-__global__ void __launch_bounds__(TILE_PIX) apply_weights_kernel(const AwArgs a) {
+__device__ __forceinline__ void apply_weights_walk(const AwArgs& a, const unsigned ty, const size_t w_stride,
+                                                   const size_t c_stride) {
   __shared__ float4 s_q0[TILE_PIX], s_q1[TILE_PIX];
   __shared__ uint32_t s_ids[TILE_PIX];
-  const int tile = blockIdx.y * a.gx + blockIdx.x;
+  const int tile = ty * a.gx + blockIdx.x;
   const int tid = threadIdx.y * TILE + threadIdx.x;
   const int lane = tid & 31;
-  const uint2 pix = make_uint2(blockIdx.x * TILE + threadIdx.x, blockIdx.y * TILE + threadIdx.y);
+  const uint2 pix = make_uint2(blockIdx.x * TILE + threadIdx.x, ty * TILE + threadIdx.y);
   const bool inside = pix.x < (unsigned)a.W && pix.y < (unsigned)a.H;
   const size_t pix_id = (size_t)a.W * pix.y + pix.x;
   const float2 pixf = make_float2((float)pix.x, (float)pix.y);
@@ -84,12 +86,29 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_kernel(const AwArgs a)
           float v = hit ? Cw[ch] : 0.f;
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-          if (lane == 0) atomicAdd(a.weights + (size_t)id * CH + ch, v);
+          if (lane == 0) atomicAdd(a.weights + (size_t)id * w_stride + ch, v);
         }
-        if (lane == 0) atomicAdd(a.cnt + id, CH * __popc(hits));
+        if (lane == 0) atomicAdd(a.cnt + (size_t)id * c_stride, CH * __popc(hits));
       }
     }
   }
+}
+
+template <int CH>
+__global__ void __launch_bounds__(TILE_PIX) apply_weights_kernel(const AwArgs a) {
+  apply_weights_walk<CH>(a, blockIdx.y, CH, 1);
+}
+
+// Gaussian-sharded path: blockIdx.y = k-th owned tile row (ty = own_phase + k*own_stride), and strided outputs so that
+// the same walk fills a dense [P, CH] + [P] pair or the [M, 12] rows of the sparse return (cnt as int32 bits in a slot).
+struct AwOwnerArgs : AwArgs {
+  int own_stride, own_phase;
+  int64_t w_stride, c_stride;
+};
+
+template <int CH>
+__global__ void __launch_bounds__(TILE_PIX) apply_weights_owner_kernel(const AwOwnerArgs a) {
+  apply_weights_walk<CH>(a, a.own_phase + blockIdx.y * a.own_stride, a.w_stride, a.c_stride);
 }
 
 
@@ -230,6 +249,29 @@ int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const Binni
   if (CH == 1) apply_weights_kernel<1><<<grid, block, 0, st>>>(a);
   else if (CH == 2) apply_weights_kernel<2><<<grid, block, 0, st>>>(a);
   else if (CH == 3) apply_weights_kernel<3><<<grid, block, 0, st>>>(a);
+  else {
+    set_error("apply_weights: unsupported number of channels %d (reference supports 1..3, apply_weights.cu:365-380)", CH);
+    return GSR_ERR_INVALID;
+  }
+  g_launches++;
+  return check_launch("apply_weights", s.debug != 0, st);
+}
+
+int launch_apply_weights_owner(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
+                               const float* image_weights, int CH, float* weights, int64_t w_stride, int32_t* cnt,
+                               int64_t c_stride, const TileOwner& own, cudaStream_t st) {
+  AwOwnerArgs a;
+  a.ranges = im.ranges; a.point_list = b.point_list; a.records = g.records;
+  a.W = s.image_width; a.H = s.image_height;
+  a.gx = (a.W + TILE - 1) / TILE; a.gy = (a.H + TILE - 1) / TILE;
+  a.image_weights = image_weights; a.weights = weights; a.cnt = cnt;
+  a.own_stride = own.stride; a.own_phase = own.phase; a.w_stride = w_stride; a.c_stride = c_stride;
+  const int rows = own.owned_rows(a.gy);
+  if (a.gx * rows == 0) return GSR_OK;
+  dim3 grid(a.gx, rows), block(TILE, TILE);
+  if (CH == 1) apply_weights_owner_kernel<1><<<grid, block, 0, st>>>(a);
+  else if (CH == 2) apply_weights_owner_kernel<2><<<grid, block, 0, st>>>(a);
+  else if (CH == 3) apply_weights_owner_kernel<3><<<grid, block, 0, st>>>(a);
   else {
     set_error("apply_weights: unsupported number of channels %d (reference supports 1..3, apply_weights.cu:365-380)", CH);
     return GSR_ERR_INVALID;

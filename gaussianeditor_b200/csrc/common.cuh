@@ -211,6 +211,10 @@ int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, ui
 int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                          const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st,
                          const DetWS* det = nullptr, int P = 0, int64_t R = 0);
+// sharded path: the walk of the owned tiles only; splat id adds to weights[id*w_stride + ch] and cnt[id*c_stride]
+int launch_apply_weights_owner(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
+                               const float* image_weights, int CH, float* weights, int64_t w_stride, int32_t* cnt,
+                               int64_t c_stride, const TileOwner& own, cudaStream_t st);
 
 // ---- host + device helpers ----------------------------------------------------------------------------
 // The per-pixel hit test and the sub-block culling predicate compile for the host too (oracle/subblock_check.cpp

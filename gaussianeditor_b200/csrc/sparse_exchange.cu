@@ -358,6 +358,36 @@ sparse_gather_kernel(int n, int world, int cap, const uint8_t* __restrict__ dest
   o[0] = a0; o[1] = a1; o[2] = a2;
 }
 
+// semantic tracing: weights[i, ch] += and cnt[i] += the returned rows of Gaussian i (same slots and order as above); the
+// count travels as int32 bits in slot GSR_SPARSE_AW_CNT_SLOT of the row
+static_assert(GSR_SPARSE_AW_CNT_SLOT >= 3 && GSR_SPARSE_AW_CNT_SLOT < ACC_STRIDE, "count slot");
+__global__ void __launch_bounds__(SP_THREADS)
+sparse_aw_gather_kernel(int n, int world, int cap, int CH, const uint8_t* __restrict__ dest_mask,
+                        const uint32_t* __restrict__ blk_base, const float* __restrict__ ret, float* __restrict__ weights,
+                        int32_t* __restrict__ cnt) {
+  __shared__ uint32_t s_cnt[SP_THREADS / 32][GSR_MAX_PEERS];
+  const int idx = blockIdx.x * SP_THREADS + threadIdx.x;
+  const uint32_t m = idx < n ? dest_mask[idx] : 0u;
+  uint32_t slot[GSR_MAX_PEERS];
+  sparse_slots(m, world, blk_base, slot, s_cnt);
+  if (idx >= n || m == 0) return;
+  float w0 = 0.f, w1 = 0.f, w2 = 0.f;
+  int32_t c = 0;
+#pragma unroll
+  for (int d = 0; d < GSR_MAX_PEERS; d++) {
+    if (!((m >> d) & 1u) || slot[d] >= (uint32_t)cap) continue;
+    const float* p = ret + ((size_t)d * cap + slot[d]) * ACC_STRIDE;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(p));
+    w0 += v.x; w1 += v.y; w2 += v.z;
+    c += __float_as_int(__ldg(p + GSR_SPARSE_AW_CNT_SLOT));
+  }
+  float* w = weights + (size_t)idx * CH;
+  w[0] += w0;
+  if (CH > 1) w[1] += w1;
+  if (CH > 2) w[2] += w2;
+  cnt[idx] += c;
+}
+
 // ---- frame broadcast: owned tile rows of the [4,H,W] frame -> every rank's frame ----------------------------------
 struct FrameArgs {
   int W, H, gy, world, me, nrows;  // nrows = owned tile rows
@@ -590,6 +620,32 @@ int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard
   rc = check_launch("sparse_gather", s->debug != 0, st);
   if (rc) return rc;
   return launch_preprocess_bwd(*s, *shard, g, radii_local, (const float*)acc_slice, *gr, st);
+}
+
+int gsr_sparse_apply_weights_gather(const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                    const void* cand_ws, size_t cand_bytes, int32_t n, int32_t CH, float* weights,
+                                    int32_t* cnt, void* stream) {
+  int rc = check_plan(plan);
+  if (rc) return rc;
+  if (CH < 1 || CH > 3) { set_error("sparse_apply_weights_gather: num_channels %d outside 1..3", CH); return GSR_ERR_INVALID; }
+  if (n < 0 || n > plan->slice_len) { set_error("sparse_apply_weights_gather: n = %d does not fit slice_len", n); return GSR_ERR_INVALID; }
+  if (!local_ws || !cand_ws || !weights || !cnt) { set_error("sparse_apply_weights_gather: null argument"); return GSR_ERR_INVALID; }
+  if (n == 0) return GSR_OK;
+  GeometryWS g;
+  if (!carve_geometry(const_cast<void*>(local_ws), plan->slice_len, g)) return GSR_ERR_CUDA;
+  SparseLocal sl;
+  carve_sparse_local(const_cast<void*>(local_ws), plan->slice_len, g, sl);
+  if (sl.total > local_bytes) { set_error("local workspace too small: %zu < %zu", local_bytes, sl.total); return GSR_ERR_WORKSPACE; }
+  SparseCand sc;
+  if (!carve_sparse_cand(const_cast<void*>(cand_ws), plan->world, plan->seg_cap, sc)) return GSR_ERR_CUDA;
+  if (sc.total > cand_bytes) { set_error("candidate workspace too small: %zu < %zu", cand_bytes, sc.total); return GSR_ERR_WORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  StageScope t(ST_APPLY_W, st);
+  sparse_aw_gather_kernel<<<(n + SP_THREADS - 1) / SP_THREADS, SP_THREADS, 0, st>>>(n, plan->world, plan->seg_cap, CH,
+                                                                                    sl.dest_mask, sl.blk_base, sc.ret,
+                                                                                    weights, cnt);
+  g_launches++;
+  return check_launch("sparse_apply_weights_gather", false, st);
 }
 
 int gsr_sparse_view(void* cand_ws, int32_t world, int32_t seg_cap, gsr_sparse_view_t* out) {

@@ -434,6 +434,24 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
         return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None
 
 
+def mark_visible(rs, positions):
+    """Frustum test of `positions` [P,3] under the camera of `rs` -> bool [P] (GaussianRasterizer.markVisible)."""
+    # __init__.py:248-256 / rasterize_points.cu:159-175
+    lib = _lib.load()
+    with torch.no_grad():
+        device = positions.device
+        positions = _f32c(positions, device)
+        P = positions.size(0)
+        visible = torch.zeros(P, dtype=torch.bool, device=device)
+        if P > 0:
+            with torch.cuda.device(device):
+                view = _f32c(rs.viewmatrix, device); proj = _f32c(rs.projmatrix, device)
+                st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+                _lib.check(lib.gsr_mark_visible(P, _ptr(positions), _ptr(view), _ptr(proj), _ptr(visible), st),
+                           "gsr_mark_visible")
+    return visible
+
+
 class GaussianRasterizer(nn.Module):
     def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False,
                  deterministic=None):
@@ -476,21 +494,7 @@ class GaussianRasterizer(nn.Module):
                                             raw_rotations, self.raster_settings)
 
     def markVisible(self, positions):
-        # __init__.py:248-256 / rasterize_points.cu:159-175
-        lib = _lib.load()
-        with torch.no_grad():
-            rs = self.raster_settings
-            device = positions.device
-            positions = _f32c(positions, device)
-            P = positions.size(0)
-            visible = torch.zeros(P, dtype=torch.bool, device=device)
-            if P > 0:
-                with torch.cuda.device(device):
-                    view = _f32c(rs.viewmatrix, device); proj = _f32c(rs.projmatrix, device)
-                    st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-                    _lib.check(lib.gsr_mark_visible(P, _ptr(positions), _ptr(view), _ptr(proj), _ptr(visible), st),
-                               "gsr_mark_visible")
-        return visible
+        return mark_visible(self.raster_settings, positions)
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):

@@ -33,7 +33,7 @@ import torch.nn as nn
 
 from . import _lib
 from .rasterizer import (GaussianRasterizationSettings, _f32c, _geometry_bytes, _make_cloud, _make_settings,
-                         _pinned_i32, _ptr)
+                         _pinned_i32, _ptr, mark_visible)
 
 ACC_STRIDE = 12  # floats per Gaussian in the 2-D gradient accumulators (csrc/common.cuh)
 
@@ -408,6 +408,97 @@ def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor):
     return (dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D)
 
 
+def owner_apply_weights(s, own, P: int, R: int, geom: torch.Tensor, radii: torch.Tensor, image_weights: torch.Tensor,
+                        weights: torch.Tensor, w_stride: int, cnt: torch.Tensor, c_stride: int, get):
+    """gsr_shard_apply_weights: bin + walk the owned tiles of a P-record workspace `geom` (after the order stage),
+    adding the hits of record i to weights[i*w_stride + ch] and cnt[i*c_stride]. `get(name, numel, dtype, grow)`
+    supplies the binning and image scratch, sized from the settings `s` (not from a frame size fixed elsewhere)."""
+    lib = _lib.load()
+    device = geom.device
+    W, H = int(s.image_width), int(s.image_height)
+    CH = int(image_weights.size(0))
+    with torch.cuda.device(device):
+        bbytes = lib.gsr_binning_bytes(P, R, W, H) if R > 0 else 0
+        binning = get("binning", bbytes, torch.uint8, 1.25)
+        ibytes = lib.gsr_image_bytes(W, H)
+        img = get("img", ibytes, torch.uint8, 1.0)
+        st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(lib.gsr_shard_apply_weights(C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning),
+                                               bbytes, _ptr(img), ibytes, _ptr(radii), _ptr(image_weights), CH,
+                                               _ptr(weights), w_stride, _ptr(cnt), c_stride, st),
+                   "gsr_shard_apply_weights")
+
+
+def shard_apply_weights(buf: ShardBuffers, image_weights: torch.Tensor, weights_total: torch.Tensor,
+                        cnt_total: torch.Tensor):
+    """Semantic tracing of the owned tiles (after shard_order): adds into `weights_total` [P_pad, CH] float32 and
+    `cnt_total` [P_pad] int32, indexed by global Gaussian index (the caller zero-fills them)."""
+    device = buf.geom.device
+    owner_apply_weights(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.radii, _f32c(image_weights, device),
+                        weights_total, int(image_weights.size(0)), cnt_total, 1,
+                        lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow))
+
+
+def check_apply_weights_args(plan: ShardPlan, rs, means3D, weights, cnt, image_weights, scales, rotations,
+                             cov3Ds_precomp) -> int:
+    """The argument checks of ShardedGaussianRasterizer.apply_weights (this rank's rows), all made before any collective
+    so that a bad argument raises here instead of leaving the peers waiting. Returns CH."""
+    assert weights is not None
+    assert cnt is not None
+    assert image_weights is not None
+    if ((scales is None or rotations is None) and cov3Ds_precomp is None) or (
+            (scales is not None or rotations is not None) and cov3Ds_precomp is not None):
+        raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
+    if not means3D.is_cuda:
+        raise RuntimeError("the rasterizer needs CUDA tensors (there is no CPU path)")
+    if means3D.size(0) != plan.count:
+        raise RuntimeError(f"rank {plan.rank} owns {plan.count} Gaussians, got {means3D.size(0)}")
+    if not (weights.is_cuda and weights.dtype == torch.float32 and weights.is_contiguous()):
+        raise RuntimeError("weights must be a contiguous float32 CUDA tensor (it is updated in place)")
+    if not (cnt.is_cuda and cnt.dtype == torch.int32 and cnt.is_contiguous()):
+        raise RuntimeError("cnt must be a contiguous int32 CUDA tensor (it is updated in place)")
+    H, W = int(rs.image_height), int(rs.image_width)
+    if image_weights.dim() != 3 or not 1 <= image_weights.size(0) <= 3 or tuple(image_weights.shape[1:]) != (H, W):
+        raise RuntimeError(f"image_weights must be [CH, {H}, {W}] with CH in 1..3, got {tuple(image_weights.shape)}")
+    CH = int(image_weights.size(0))
+    if weights.numel() != plan.count * CH or (weights.dim() > 0 and weights.size(0) != plan.count):
+        raise RuntimeError(f"weights must be this rank's [{plan.count}, {CH}] rows, got {tuple(weights.shape)}")
+    if cnt.numel() != plan.count:
+        raise RuntimeError(f"cnt must be this rank's [{plan.count}, 1] rows, got {tuple(cnt.shape)}")
+    return CH
+
+
+def dense_apply_weights(plan: ShardPlan, exchange: "Exchange", pool: "WorkspacePool", rs, means3D, opacities, scales,
+                        rotations, cov3Ds_precomp, image_weights, weights, cnt):
+    """One view of semantic tracing in the dense exchange: preprocess -> all-gather (or barrier) -> order -> walk of
+    the owned tiles into zeroed [P_pad, CH] / [P_pad] buffers -> reduce-scatter of both (cnt stays int32) -> this
+    rank's slices added into `weights` / `cnt`."""
+    device = means3D.device
+    empty = torch.empty(0, dtype=torch.float32, device=device)
+    CH = int(image_weights.size(0))
+    ws = pool.take(device)
+    try:
+        # this rank's means3D stands in the colors_precomp slot, as on one GPU: the colours are never used
+        buf = shard_preprocess(plan, rs, means3D, empty, means3D, opacities, scales, rotations, cov3Ds_precomp, ws=ws)
+        if buf.peer is not None:
+            exchange.barrier(device)
+        else:
+            exchange.all_gather_inplace(exchange_view(buf))
+        shard_order(buf)
+        w_total = buf.alloc("aw_weights", plan.P_pad * CH, torch.float32, device).view(plan.P_pad, CH).zero_()
+        c_total = buf.alloc("aw_cnt", plan.P_pad, torch.int32, device).zero_()
+        shard_apply_weights(buf, image_weights, w_total, c_total)
+        w_slice = buf.alloc("aw_weights_slice", plan.slice_len * CH, torch.float32, device).view(plan.slice_len, CH)
+        c_slice = buf.alloc("aw_cnt_slice", plan.slice_len, torch.int32, device)
+        exchange.reduce_scatter_sum(w_total, w_slice)
+        exchange.reduce_scatter_sum(c_total, c_slice)
+        n = plan.count
+        weights.view(n, CH).add_(w_slice[:n])
+        cnt.view(n).add_(c_slice[:n])
+    finally:
+        pool.give(ws)
+
+
 # ---------------------------------------------------------------------------------------------------------
 # autograd + module (one process per GPU)
 # ---------------------------------------------------------------------------------------------------------
@@ -466,13 +557,13 @@ def p2p_available(exchange: "Exchange") -> bool:
 
 
 def _check_deterministic_flag():
-    """The sharded backward adds gradient rows with float atomics, whose order changes from call to call. Under
+    """The sharded backward and apply_weights add rows with float atomics, whose order changes from call to call. Under
     ``torch.use_deterministic_algorithms(True)`` that is an error (a warning with ``warn_only=True``), as for any PyTorch op
     without a deterministic implementation; the single-GPU ``GaussianRasterizer`` has one."""
     if not torch.are_deterministic_algorithms_enabled():
         return
-    msg = ("ShardedGaussianRasterizer does not have a deterministic implementation: its backward adds gradients with "
-           "float atomics. Use the single-GPU GaussianRasterizer (deterministic mode) or turn the flag off with "
+    msg = ("ShardedGaussianRasterizer does not have a deterministic implementation: its backward and apply_weights add "
+           "with float atomics. Use the single-GPU GaussianRasterizer (deterministic mode) or turn the flag off with "
            "torch.use_deterministic_algorithms(False).")
     if torch.is_deterministic_algorithms_warn_only_enabled():
         warnings.warn(msg)
@@ -551,3 +642,29 @@ class ShardedGaussianRasterizer(nn.Module):
                                                     cov3D_precomp, rs, self.sparse_pool, self.exchange)
         return _ShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                        cov3D_precomp, rs, self.plan, self.exchange, self.pool)
+
+    def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
+                      cov3Ds_precomp=None, cnt=None, image_weights=None):
+        """Semantic tracing of the sharded cloud (``GaussianRasterizer.apply_weights``, collective: every rank calls it
+        for the same view). The per-Gaussian tensors, ``weights`` [n,CH] float32 and ``cnt`` [n,1] int32 are THIS RANK's
+        rows and are updated in place (accumulated over calls); ``image_weights`` [CH,H,W] is the full mask, the same on
+        every rank. ``cnt`` equals the single-GPU result bit for bit, ``weights`` up to the order of the float sums."""
+        _check_deterministic_flag()
+        rs = self.raster_settings
+        check_apply_weights_args(self.plan, rs, means3D, weights, cnt, image_weights, scales, rotations, cov3Ds_precomp)
+        empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
+        scales = empty if scales is None else scales
+        rotations = empty if rotations is None else rotations
+        cov3Ds_precomp = empty if cov3Ds_precomp is None else cov3Ds_precomp
+        with torch.no_grad():
+            if self.mode == "sparse":
+                from . import sparse_sharded as SS
+                SS.sparse_apply_weights(self.sparse_pool, rs, means3D, opacities, scales, rotations, cov3Ds_precomp,
+                                        image_weights, weights, cnt)
+            else:
+                dense_apply_weights(self.plan, self.exchange, self.pool, rs, means3D, opacities, scales, rotations,
+                                    cov3Ds_precomp, image_weights, weights, cnt)
+
+    def markVisible(self, positions):
+        """``GaussianRasterizer.markVisible`` of this rank's rows ``positions`` [n,3] (no collective)."""
+        return mark_visible(self.raster_settings, positions)

@@ -36,6 +36,7 @@ from .sharded import ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, shard_slice
 
 MAXP = 8  # GSR_MAX_PEERS
 CTRL_BYTES, CTRL_MATRIX_OFFSET, CTRL_ERROR_OFFSET = 512, 64, 32   # GSR_PEER_CTRL_{BYTES,MATRIX_OFFSET,ERROR_OFFSET}
+AW_CNT_SLOT = 11   # GSR_SPARSE_AW_CNT_SLOT: float of an apply_weights candidate row that carries the int32 count bits
 
 
 def _align(n: int, a: int = 256) -> int:
@@ -347,6 +348,79 @@ def _mark(name: str):
         TRACE.append((name, ev))
 
 
+def _preprocess_and_order(rk: SparseRank, pool: SparsePool, rs, means3D, sh, colors_precomp, opacities, scales, rotations,
+                          cov3Ds_precomp):
+    """preprocess + push -- barrier with the count row -- order, redone with the exact capacity while a segment
+    overflows; then the capacity of the next step. Returns (step, num_rendered of this rank, largest segment)."""
+    while True:
+        st = sparse_preprocess(rk, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                               pool.cap)
+        _mark("preprocess+push")
+        peer_barrier(rk, with_row=True)                # counts + barrier: every push has landed
+        rk.queue_barrier_check()                       # sticky error word (this and earlier barriers) -> pinned
+        _mark("count all-reduce")
+        R, max_count = sparse_order(st)                # waits for R, queued behind that copy
+        rk.raise_if_barrier_failed()
+        _mark("order")
+        if max_count <= st.cap:
+            break
+        pool.redo += 1                                  # same decision on every rank (the matrix is global)
+        pool.cap = next_capacity(max_count, rk.cap_alloc)
+    pool.cap = next_capacity(max_count, rk.cap_alloc)
+    return st, R, max_count
+
+
+def apply_weights_walk(st: SparseStep, image_weights: torch.Tensor, acc: torch.Tensor):
+    """Semantic tracing of the owned tiles of the candidate cloud into the zeroed rows `acc` [world*cap, 12]: weights in
+    floats 0..CH-1, the count as int32 bits in float GSR_SPARSE_AW_CNT_SLOT (so that sparse_return carries it exactly)."""
+    from .sharded import owner_apply_weights
+    rk = st.rk
+    M = rk.plan.world * st.cap
+    owner_apply_weights(st.s, rk.plan.owner(), M, st.R, rk.cand, st.radii_cand, _f32c(image_weights, rk.device), acc,
+                        ACC_STRIDE, acc.view(torch.int32)[:, AW_CNT_SLOT], ACC_STRIDE,
+                        lambda name, n, dtype, grow: rk.get(name, n, dtype, grow))
+
+
+def apply_weights_gather(st: SparseStep, weights: torch.Tensor, cnt: torch.Tensor):
+    """Owner side, after the return barrier: weights [n, CH] += and cnt [n] += the returned rows of each owned Gaussian,
+    in ascending rank order."""
+    lib = _lib.load()
+    rk = st.rk
+    CH = int(weights.size(1)) if weights.dim() > 1 else 1
+    with torch.cuda.device(rk.device):
+        stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
+        gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
+        _lib.check(lib.gsr_sparse_apply_weights_gather(C.byref(st.cplan), _ptr(rk.local), rk.local_bytes, _ptr(rk.cand), gb,
+                                                       st.n, CH, _ptr(weights), _ptr(cnt), stream),
+                   "gsr_sparse_apply_weights_gather")
+
+
+def sparse_apply_weights(pool: SparsePool, rs, means3D, opacities, scales, rotations, cov3Ds_precomp, image_weights,
+                         weights, cnt):
+    """One view of semantic tracing with the sparse exchange (arguments checked by the caller): preprocess + push --
+    barrier -- order (as the forward) -> walk of the owned tiles into zeroed candidate rows -> return -- barrier --
+    gather into this rank's `weights` / `cnt`. A rank without owned tile rows or instances still takes part in every
+    barrier. The workspace goes back to the pool before returning."""
+    rk = pool.take()
+    empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
+    _mark("start")
+    try:
+        # this rank's means3D stands in the colors_precomp slot, as on one GPU: the colours are never used
+        st, _, _ = _preprocess_and_order(rk, pool, rs, means3D, empty, means3D, opacities, scales, rotations,
+                                         cov3Ds_precomp)
+        M = rk.plan.world * st.cap
+        acc = rk.get("acc", M * ACC_STRIDE, torch.float32, grow=1.25).view(M, ACC_STRIDE).zero_()
+        apply_weights_walk(st, image_weights, acc)
+        _mark("walk")
+        sparse_return(st, acc)
+        peer_barrier(rk)
+        _mark("return+barrier")
+        apply_weights_gather(st, weights, cnt)
+        _mark("gather")
+    finally:
+        pool.give(rk)
+
+
 class _SparseShardedRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange):
@@ -354,24 +428,11 @@ class _SparseShardedRasterize(torch.autograd.Function):
         device = means3D.device
         _mark("start")
         try:
-            while True:
-                st = sparse_preprocess(rk, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                       pool.cap)
-                _mark("preprocess+push")
-                peer_barrier(rk, with_row=True)                # counts + barrier: every push has landed
-                rk.queue_barrier_check()                       # sticky error word (this and earlier barriers) -> pinned
-                _mark("count all-reduce")
-                R, max_count = sparse_order(st)                # waits for R, queued behind that copy
-                rk.raise_if_barrier_failed()
-                _mark("order")
-                if max_count <= st.cap:
-                    break
-                pool.redo += 1                                  # same decision on every rank (the matrix is global)
-                pool.cap = next_capacity(max_count, rk.cap_alloc)
+            st, R, max_count = _preprocess_and_order(rk, pool, rs, means3D, sh, colors_precomp, opacities, scales,
+                                                     rotations, cov3Ds_precomp)
         except BaseException:
             pool.give(rk)                                       # a failed forward must not leak its workspace
             raise
-        pool.cap = next_capacity(max_count, rk.cap_alloc)
         weakref.finalize(st, pool.give, rk)
         # Every pixel has exactly one writer (the owner of its tile row; empty tiles are written too), so the frame needs
         # no zero-fill -- and must not get one: a faster peer may already have stored its rows here.

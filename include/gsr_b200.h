@@ -351,6 +351,22 @@ GSR_API int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud
                                   int32_t index_base, const void* geometry, size_t geometry_bytes,
                                   const int32_t* radii_total, const void* acc_slice, const gsr_grads* grads,
                                   void* stream);
+/* Semantic tracing (gsr_apply_weights) of a sharded cloud. After gsr_shard_order (with the same owner and workspaces),
+ * bins the owned tile rows and walks them: every hit of splat i (GLOBAL index) adds the pixel's mask value to
+ * weights_total[i*weights_stride + ch] (ch < num_channels, float atomics) and num_channels to
+ * cnt_total[i*cnt_stride] (int32 atomics). Nothing is zeroed here. num_channels is 1..3, weights_stride >= num_channels,
+ * cnt_stride >= 1 (elements); image_weights is the full [num_channels, H, W] mask on every rank. Timed under the
+ * "apply_weights" stage. The sequence of one view (the colours are unused: any valid [shard.P, 3] buffer, e.g. means3D,
+ * may stand in the colors_precomp slot, as gsr_apply_weights' callers do):
+ *   gsr_shard_preprocess -> ALL-GATHER (or gsr_shard_preprocess_p2p -> barrier) -> gsr_shard_order
+ *   gsr_shard_apply_weights into ZEROED [P_total, CH] float + [P_total] int32 buffers (strides CH and 1)
+ *   -> REDUCE-SCATTER(sum) of both buffers -> add this rank's slices into its weights [shard.P, CH] / cnt [shard.P]
+ * The sparse exchange uses the same call on the candidates (see gsr_sparse_apply_weights_gather). */
+GSR_API int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                    int32_t num_rendered, void* geometry, size_t geometry_bytes, void* binning,
+                                    size_t binning_bytes, void* image, size_t image_bytes, const int32_t* radii_total,
+                                    const float* image_weights, int32_t num_channels, float* weights_total,
+                                    int64_t weights_stride, int32_t* cnt_total, int64_t cnt_stride, void* stream);
 
 /* ---- fused preprocess + all-gather over NVLink peer memory ---------------------------------------------------
  * Instead of gsr_shard_preprocess followed by an all-gather, every rank's preprocess kernel pushes its block of
@@ -418,6 +434,21 @@ GSR_API int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_clou
                                    const void* local_ws, size_t local_bytes, const int32_t* radii_local,
                                    const void* cand_ws, size_t cand_bytes, void* acc_slice /* [shard.P,12] scratch */,
                                    size_t acc_bytes, const gsr_grads* grads, void* stream);
+/* Semantic tracing with the sparse exchange. The candidate rows carry the hits: weights in floats 0..CH-1 and the
+ * count as int32 BITS in float GSR_SPARSE_AW_CNT_SLOT (never converted), and gsr_sparse_return copies rows bit for bit.
+ *   gsr_sparse_preprocess -- gsr_peer_barrier(with_matrix_row) -- gsr_sparse_order   (as in the forward, overflow redo
+ *                                                                                    included)
+ *   gsr_shard_apply_weights on the candidates (P_total = world*seg_cap, candidate workspace as `geometry`) into ZEROED
+ *       rows acc [world*seg_cap, 12]: weights_total = acc, weights_stride = 12,
+ *       cnt_total = (int32_t*)(acc + GSR_SPARSE_AW_CNT_SLOT), cnt_stride = 12
+ *   gsr_sparse_return(acc) -- barrier --
+ *   gsr_sparse_apply_weights_gather: weights[i, ch] += and cnt[i] += the <= world returned rows of each owned Gaussian i,
+ *       in ascending rank order (float adds for the weights, integer adds for the count), in place: weights [n, CH]
+ *       and cnt [n] accumulate over views like gsr_apply_weights. local_ws is the one gsr_sparse_preprocess filled. */
+#define GSR_SPARSE_AW_CNT_SLOT 11
+GSR_API int gsr_sparse_apply_weights_gather(const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                            const void* cand_ws, size_t cand_bytes, int32_t n, int32_t num_channels,
+                                            float* weights, int32_t* cnt, void* stream);
 /* Cross-rank barrier over peer memory (replaces the 4-byte NCCL all-reduces of the dense scheme: ~5 us instead of
  * ~25 us at 8 GPUs). Every rank's peer-visible block starts with GSR_PEER_CTRL_BYTES of control words, zeroed once at
  * creation: flags[rank] = number of the last barrier that rank reached, and the [GSR_MAX_PEERS, GSR_MAX_PEERS] int32

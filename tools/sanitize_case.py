@@ -134,5 +134,20 @@ for st, a in zip(steps, accs):
     SS.sparse_return(st, a)
 for st in steps:
     SS.sparse_backward_preprocess(st)
+
+# sharded semantic tracing: dense (two virtual ranks on shared arrays) and sparse (the three ranks above)
+iw3 = torch.rand(3, cam.image_height, cam.image_width, device=dev)
+w_tot = torch.zeros(plans[0].P_pad, 3, device=dev); c_tot = torch.zeros(plans[0].P_pad, dtype=torch.int32, device=dev)
+for b in bufs:
+    S.shard_order(b)
+    S.shard_apply_weights(b, iw3, w_tot, c_tot)
+steps, res = sparse_forward(max(res[0][1], 1))
+accs = [torch.zeros(3 * st.cap, S.ACC_STRIDE, device=dev) for st in steps]
+for st, a in zip(steps, accs):
+    SS.apply_weights_walk(st, iw3, a)
+for st, a in zip(steps, accs):
+    SS.sparse_return(st, a)
+for st in steps:
+    SS.apply_weights_gather(st, torch.zeros(st.n, 3, device=dev), torch.zeros(st.n, 1, dtype=torch.int32, device=dev))
 torch.cuda.synchronize()
 print("SANITIZE_CASE_DONE")

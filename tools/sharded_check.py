@@ -21,12 +21,50 @@ from gaussianeditor_b200.rasterizer import GaussianRasterizer  # noqa: E402
 from util import cloud_tensors, rel_l2, settings_from  # noqa: E402
 
 
+def check_apply_weights(rast, full, loc, cams, bg, sh_degree, dev):
+    """Semantic tracing on the shard vs the full cloud: two views accumulated into the same rows (CH = 1 with a binary
+    mask, CH = 3 with a float mask), `cnt` bit-identical, `weights` within the float-sum bounds, rows that no splat hits
+    untouched; markVisible equals the slice of the full-cloud result. The masks are identical on every rank."""
+    plan = rast.plan
+    P = full["means3D"].shape[0]
+    ok, worst = True, 0.0
+    m3, op = full["means3D"].detach(), full["opacities"].detach()
+    sc, ro = full["scales"].detach(), full["rotations"].detach()
+    lm3, lop, lsc, lro = (loc[k].detach() for k in ("means3D", "opacities", "scales", "rotations"))
+    for CH, binary in ((1, True), (3, False)):
+        w_ref = torch.zeros(P, CH, device=dev); c_ref = torch.zeros(P, 1, dtype=torch.int32, device=dev)
+        w = torch.full((plan.count, CH), 7.0, device=dev); c = torch.full((plan.count, 1), 5, dtype=torch.int32, device=dev)
+        for i, cam in enumerate(cams[:2]):
+            rs = settings_from(cam, bg, sh_degree, dev)
+            g = torch.Generator().manual_seed(100 * CH + i)
+            m = torch.rand(CH, cam.image_height, cam.image_width, generator=g)
+            iw = ((m > 0.5).float() if binary else m).to(dev)
+            GaussianRasterizer(rs).apply_weights(m3, None, op, None, w_ref, sc, ro, None, c_ref, iw)
+            rast.raster_settings = rs
+            rast.apply_weights(lm3, None, lop, None, w, lsc, lro, None, c, iw)
+            if i == 0:
+                vis = rast.markVisible(lm3)
+                ok = ok and torch.equal(vis, S.shard_slice(GaussianRasterizer(rs).markVisible(m3), plan))
+        wr, cr = S.shard_slice(w_ref, plan), S.shard_slice(c_ref, plan)
+        ok = ok and torch.equal(c - 5, cr) and bool((w[(cr == 0).view(-1)] == 7.0).all())
+        dw = w - 7.0
+        if binary:
+            ok = ok and torch.equal(dw, wr)
+        else:
+            worst = max(worst, rel_l2(dw.cpu().numpy(), wr.cpu().numpy()))
+            ok = ok and float((dw - wr).abs().max()) <= 1e-4 * float(wr.abs().max())
+    ok = ok and worst <= 1e-5
+    return ok, f" apply_weights_worst_rel_l2={worst:.2e}"
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="c3")
     ap.add_argument("--P", type=int, default=None)
     ap.add_argument("--p2p", action="store_true", help="dense mode: fused preprocess + all-gather over peer memory")
     ap.add_argument("--mode", default="dense", choices=["dense", "sparse"])
+    ap.add_argument("--apply-weights", action="store_true",
+                    help="also check semantic tracing (CH = 1 and 3) and markVisible against the full cloud")
     a = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     dev = torch.device("cuda", local)
@@ -87,6 +125,10 @@ def main():
     for g, w in pairs:
         worst = max(worst, rel_l2(g.cpu().numpy(), w.cpu().numpy()))
     ok = ok and worst <= 2e-5
+    aw_msg = ""
+    if a.apply_weights:
+        aw_ok, aw_msg = check_apply_weights(rast, full, loc, cams, bg, cloud.sh_degree, dev)
+        ok = ok and aw_ok
     flag = torch.tensor([1 if ok else 0], device=dev)
     dist.all_reduce(flag, op=dist.ReduceOp.MIN)
     if rank == 0:
@@ -96,7 +138,7 @@ def main():
             extra = f" sparse={SS._SparseShardedRasterize.last} redo={rast.sparse_pool.redo}"
         else:
             extra = f" R_rank0={S._ShardedRasterize.last_R}"
-        print(f"world={world} mode={a.mode} p2p={a.p2p} P={P}{extra} worst_grad_rel_l2={worst:.2e}")
+        print(f"world={world} mode={a.mode} p2p={a.p2p} P={P}{extra} worst_grad_rel_l2={worst:.2e}{aw_msg}")
         print("SHARDED_CHECK_OK" if int(flag) == 1 else "SHARDED_CHECK_FAILED")
     del scolor, sradii, sdepth
     import gc
