@@ -32,6 +32,7 @@ SYMBOLS = [
     "gsr_deterministic_scratch_bytes", "gsr_backward_deterministic", "gsr_backward_raw_deterministic",
     "gsr_apply_weights_deterministic",
     "gsr_shard_apply_weights", "gsr_sparse_apply_weights_gather",
+    "gsr_shard_backward_render_deterministic", "gsr_shard_apply_weights_deterministic",
 ]
 
 
@@ -195,6 +196,12 @@ def load():
     lib.gsr_shard_backward_preprocess.argtypes = [S, Cl, i32, i32, vp, sz, vp, vp, C.POINTER(Grads), vp]
     lib.gsr_shard_apply_weights.restype = C.c_int
     lib.gsr_shard_apply_weights.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, i32, vp, i64, vp, i64, vp]
+    lib.gsr_shard_backward_render_deterministic.restype = C.c_int
+    lib.gsr_shard_backward_render_deterministic.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, sz, vp, sz,
+                                                            vp]
+    lib.gsr_shard_apply_weights_deterministic.restype = C.c_int
+    lib.gsr_shard_apply_weights_deterministic.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, i32, vp, i64,
+                                                          vp, i64, vp, sz, vp]
     lib.gsr_peer_alloc.restype = C.c_int; lib.gsr_peer_alloc.argtypes = [sz, C.POINTER(vp), vp]
     lib.gsr_peer_open.restype = C.c_int; lib.gsr_peer_open.argtypes = [vp, C.POINTER(vp)]
     lib.gsr_peer_close.restype = C.c_int; lib.gsr_peer_close.argtypes = [vp]

@@ -661,10 +661,11 @@ int gsr_shard_render(const gsr_settings* s, const gsr_tile_owner* owner, int32_t
   return launch_render_fwd(*s, g, b, im, out_color, out_depth, st, own);
 }
 
-int gsr_shard_backward_render(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
-                              const void* geometry, size_t geometry_bytes, const void* binning, size_t binning_bytes,
-                              const void* image, size_t image_bytes, const float* dL_dout_color, void* acc_total,
-                              size_t acc_bytes, void* stream) {
+static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                                      const void* geometry, size_t geometry_bytes, const void* binning,
+                                      size_t binning_bytes, const void* image, size_t image_bytes,
+                                      const float* dL_dout_color, void* acc_total, size_t acc_bytes, void* stream,
+                                      const DetScratch* ds) {
   int rc = check_settings(s);
   if (rc) return rc;
   TileOwner own;
@@ -673,6 +674,8 @@ int gsr_shard_backward_render(const gsr_settings* s, const gsr_tile_owner* owner
   if (P_total <= 0 || R < 0 || !dL_dout_color) { set_error("shard_backward_render: bad arguments"); return GSR_ERR_INVALID; }
   const size_t need = (size_t)P_total * ACC_STRIDE * sizeof(float);
   if (!acc_total || acc_bytes < need) { set_error("accumulators too small: %zu < %zu", acc_bytes, need); return GSR_ERR_WORKSPACE; }
+  DetWS det;
+  if (ds && (rc = carve_det_checked(*ds, P_total, R, 0, det))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   gsr_cloud c{};
   c.P = P_total;
@@ -681,17 +684,39 @@ int gsr_shard_backward_render(const gsr_settings* s, const gsr_tile_owner* owner
                  const_cast<void*>(image), image_bytes, g, b, im);
   if (rc) return rc;
   StageScope t(ST_RENDER_BWD, st);
-  cudaError_t e = cudaMemsetAsync(acc_total, 0, need, st);
-  if (e != cudaSuccess) return check_cuda(e, "accumulator memset");
+  if (!ds || R == 0) {  // the deterministic reduction writes every accumulator row itself
+    cudaError_t e = cudaMemsetAsync(acc_total, 0, need, st);
+    if (e != cudaSuccess) return check_cuda(e, "accumulator memset");
+  }
   if (R == 0) return GSR_OK;
-  return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own);
+  return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own, nullptr, nullptr,
+                           ds ? &det : nullptr, P_total, R);
 }
 
-int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
-                            void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
-                            size_t image_bytes, const int32_t* radii_total, const float* image_weights, int32_t CH,
-                            float* weights_total, int64_t weights_stride, int32_t* cnt_total, int64_t cnt_stride,
-                            void* stream) {
+int gsr_shard_backward_render(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                              const void* geometry, size_t geometry_bytes, const void* binning, size_t binning_bytes,
+                              const void* image, size_t image_bytes, const float* dL_dout_color, void* acc_total,
+                              size_t acc_bytes, void* stream) {
+  return shard_backward_render_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                    image_bytes, dL_dout_color, acc_total, acc_bytes, stream, nullptr);
+}
+
+int gsr_shard_backward_render_deterministic(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                            int32_t R, const void* geometry, size_t geometry_bytes, const void* binning,
+                                            size_t binning_bytes, const void* image, size_t image_bytes,
+                                            const float* dL_dout_color, void* acc_total, size_t acc_bytes,
+                                            void* det_scratch, size_t det_scratch_bytes, void* stream) {
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  return shard_backward_render_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                    image_bytes, dL_dout_color, acc_total, acc_bytes, stream, &ds);
+}
+
+static int shard_apply_weights_impl(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                                    void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes,
+                                    void* image, size_t image_bytes, const int32_t* radii_total,
+                                    const float* image_weights, int32_t CH, float* weights_total,
+                                    int64_t weights_stride, int32_t* cnt_total, int64_t cnt_stride, void* stream,
+                                    const DetScratch* ds) {
   int rc = check_settings(s);
   if (rc) return rc;
   TileOwner own;
@@ -706,6 +731,12 @@ int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner* owner, 
     set_error("shard_apply_weights: need weights_stride >= num_channels and cnt_stride >= 1");
     return GSR_ERR_INVALID;
   }
+  if (ds && weights_stride != CH) {  // the reduction adds into packed [P_total, CH] weights
+    set_error("shard_apply_weights_deterministic: need weights_stride == num_channels");
+    return GSR_ERR_INVALID;
+  }
+  DetWS det;
+  if (ds && (rc = carve_det_checked(*ds, P_total, R, CH, det))) return rc;
   if (R == 0) return GSR_OK;
   cudaStream_t st = (cudaStream_t)stream;
   gsr_cloud c{};
@@ -715,9 +746,32 @@ int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner* owner, 
   if (rc) return rc;
   rc = run_binning(*s, c, R, false, g, b, im, radii_total, st, own);
   if (rc) return rc;
-  StageScope t(ST_APPLY_W, st);
+  StageScope t(ST_APPLY_W, st);  // deterministic mode: includes the reduction
   return launch_apply_weights_owner(*s, g, b, im, image_weights, CH, weights_total, weights_stride, cnt_total, cnt_stride,
-                                    own, st);
+                                    own, st, ds ? &det : nullptr, P_total, R);
+}
+
+int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                            void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                            size_t image_bytes, const int32_t* radii_total, const float* image_weights, int32_t CH,
+                            float* weights_total, int64_t weights_stride, int32_t* cnt_total, int64_t cnt_stride,
+                            void* stream) {
+  return shard_apply_weights_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                  image_bytes, radii_total, image_weights, CH, weights_total, weights_stride, cnt_total,
+                                  cnt_stride, stream, nullptr);
+}
+
+int gsr_shard_apply_weights_deterministic(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                          int32_t R, void* geometry, size_t geometry_bytes, void* binning,
+                                          size_t binning_bytes, void* image, size_t image_bytes,
+                                          const int32_t* radii_total, const float* image_weights, int32_t CH,
+                                          float* weights_total, int64_t weights_stride, int32_t* cnt_total,
+                                          int64_t cnt_stride, void* det_scratch, size_t det_scratch_bytes,
+                                          void* stream) {
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  return shard_apply_weights_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                  image_bytes, radii_total, image_weights, CH, weights_total, weights_stride, cnt_total,
+                                  cnt_stride, stream, &ds);
 }
 
 int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,

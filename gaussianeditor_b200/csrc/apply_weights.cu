@@ -116,11 +116,14 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_owner_kernel(const AwO
 // memory [8 warps][256][CH]. At the round boundary (where __syncthreads_count already synchronises, and so also before
 // the early break) thread t adds the 8 warp entries of splat t in warp order and stores the row at that instance's
 // emission slot, with its flag; the reduction kernel adds each Gaussian's rows to `weights`. `cnt` keeps its integer
-// atomics, which are exact.
+// atomics, which are exact. Ownership as in apply_weights_owner_kernel: blockIdx.y = k-th owned tile row ({1, 0} on a
+// single GPU), and the count of splat id goes to cnt[id*c_stride].
 struct AwDetArgs : AwArgs {
   const uint32_t* excl;
   float* rows;     // [R, CH]
   uint8_t* flags;  // [R]
+  int own_stride, own_phase;
+  int64_t c_stride;
 };
 
 template <int CH>
@@ -130,10 +133,11 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_det_kernel(const AwDet
   __shared__ uint32_t s_ids[TILE_PIX];
   __shared__ uint32_t s_slot[TILE_PIX];
   __shared__ float s_w[NW][TILE_PIX][CH];
-  const int tile = blockIdx.y * a.gx + blockIdx.x;
+  const unsigned ty = a.own_phase + blockIdx.y * a.own_stride;
+  const int tile = ty * a.gx + blockIdx.x;
   const int tid = threadIdx.y * TILE + threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5;
-  const uint2 pix = make_uint2(blockIdx.x * TILE + threadIdx.x, blockIdx.y * TILE + threadIdx.y);
+  const uint2 pix = make_uint2(blockIdx.x * TILE + threadIdx.x, ty * TILE + threadIdx.y);
   const bool inside = pix.x < (unsigned)a.W && pix.y < (unsigned)a.H;
   const size_t pix_id = (size_t)a.W * pix.y + pix.x;
   const float2 pixf = make_float2((float)pix.x, (float)pix.y);
@@ -175,7 +179,8 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_det_kernel(const AwDet
       s_q0[tid] = q0;
       s_q1[tid] = __ldg(r + 1);
       s_ids[tid] = id;
-      s_slot[tid] = emission_slot(ex, q0.x, q0.y, __float_as_int(__ldg(r + 2).w), a.gx, a.gy, blockIdx.x, blockIdx.y);
+      s_slot[tid] = emission_slot(ex, q0.x, q0.y, __float_as_int(__ldg(r + 2).w), a.gx, a.gy, blockIdx.x, ty,
+                                  a.own_stride, a.own_phase);
     }
     __syncthreads();
     const int n = min(TILE_PIX, toDo);
@@ -207,7 +212,7 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_det_kernel(const AwDet
           for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
           if (lane == 0) s_w[warp][j][ch] = v;
         }
-        if (lane == 0) atomicAdd(a.cnt + s_ids[j], CH * __popc(hits));
+        if (lane == 0) atomicAdd(a.cnt + (size_t)s_ids[j] * a.c_stride, CH * __popc(hits));
       } else if (lane == 0) {
 #pragma unroll
         for (int ch = 0; ch < CH; ch++) s_w[warp][j][ch] = 0.f;
@@ -219,6 +224,24 @@ __global__ void __launch_bounds__(TILE_PIX) apply_weights_det_kernel(const AwDet
     __syncthreads();
     flush(prev_n);
   }
+}
+
+// Deterministic walk of the owned tile rows (grid.y of them) + the reduction into the packed weights [P, CH].
+int launch_apply_weights_det(const gsr_settings& s, const GeometryWS& g, const AwArgs& a, int CH, int64_t c_stride,
+                             const TileOwner& own, dim3 grid, cudaStream_t st, const DetWS& det, int P, int64_t R) {
+  int rc = launch_det_prepare(P, R, 1, g, det, st);
+  if (rc) return rc;
+  AwDetArgs da;
+  static_cast<AwArgs&>(da) = a;
+  da.excl = det.excl; da.rows = det.rows; da.flags = det.flags;
+  da.own_stride = own.stride; da.own_phase = own.phase; da.c_stride = c_stride;
+  const dim3 block(TILE, TILE);
+  if (CH == 1) apply_weights_det_kernel<1><<<grid, block, 0, st>>>(da);
+  else if (CH == 2) apply_weights_det_kernel<2><<<grid, block, 0, st>>>(da);
+  else apply_weights_det_kernel<3><<<grid, block, 0, st>>>(da);
+  g_launches++;
+  if ((rc = check_launch("apply_weights", s.debug != 0, st))) return rc;
+  return launch_det_reduce_weights(P, CH, g, det, a.weights, st);
 }
 
 }  // namespace
@@ -233,19 +256,8 @@ int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const Binni
   a.image_weights = image_weights; a.weights = weights; a.cnt = cnt;
   if (a.gx * a.gy == 0) return GSR_OK;
   dim3 grid(a.gx, a.gy), block(TILE, TILE);
-  if (det != nullptr && CH >= 1 && CH <= 3) {
-    int rc = launch_det_prepare(P, R, 1, g, *det, st);
-    if (rc) return rc;
-    AwDetArgs da;
-    static_cast<AwArgs&>(da) = a;
-    da.excl = det->excl; da.rows = det->rows; da.flags = det->flags;
-    if (CH == 1) apply_weights_det_kernel<1><<<grid, block, 0, st>>>(da);
-    else if (CH == 2) apply_weights_det_kernel<2><<<grid, block, 0, st>>>(da);
-    else apply_weights_det_kernel<3><<<grid, block, 0, st>>>(da);
-    g_launches++;
-    if ((rc = check_launch("apply_weights", s.debug != 0, st))) return rc;
-    return launch_det_reduce_weights(P, CH, g, *det, weights, st);
-  }
+  if (det != nullptr && CH >= 1 && CH <= 3)
+    return launch_apply_weights_det(s, g, a, CH, 1, TileOwner(), grid, st, *det, P, R);
   if (CH == 1) apply_weights_kernel<1><<<grid, block, 0, st>>>(a);
   else if (CH == 2) apply_weights_kernel<2><<<grid, block, 0, st>>>(a);
   else if (CH == 3) apply_weights_kernel<3><<<grid, block, 0, st>>>(a);
@@ -259,7 +271,8 @@ int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const Binni
 
 int launch_apply_weights_owner(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                                const float* image_weights, int CH, float* weights, int64_t w_stride, int32_t* cnt,
-                               int64_t c_stride, const TileOwner& own, cudaStream_t st) {
+                               int64_t c_stride, const TileOwner& own, cudaStream_t st, const DetWS* det, int P,
+                               int64_t R) {
   AwOwnerArgs a;
   a.ranges = im.ranges; a.point_list = b.point_list; a.records = g.records;
   a.W = s.image_width; a.H = s.image_height;
@@ -269,6 +282,12 @@ int launch_apply_weights_owner(const gsr_settings& s, const GeometryWS& g, const
   const int rows = own.owned_rows(a.gy);
   if (a.gx * rows == 0) return GSR_OK;
   dim3 grid(a.gx, rows), block(TILE, TILE);
+  if (det != nullptr && CH >= 1 && CH <= 3 && w_stride == CH)
+    return launch_apply_weights_det(s, g, a, CH, c_stride, own, grid, st, *det, P, R);
+  if (det != nullptr) {
+    set_error("apply_weights: deterministic mode needs 1..3 channels and weights_stride == num_channels");
+    return GSR_ERR_INVALID;
+  }
   if (CH == 1) apply_weights_owner_kernel<1><<<grid, block, 0, st>>>(a);
   else if (CH == 2) apply_weights_owner_kernel<2><<<grid, block, 0, st>>>(a);
   else if (CH == 3) apply_weights_owner_kernel<3><<<grid, block, 0, st>>>(a);

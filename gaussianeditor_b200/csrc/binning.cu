@@ -46,15 +46,6 @@ struct GatherTilesOp {
   __host__ __device__ __forceinline__ uint32_t operator()(uint32_t rank) const { return tiles[order[rank]]; }
 };
 
-// Rows of the rectangle [rmin.y, rmax.y) this rank owns (ty % stride == phase): first owned row and their number.
-__device__ __forceinline__ void owned_rows(uint32_t ymin, uint32_t ymax, int stride, int phase, uint32_t& y0, uint32_t& ny) {
-  if (stride == 1) { y0 = ymin; ny = ymax - ymin; return; }
-  int d = (phase - (int)ymin) % stride;
-  if (d < 0) d += stride;
-  y0 = ymin + (uint32_t)d;
-  ny = y0 < ymax ? (ymax - y0 + (uint32_t)stride - 1u) / (uint32_t)stride : 0u;
-}
-
 // Sharded path, after the all-gather of the splat records: rebuild the per-Gaussian arrays of all P Gaussians from
 // the records (radius = q2.w, depth key = bits of q1.z), count the OWNED tiles and write the identity permutation the
 // depth sort carries. A Gaussian that touches none of this rank's tile rows gets the "culled" depth key, so that --

@@ -1,6 +1,9 @@
 // Shared declarations of the sm_90a rasterizer kernels (internal; the public surface is include/gsr_b200.h).
 #pragma once
 #include <cuda_runtime.h>
+#ifndef __CUDACC__
+#include <algorithm>  // min/max of the host/device helpers below, for a pure host compiler
+#endif
 #include <atomic>
 #include <math.h>
 #include <stdint.h>
@@ -96,11 +99,12 @@ constexpr int ACC_STRIDE = 12;
 
 // Deterministic mode (deterministic.cu): the float atomics of render_bwd and apply_weights are replaced by plain stores
 // of one row per (instance, tile half) -- per instance for apply_weights -- at the instance's EMISSION SLOT, the
-// position binning gave it before the tile sort:
+// position binning gave it before the tile sort (emission_slot below):
 //   slot(g, tile) = excl[g] + (ty - rmin.y) * (rmax.x - rmin.x) + (tx - rmin.x)
-// with excl[g] the exclusive prefix of the tile counts in depth order and [rmin, rmax) the tile rectangle (tile_rect).
-// The slots of Gaussian g are [excl[g], excl[g] + tiles_touched[g]), so one reduction kernel adds each Gaussian's
-// flagged rows in a fixed order: the result depends on the data only, never on timing.
+// with excl[g] the exclusive prefix of the tile counts in depth order and [rmin, rmax) the tile rectangle (tile_rect);
+// on a sharded rank that owns the tile rows ty % stride == phase, (ty - rmin.y) becomes the index of ty among the
+// rectangle's owned rows. The slots of Gaussian g are [excl[g], excl[g] + tiles_touched[g]), so one reduction kernel
+// adds each Gaussian's flagged rows in a fixed order: the result depends on the data only, never on timing.
 struct DetWS {
   uint32_t* excl;   // [P]
   uint8_t* flags;   // [2R]: row written this call
@@ -183,7 +187,7 @@ int launch_tile_count(const GeometryWS& g, int gx, int gy, const TileOwner& own,
 int launch_render_fwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       float* out_color, float* out_depth, cudaStream_t st, const TileOwner& own = TileOwner());
 // dL_ddepth != nullptr: also the depth image's upstream [H*W]; dL/dz of each splat goes to acc slot 9 (variant 15 only)
-// det != nullptr: deterministic mode (single-GPU only): rows + reduction instead of atomics; acc needs no memset
+// det != nullptr: deterministic mode: rows + reduction instead of atomics; acc needs no memset (all P rows written)
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own = TileOwner(),
                       const float* dL_dalpha_img = nullptr, const float* dL_ddepth = nullptr,
@@ -211,10 +215,12 @@ int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, ui
 int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                          const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st,
                          const DetWS* det = nullptr, int P = 0, int64_t R = 0);
-// sharded path: the walk of the owned tiles only; splat id adds to weights[id*w_stride + ch] and cnt[id*c_stride]
+// sharded path: the walk of the owned tiles only; splat id adds to weights[id*w_stride + ch] and cnt[id*c_stride].
+// det != nullptr: deterministic mode (rows + reduction into weights); needs w_stride == CH
 int launch_apply_weights_owner(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                                const float* image_weights, int CH, float* weights, int64_t w_stride, int32_t* cnt,
-                               int64_t c_stride, const TileOwner& own, cudaStream_t st);
+                               int64_t c_stride, const TileOwner& own, cudaStream_t st, const DetWS* det = nullptr,
+                               int P = 0, int64_t R = 0);
 
 // ---- host + device helpers ----------------------------------------------------------------------------
 // The per-pixel hit test and the sub-block culling predicate compile for the host too (oracle/subblock_check.cpp
@@ -312,6 +318,45 @@ __host__ __device__ __forceinline__ uint32_t splat_subblock_mask(const float4 q0
   return mask;
 }
 
+// Tile rectangles and emission slots. They compile for the host too, so that a CPU test can check the slots on a
+// forward state; a pure host compiler takes min/max from <algorithm> (nvcc provides them for both sides).
+#ifndef __CUDACC__
+using std::max;
+using std::min;
+#endif
+
+// tile rectangle [rmin, rmax) of a splat (auxiliary.h:46-56); binning and the deterministic kernels share it
+__host__ __device__ __forceinline__ void tile_rect(float px, float py, int radius, int gx, int gy, uint2& rmin,
+                                                   uint2& rmax) {
+  rmin.x = (unsigned)min(gx, max((int)0, (int)((px - radius) / TILE)));
+  rmin.y = (unsigned)min(gy, max((int)0, (int)((py - radius) / TILE)));
+  rmax.x = (unsigned)min(gx, max((int)0, (int)((px + radius + TILE - 1) / TILE)));
+  rmax.y = (unsigned)min(gy, max((int)0, (int)((py + radius + TILE - 1) / TILE)));
+}
+// Rows of the rectangle [ymin, ymax) this rank owns (ty % stride == phase): first owned row and their number.
+__host__ __device__ __forceinline__ void owned_rows(uint32_t ymin, uint32_t ymax, int stride, int phase, uint32_t& y0,
+                                                    uint32_t& ny) {
+  if (stride == 1) { y0 = ymin; ny = ymax - ymin; return; }
+  int d = (phase - (int)ymin) % stride;
+  if (d < 0) d += stride;
+  y0 = ymin + (uint32_t)d;
+  ny = y0 < ymax ? (ymax - y0 + (uint32_t)stride - 1u) / (uint32_t)stride : 0u;
+}
+// Emission slot of instance (tx, ty) of the Gaussian with exclusive prefix `excl` and radius `radius` at (px, py), on
+// a rank that owns the tile rows ty % stride == phase. Binning emits a Gaussian's instances row by row over its owned
+// rows (tile y0 + ry*stride, owned_rows), so the slot is excl + ((ty - y0)/stride)*(rmax.x - rmin.x) + (tx - rmin.x);
+// with {1, 0} (every row) it is excl + (ty - rmin.y)*(rmax.x - rmin.x) + (tx - rmin.x).
+__host__ __device__ __forceinline__ uint32_t emission_slot(uint32_t excl, float px, float py, int radius, int gx, int gy,
+                                                           int tx, int ty, int stride, int phase) {
+  uint2 rmin, rmax;
+  tile_rect(px, py, radius, gx, gy, rmin, rmax);
+  uint32_t y0, ny;
+  owned_rows(rmin.y, rmax.y, stride, phase, y0, ny);
+  const uint32_t dy = (uint32_t)ty - y0;
+  const uint32_t ry = stride == 1 ? dy : dy / (uint32_t)stride;
+  return excl + ry * (rmax.x - rmin.x) + ((uint32_t)tx - rmin.x);
+}
+
 #ifdef __CUDACC__
 // ---- device helpers ---------------------------------------------------------------------------------
 
@@ -319,21 +364,6 @@ __host__ __device__ __forceinline__ uint32_t splat_subblock_mask(const float4 q0
 __device__ __forceinline__ int owned_tile(int n, int gx, int stride, int phase) {
   const int r = n / gx;
   return (phase + r * stride) * gx + (n - r * gx);
-}
-
-// tile rectangle [rmin, rmax) of a splat (auxiliary.h:46-56); binning and the deterministic backward share it
-__device__ __forceinline__ void tile_rect(float px, float py, int radius, int gx, int gy, uint2& rmin, uint2& rmax) {
-  rmin.x = (unsigned)min(gx, max((int)0, (int)((px - radius) / TILE)));
-  rmin.y = (unsigned)min(gy, max((int)0, (int)((py - radius) / TILE)));
-  rmax.x = (unsigned)min(gx, max((int)0, (int)((px + radius + TILE - 1) / TILE)));
-  rmax.y = (unsigned)min(gy, max((int)0, (int)((py + radius + TILE - 1) / TILE)));
-}
-// emission slot of the instance (Gaussian with exclusive prefix `excl` and radius `radius` at (px, py), tile (tx, ty))
-__device__ __forceinline__ uint32_t emission_slot(uint32_t excl, float px, float py, int radius, int gx, int gy, int tx,
-                                                  int ty) {
-  uint2 rmin, rmax;
-  tile_rect(px, py, radius, gx, gy, rmin, rmax);
-  return excl + ((uint32_t)ty - rmin.y) * (rmax.x - rmin.x) + ((uint32_t)tx - rmin.x);
 }
 
 // the four corners of a tile rectangle [rmin, rmax) in replica (idx & (copies-1)) of the (gy+1) x (gx+1) difference array

@@ -524,7 +524,8 @@ __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(co
     if (mask != 0) {
       const int slot = __popc(keep & ((1u << lane) - 1u));
       uint32_t es = 0;  // DET: the instance's emission slot, kept in sid (the flush needs no Gaussian index then)
-      if constexpr (DET) es = emission_slot(ex, q0.x, q0.y, __float_as_int(q2.w), a.gx, a.gy, tx, ty);
+      if constexpr (DET)
+        es = emission_slot(ex, q0.x, q0.y, __float_as_int(q2.w), a.gx, a.gy, tx, ty, a.own_stride, a.own_phase);
       q1.w = __uint_as_float(mask);
       q2.w = __uint_as_float((uint32_t)pos);
       stg[0][slot] = q0;
@@ -724,7 +725,6 @@ int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningW
   const int ntiles = a.gx * own.owned_rows(a.gy);  // tiles this rank walks (all of them when own = {1,0})
   if (ntiles == 0) return GSR_OK;
   if (det != nullptr) {  // deterministic mode: variant 15 (or its depth form) writes rows, one kernel reduces them
-    if (own.stride != 1) { set_error("render_bwd: deterministic mode is single-GPU only"); return GSR_ERR_INVALID; }
     int rc = launch_det_prepare(P, R, 2, g, *det, st);
     if (rc) return rc;
     const int blocks = (ntiles * 2 + BW_WARPS - 1) / BW_WARPS;

@@ -47,14 +47,6 @@ uint32_t higher_msb(uint32_t n) {
   return msb;
 }
 
-__device__ __forceinline__ void owned_rows(uint32_t ymin, uint32_t ymax, int stride, int phase, uint32_t& y0, uint32_t& ny) {
-  if (stride == 1) { y0 = ymin; ny = ymax - ymin; return; }
-  int d = (phase - (int)ymin) % stride;
-  if (d < 0) d += stride;
-  y0 = ymin + (uint32_t)d;
-  ny = y0 < ymax ? (ymax - y0 + (uint32_t)stride - 1u) / (uint32_t)stride : 0u;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // ranges + digit bases from the difference array (one CTA; the arrays are a few tens of KB and L2-resident)
 // ---------------------------------------------------------------------------------------------------------------

@@ -143,6 +143,30 @@ class Exchange:
             n = out.shape[0]
             out.copy_(tmp[self.rank * n:(self.rank + 1) * n])
 
+    def reduce_scatter_ordered(self, total: torch.Tensor, out: torch.Tensor):
+        """reduce_scatter_sum with a fixed summation order: every rank's slice comes here whole (all-to-all) and the
+        slices are added in ascending rank order with plain tensor adds, so the result is the same bits on every call
+        (NCCL's reduce-scatter does not promise an order). For the float sums of deterministic mode."""
+        n = out.shape[0]
+        if self.world == 1:
+            out.copy_(total[:n])
+            return
+        recv = torch.empty((self.world,) + tuple(out.shape), dtype=out.dtype, device=out.device)
+        send = total[:self.world * n].contiguous()
+        if self.backend == "nccl":
+            self.dist.all_to_all_single(recv, send, group=self.group)
+        else:
+            try:
+                self.dist.all_to_all_single(recv, send, group=self.group)
+            except (RuntimeError, NotImplementedError):   # a gloo build without all-to-all: gather and keep own slice
+                parts = [torch.empty_like(send) for _ in range(self.world)]
+                self.dist.all_gather(parts, send, group=self.group)
+                for r, p in enumerate(parts):
+                    recv[r].copy_(p[self.rank * n:(self.rank + 1) * n])
+        out.copy_(recv[0])
+        for r in range(1, self.world):
+            out.add_(recv[r])
+
 
 # ---------------------------------------------------------------------------------------------------------
 # peer-mapped geometry workspaces (fused preprocess + all-gather over NVLink)
@@ -365,19 +389,33 @@ def shard_render(buf: ShardBuffers, color: torch.Tensor, depth: torch.Tensor):
                                         _ptr(color), _ptr(depth), st), "gsr_shard_render")
 
 
-def shard_backward_render(buf: ShardBuffers, grad_out_color: torch.Tensor) -> torch.Tensor:
-    """Backward stage 1: this rank's tiles -> partial accumulators [P_pad, 12] (zero for untouched Gaussians)."""
+def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: torch.Tensor, img: torch.Tensor,
+                          grad_out_color: torch.Tensor, acc: torch.Tensor, deterministic: bool, get):
+    """gsr_shard_backward_render (or its deterministic form) of the owned tiles of a P-record workspace into
+    acc [P, 12]; `get(name, numel, dtype, grow)` supplies the deterministic scratch."""
     lib = _lib.load()
-    device = buf.geom.device
+    device = geom.device
     with torch.cuda.device(device):
-        s, own = buf.s, buf.own
         grad_out_color = _f32c(grad_out_color, device)
-        acc = buf.alloc("acc", buf.plan.P_pad * ACC_STRIDE, torch.float32, device).view(buf.plan.P_pad, ACC_STRIDE)
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-        _lib.check(lib.gsr_shard_backward_render(C.byref(s), C.byref(own), buf.plan.P_pad, buf.R, _ptr(buf.geom),
-                                                 buf.geom.numel(), _ptr(buf.binning), buf.binning.numel(),
-                                                 _ptr(buf.img), buf.img.numel(), _ptr(grad_out_color), _ptr(acc),
-                                                 acc.numel() * 4, st), "gsr_shard_backward_render")
+        args = (C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), binning.numel(), _ptr(img),
+                img.numel(), _ptr(grad_out_color), _ptr(acc), acc.numel() * 4)
+        if deterministic:
+            dbytes = lib.gsr_deterministic_scratch_bytes(P, R, 0)
+            det = get("det", dbytes, torch.uint8, 1.25)
+            _lib.check(lib.gsr_shard_backward_render_deterministic(*args, _ptr(det), dbytes, st),
+                       "gsr_shard_backward_render_deterministic")
+        else:
+            _lib.check(lib.gsr_shard_backward_render(*args, st), "gsr_shard_backward_render")
+
+
+def shard_backward_render(buf: ShardBuffers, grad_out_color: torch.Tensor, deterministic: bool = False) -> torch.Tensor:
+    """Backward stage 1: this rank's tiles -> partial accumulators [P_pad, 12] (zero for untouched Gaussians). With
+    `deterministic` each row is the same bits on every call (no float atomics)."""
+    device = buf.geom.device
+    acc = buf.alloc("acc", buf.plan.P_pad * ACC_STRIDE, torch.float32, device).view(buf.plan.P_pad, ACC_STRIDE)
+    owner_backward_render(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.binning, buf.img, grad_out_color, acc,
+                          deterministic, lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow))
     return acc
 
 
@@ -409,10 +447,12 @@ def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor):
 
 
 def owner_apply_weights(s, own, P: int, R: int, geom: torch.Tensor, radii: torch.Tensor, image_weights: torch.Tensor,
-                        weights: torch.Tensor, w_stride: int, cnt: torch.Tensor, c_stride: int, get):
+                        weights: torch.Tensor, w_stride: int, cnt: torch.Tensor, c_stride: int, get,
+                        deterministic: bool = False):
     """gsr_shard_apply_weights: bin + walk the owned tiles of a P-record workspace `geom` (after the order stage),
     adding the hits of record i to weights[i*w_stride + ch] and cnt[i*c_stride]. `get(name, numel, dtype, grow)`
-    supplies the binning and image scratch, sized from the settings `s` (not from a frame size fixed elsewhere)."""
+    supplies the binning and image scratch, sized from the settings `s` (not from a frame size fixed elsewhere).
+    `deterministic` (gsr_shard_apply_weights_deterministic) needs packed weights, w_stride == CH."""
     lib = _lib.load()
     device = geom.device
     W, H = int(s.image_width), int(s.image_height)
@@ -423,20 +463,25 @@ def owner_apply_weights(s, own, P: int, R: int, geom: torch.Tensor, radii: torch
         ibytes = lib.gsr_image_bytes(W, H)
         img = get("img", ibytes, torch.uint8, 1.0)
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-        _lib.check(lib.gsr_shard_apply_weights(C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning),
-                                               bbytes, _ptr(img), ibytes, _ptr(radii), _ptr(image_weights), CH,
-                                               _ptr(weights), w_stride, _ptr(cnt), c_stride, st),
-                   "gsr_shard_apply_weights")
+        args = (C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), bbytes, _ptr(img), ibytes,
+                _ptr(radii), _ptr(image_weights), CH, _ptr(weights), w_stride, _ptr(cnt), c_stride)
+        if deterministic:
+            dbytes = lib.gsr_deterministic_scratch_bytes(P, R, CH)
+            det = get("det", dbytes, torch.uint8, 1.25)
+            _lib.check(lib.gsr_shard_apply_weights_deterministic(*args, _ptr(det), dbytes, st),
+                       "gsr_shard_apply_weights_deterministic")
+        else:
+            _lib.check(lib.gsr_shard_apply_weights(*args, st), "gsr_shard_apply_weights")
 
 
 def shard_apply_weights(buf: ShardBuffers, image_weights: torch.Tensor, weights_total: torch.Tensor,
-                        cnt_total: torch.Tensor):
+                        cnt_total: torch.Tensor, deterministic: bool = False):
     """Semantic tracing of the owned tiles (after shard_order): adds into `weights_total` [P_pad, CH] float32 and
     `cnt_total` [P_pad] int32, indexed by global Gaussian index (the caller zero-fills them)."""
     device = buf.geom.device
     owner_apply_weights(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.radii, _f32c(image_weights, device),
                         weights_total, int(image_weights.size(0)), cnt_total, 1,
-                        lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow))
+                        lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow), deterministic)
 
 
 def check_apply_weights_args(plan: ShardPlan, rs, means3D, weights, cnt, image_weights, scales, rotations,
@@ -469,10 +514,11 @@ def check_apply_weights_args(plan: ShardPlan, rs, means3D, weights, cnt, image_w
 
 
 def dense_apply_weights(plan: ShardPlan, exchange: "Exchange", pool: "WorkspacePool", rs, means3D, opacities, scales,
-                        rotations, cov3Ds_precomp, image_weights, weights, cnt):
+                        rotations, cov3Ds_precomp, image_weights, weights, cnt, deterministic: bool = False):
     """One view of semantic tracing in the dense exchange: preprocess -> all-gather (or barrier) -> order -> walk of
     the owned tiles into zeroed [P_pad, CH] / [P_pad] buffers -> reduce-scatter of both (cnt stays int32) -> this
-    rank's slices added into `weights` / `cnt`."""
+    rank's slices added into `weights` / `cnt`. `deterministic`: deterministic walk and the weights reduce-scattered
+    in ascending rank order (the integer counts are exact either way)."""
     device = means3D.device
     empty = torch.empty(0, dtype=torch.float32, device=device)
     CH = int(image_weights.size(0))
@@ -487,10 +533,10 @@ def dense_apply_weights(plan: ShardPlan, exchange: "Exchange", pool: "WorkspaceP
         shard_order(buf)
         w_total = buf.alloc("aw_weights", plan.P_pad * CH, torch.float32, device).view(plan.P_pad, CH).zero_()
         c_total = buf.alloc("aw_cnt", plan.P_pad, torch.int32, device).zero_()
-        shard_apply_weights(buf, image_weights, w_total, c_total)
+        shard_apply_weights(buf, image_weights, w_total, c_total, deterministic)
         w_slice = buf.alloc("aw_weights_slice", plan.slice_len * CH, torch.float32, device).view(plan.slice_len, CH)
         c_slice = buf.alloc("aw_cnt_slice", plan.slice_len, torch.int32, device)
-        exchange.reduce_scatter_sum(w_total, w_slice)
+        (exchange.reduce_scatter_ordered if deterministic else exchange.reduce_scatter_sum)(w_total, w_slice)
         exchange.reduce_scatter_sum(c_total, c_slice)
         n = plan.count
         weights.view(n, CH).add_(w_slice[:n])
@@ -505,7 +551,7 @@ def dense_apply_weights(plan: ShardPlan, exchange: "Exchange", pool: "WorkspaceP
 class _ShardedRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, plan,
-                exchange, pool):
+                exchange, pool, deterministic=False):
         ws = pool.take(means3D.device) if pool is not None else None
         buf = shard_preprocess(plan, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                ws=ws)
@@ -519,7 +565,7 @@ class _ShardedRasterize(torch.autograd.Function):
         frame = torch.zeros(4, buf.H, buf.W, dtype=torch.float32, device=means3D.device)
         shard_render(buf, frame[:3], frame[3:])
         exchange.all_reduce_sum(frame)
-        ctx.buf, ctx.exchange = buf, exchange
+        ctx.buf, ctx.exchange, ctx.deterministic = buf, exchange, deterministic
         # a fresh tensor, like the single-GPU path and the reference: buf.radii lives in the pooled StepWorkspace and is
         # overwritten by the next forward that takes that workspace
         radii = shard_slice(buf.radii, plan).clone()
@@ -529,13 +575,13 @@ class _ShardedRasterize(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_out_color, grad_radii, grad_depth):
-        buf, exchange = ctx.buf, ctx.exchange
-        acc = shard_backward_render(buf, grad_out_color)
+        buf, exchange, det = ctx.buf, ctx.exchange, ctx.deterministic
+        acc = shard_backward_render(buf, grad_out_color, det)
         acc_slice = buf.alloc("acc_slice", buf.plan.slice_len * ACC_STRIDE, torch.float32,
                               acc.device).view(buf.plan.slice_len, ACC_STRIDE)
-        exchange.reduce_scatter_sum(acc, acc_slice)
+        (exchange.reduce_scatter_ordered if det else exchange.reduce_scatter_sum)(acc, acc_slice)
         grads = shard_backward_preprocess(buf, acc_slice)
-        return (*grads, None, None, None, None)
+        return (*grads, None, None, None, None, None)
 
 
 def p2p_available(exchange: "Exchange") -> bool:
@@ -557,13 +603,14 @@ def p2p_available(exchange: "Exchange") -> bool:
 
 
 def _check_deterministic_flag():
-    """The sharded backward and apply_weights add rows with float atomics, whose order changes from call to call. Under
-    ``torch.use_deterministic_algorithms(True)`` that is an error (a warning with ``warn_only=True``), as for any PyTorch op
-    without a deterministic implementation; the single-GPU ``GaussianRasterizer`` has one."""
+    """By default the sharded backward and apply_weights add rows with float atomics, whose order changes from call to
+    call. Under ``torch.use_deterministic_algorithms(True)`` that is an error (a warning with ``warn_only=True``), as for
+    any PyTorch op without a deterministic implementation, unless the module was built with ``deterministic=True``."""
     if not torch.are_deterministic_algorithms_enabled():
         return
-    msg = ("ShardedGaussianRasterizer does not have a deterministic implementation: its backward and apply_weights add "
-           "with float atomics. Use the single-GPU GaussianRasterizer (deterministic mode) or turn the flag off with "
+    msg = ("ShardedGaussianRasterizer(deterministic=None/False) is not deterministic: its backward and apply_weights add "
+           "with float atomics. Construct it with deterministic=True (results reproducible for a fixed number of ranks), "
+           "use the single-GPU GaussianRasterizer (deterministic mode) or turn the flag off with "
            "torch.use_deterministic_algorithms(False).")
     if torch.is_deterministic_algorithms_warn_only_enabled():
         warnings.warn(msg)
@@ -582,12 +629,20 @@ class ShardedGaussianRasterizer(nn.Module):
     sorts and reduces all P_total records (fused peer-store all-gather with ``p2p=True``, NCCL all-gather otherwise).
     ``max_in_flight``: forwards whose autograd state may be alive at the same time (GaussianEditor: 2; the peer-mapped
     workspaces are created collectively up front, one per slot).
+    ``deterministic``: ``True`` selects the deterministic backward and ``apply_weights`` (no float atomics, partial
+    sums of the ranks added in ascending rank order) in both modes and lets ``torch.use_deterministic_algorithms(True)``
+    pass. Gradients, ``weights`` and ``cnt`` are then the same bits on every call and in every process for a FIXED
+    number of ranks, and the dense and sparse modes give the same bits; at one rank they equal
+    ``GaussianRasterizer(deterministic=True)``. With more ranks they are not the single-GPU bits (the sums are grouped
+    per rank). ``None`` / ``False``: float atomics, and torch's deterministic flag raises (or warns).
     """
 
     def __init__(self, raster_settings: GaussianRasterizationSettings, P_total: int, group=None,
-                 p2p: Optional[bool] = None, mode: Optional[str] = None, max_in_flight: int = 3):
+                 p2p: Optional[bool] = None, mode: Optional[str] = None, max_in_flight: int = 3,
+                 deterministic: Optional[bool] = None):
         super().__init__()
         self.raster_settings = raster_settings
+        self.deterministic = bool(deterministic)
         self.exchange = Exchange(group)
         self.plan = ShardPlan(int(P_total), self.exchange.world, self.exchange.rank)
         can_p2p = p2p_available(self.exchange) if (p2p is None or p2p or mode == "sparse") else False
@@ -620,7 +675,8 @@ class ShardedGaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
-        _check_deterministic_flag()
+        if not getattr(self, "deterministic", False):
+            _check_deterministic_flag()
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
             raise Exception("Please provide excatly one of either SHs or precomputed colors!")
         if ((scales is None or rotations is None) and cov3D_precomp is None) or (
@@ -639,17 +695,20 @@ class ShardedGaussianRasterizer(nn.Module):
             if int(rs.image_width) != rk0.W or int(rs.image_height) != rk0.H:
                 raise RuntimeError("sparse mode: the image size is fixed at construction (peer-mapped frames)")
             return SS._SparseShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                                    cov3D_precomp, rs, self.sparse_pool, self.exchange)
+                                                    cov3D_precomp, rs, self.sparse_pool, self.exchange,
+                                                    self.deterministic)
         return _ShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                       cov3D_precomp, rs, self.plan, self.exchange, self.pool)
+                                       cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic)
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):
         """Semantic tracing of the sharded cloud (``GaussianRasterizer.apply_weights``, collective: every rank calls it
         for the same view). The per-Gaussian tensors, ``weights`` [n,CH] float32 and ``cnt`` [n,1] int32 are THIS RANK's
         rows and are updated in place (accumulated over calls); ``image_weights`` [CH,H,W] is the full mask, the same on
-        every rank. ``cnt`` equals the single-GPU result bit for bit, ``weights`` up to the order of the float sums."""
-        _check_deterministic_flag()
+        every rank. ``cnt`` equals the single-GPU result bit for bit, ``weights`` up to the order of the float sums
+        (bit for bit from call to call with ``deterministic=True``)."""
+        if not getattr(self, "deterministic", False):
+            _check_deterministic_flag()
         rs = self.raster_settings
         check_apply_weights_args(self.plan, rs, means3D, weights, cnt, image_weights, scales, rotations, cov3Ds_precomp)
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
@@ -660,10 +719,10 @@ class ShardedGaussianRasterizer(nn.Module):
             if self.mode == "sparse":
                 from . import sparse_sharded as SS
                 SS.sparse_apply_weights(self.sparse_pool, rs, means3D, opacities, scales, rotations, cov3Ds_precomp,
-                                        image_weights, weights, cnt)
+                                        image_weights, weights, cnt, self.deterministic)
             else:
                 dense_apply_weights(self.plan, self.exchange, self.pool, rs, means3D, opacities, scales, rotations,
-                                    cov3Ds_precomp, image_weights, weights, cnt)
+                                    cov3Ds_precomp, image_weights, weights, cnt, self.deterministic)
 
     def markVisible(self, positions):
         """``GaussianRasterizer.markVisible`` of this rank's rows ``positions`` [n,3] (no collective)."""

@@ -241,19 +241,17 @@ def peer_barrier(rk: SparseRank, with_row: bool = False):
                                         1 if with_row else 0, stream), "gsr_peer_barrier")
 
 
-def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor) -> torch.Tensor:
+def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, deterministic: bool = False) -> torch.Tensor:
+    """Blend backward of the owned tiles into the candidate accumulators [world*cap, 12] (deterministic: no float
+    atomics, every row written)."""
+    from .sharded import owner_backward_render
     lib = _lib.load()
     rk = st.rk
-    with torch.cuda.device(rk.device):
-        M = rk.plan.world * st.cap
-        grad_out_color = _f32c(grad_out_color, rk.device)
-        acc = rk.get("acc", M * ACC_STRIDE, torch.float32, grow=1.25).view(M, ACC_STRIDE)
-        own = rk.plan.owner()
-        stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
-        gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
-        _lib.check(lib.gsr_shard_backward_render(C.byref(st.s), C.byref(own), M, st.R, _ptr(rk.cand), gb, _ptr(st.binning),
-                                                 st.binning.numel(), _ptr(st.img), st.img.numel(), _ptr(grad_out_color),
-                                                 _ptr(acc), acc.numel() * 4, stream), "gsr_shard_backward_render")
+    M = rk.plan.world * st.cap
+    acc = rk.get("acc", M * ACC_STRIDE, torch.float32, grow=1.25).view(M, ACC_STRIDE)
+    gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
+    owner_backward_render(st.s, rk.plan.owner(), M, st.R, rk.cand[:gb], st.binning, st.img, grad_out_color, acc,
+                          deterministic, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow))
     return acc
 
 
@@ -370,15 +368,21 @@ def _preprocess_and_order(rk: SparseRank, pool: SparsePool, rs, means3D, sh, col
     return st, R, max_count
 
 
-def apply_weights_walk(st: SparseStep, image_weights: torch.Tensor, acc: torch.Tensor):
+def apply_weights_walk(st: SparseStep, image_weights: torch.Tensor, acc: torch.Tensor, deterministic: bool = False):
     """Semantic tracing of the owned tiles of the candidate cloud into the zeroed rows `acc` [world*cap, 12]: weights in
-    floats 0..CH-1, the count as int32 bits in float GSR_SPARSE_AW_CNT_SLOT (so that sparse_return carries it exactly)."""
+    floats 0..CH-1, the count as int32 bits in float GSR_SPARSE_AW_CNT_SLOT (so that sparse_return carries it exactly).
+    Deterministic mode reduces the weights into a packed zeroed [world*cap, CH] buffer and copies them into the rows."""
     from .sharded import owner_apply_weights
     rk = st.rk
     M = rk.plan.world * st.cap
-    owner_apply_weights(st.s, rk.plan.owner(), M, st.R, rk.cand, st.radii_cand, _f32c(image_weights, rk.device), acc,
-                        ACC_STRIDE, acc.view(torch.int32)[:, AW_CNT_SLOT], ACC_STRIDE,
-                        lambda name, n, dtype, grow: rk.get(name, n, dtype, grow))
+    CH = int(image_weights.size(0))
+    get = lambda name, n, dtype, grow: rk.get(name, n, dtype, grow)
+    weights = rk.get("aw_det_weights", M * CH, torch.float32, grow=1.25).view(M, CH).zero_() if deterministic else acc
+    owner_apply_weights(st.s, rk.plan.owner(), M, st.R, rk.cand, st.radii_cand, _f32c(image_weights, rk.device), weights,
+                        CH if deterministic else ACC_STRIDE, acc.view(torch.int32)[:, AW_CNT_SLOT], ACC_STRIDE, get,
+                        deterministic)
+    if deterministic:
+        acc[:, :CH].copy_(weights)
 
 
 def apply_weights_gather(st: SparseStep, weights: torch.Tensor, cnt: torch.Tensor):
@@ -396,11 +400,12 @@ def apply_weights_gather(st: SparseStep, weights: torch.Tensor, cnt: torch.Tenso
 
 
 def sparse_apply_weights(pool: SparsePool, rs, means3D, opacities, scales, rotations, cov3Ds_precomp, image_weights,
-                         weights, cnt):
+                         weights, cnt, deterministic: bool = False):
     """One view of semantic tracing with the sparse exchange (arguments checked by the caller): preprocess + push --
     barrier -- order (as the forward) -> walk of the owned tiles into zeroed candidate rows -> return -- barrier --
     gather into this rank's `weights` / `cnt`. A rank without owned tile rows or instances still takes part in every
-    barrier. The workspace goes back to the pool before returning."""
+    barrier. The workspace goes back to the pool before returning. The gather adds in ascending rank order, so
+    `deterministic` only changes the walk."""
     rk = pool.take()
     empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
     _mark("start")
@@ -410,7 +415,7 @@ def sparse_apply_weights(pool: SparsePool, rs, means3D, opacities, scales, rotat
                                          cov3Ds_precomp)
         M = rk.plan.world * st.cap
         acc = rk.get("acc", M * ACC_STRIDE, torch.float32, grow=1.25).view(M, ACC_STRIDE).zero_()
-        apply_weights_walk(st, image_weights, acc)
+        apply_weights_walk(st, image_weights, acc, deterministic)
         _mark("walk")
         sparse_return(st, acc)
         peer_barrier(rk)
@@ -423,7 +428,8 @@ def sparse_apply_weights(pool: SparsePool, rs, means3D, opacities, scales, rotat
 
 class _SparseShardedRasterize(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange):
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange,
+                deterministic=False):
         rk = pool.take()
         device = means3D.device
         _mark("start")
@@ -443,7 +449,7 @@ class _SparseShardedRasterize(torch.autograd.Function):
         peer_barrier(rk)
         out = frame.clone()                                 # the peer-visible frame is overwritten by the next step
         _mark("frame broadcast+barrier")
-        ctx.st, ctx.exchange = st, exchange
+        ctx.st, ctx.exchange, ctx.deterministic = st, exchange, deterministic
         radii = rk.radii_local[:rk.plan.count].clone()
         ctx.mark_non_differentiable(radii)
         _SparseShardedRasterize.last = dict(R=R, cap=st.cap, max_count=max_count)
@@ -455,7 +461,7 @@ class _SparseShardedRasterize(torch.autograd.Function):
         if st is None:
             raise RuntimeError("the sharded rasterizer's backward can run once (its workspace went back to the pool)")
         _mark("loss")
-        acc = sparse_backward_render(st, grad_out_color)
+        acc = sparse_backward_render(st, grad_out_color, ctx.deterministic)
         _mark("blend backward")
         sparse_return(st, acc)
         peer_barrier(st.rk)
@@ -463,4 +469,4 @@ class _SparseShardedRasterize(torch.autograd.Function):
         grads = sparse_backward_preprocess(st)
         _mark("gather+preprocess backward")
         ctx.st = None   # the workspace goes back to the pool now, not when the output tensors die
-        return (*grads, None, None, None)
+        return (*grads, None, None, None, None)

@@ -206,7 +206,8 @@ GSR_API int gsr_backward_depth(const gsr_settings* s, const gsr_cloud* c, int32_
  * gsr_backward_deterministic takes the arguments of gsr_backward_depth, with dL_dout_depth allowed to be NULL (no
  * depth gradient), so it covers the plain, alpha, camera and depth combinations; gsr_backward_raw_deterministic is
  * the same for gsr_backward_raw_depth (fused activations, below). cnt of apply_weights is integer and was already
- * exact. Single-GPU only: the Gaussian-sharded entry points keep their atomics. */
+ * exact. The Gaussian-sharded path has its own deterministic entry points (gsr_shard_backward_render_deterministic,
+ * gsr_shard_apply_weights_deterministic, below). */
 GSR_API size_t gsr_deterministic_scratch_bytes(int32_t P, int64_t num_rendered, int32_t num_channels);
 GSR_API int gsr_backward_deterministic(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered,
                                const void* geometry, size_t geometry_bytes, const void* binning,
@@ -367,6 +368,33 @@ GSR_API int gsr_shard_apply_weights(const gsr_settings* s, const gsr_tile_owner*
                                     size_t binning_bytes, void* image, size_t image_bytes, const int32_t* radii_total,
                                     const float* image_weights, int32_t num_channels, float* weights_total,
                                     int64_t weights_stride, int32_t* cnt_total, int64_t cnt_stride, void* stream);
+/* Deterministic mode of the two sharded stages that add with float atomics (see gsr_backward_deterministic). Each
+ * instance of the owned tile rows stores its rows at its slot in this rank's emission order and one kernel adds every
+ * Gaussian's rows in a fixed order, so this rank's partial sums are bit-identical from call to call; a host that also
+ * adds the ranks' partial rows in a fixed order (ascending rank: the sparse gathers do, a reduce-scatter does not
+ * promise it) gets bit-reproducible results for a fixed number of ranks. They are not the single-GPU bits: the sums
+ * are grouped per rank. det_scratch: gsr_deterministic_scratch_bytes(P_total, num_rendered, CH) bytes (CH = 0 for the
+ * backward), contents irrelevant. All arguments are checked before any device work.
+ *   gsr_shard_backward_render_deterministic: the arguments of gsr_shard_backward_render; it writes every one of the
+ *       P_total accumulator rows (zeros for a Gaussian without hits on this rank).
+ *   gsr_shard_apply_weights_deterministic: the arguments of gsr_shard_apply_weights, but weights_total must be packed,
+ *       weights_stride == num_channels (the reduction adds into [P_total, CH]); weights are still accumulated and cnt
+ *       keeps its exact int32 atomics. With the sparse exchange, reduce into a separate zeroed [world*seg_cap, CH]
+ *       buffer, keep the count in the candidate rows (cnt_total = (int32_t*)(acc + GSR_SPARSE_AW_CNT_SLOT),
+ *       cnt_stride = 12) and copy the weights into floats 0..CH-1 of those rows before gsr_sparse_return. */
+GSR_API int gsr_shard_backward_render_deterministic(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                                    int32_t num_rendered, const void* geometry, size_t geometry_bytes,
+                                                    const void* binning, size_t binning_bytes, const void* image,
+                                                    size_t image_bytes, const float* dL_dout_color, void* acc_total,
+                                                    size_t acc_bytes, void* det_scratch, size_t det_scratch_bytes,
+                                                    void* stream);
+GSR_API int gsr_shard_apply_weights_deterministic(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                                  int32_t num_rendered, void* geometry, size_t geometry_bytes,
+                                                  void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                                                  const int32_t* radii_total, const float* image_weights,
+                                                  int32_t num_channels, float* weights_total, int64_t weights_stride,
+                                                  int32_t* cnt_total, int64_t cnt_stride, void* det_scratch,
+                                                  size_t det_scratch_bytes, void* stream);
 
 /* ---- fused preprocess + all-gather over NVLink peer memory ---------------------------------------------------
  * Instead of gsr_shard_preprocess followed by an all-gather, every rank's preprocess kernel pushes its block of

@@ -57,6 +57,61 @@ def check_apply_weights(rast, full, loc, cams, bg, sh_degree, dev):
     return ok, f" apply_weights_worst_rel_l2={worst:.2e}"
 
 
+def check_deterministic(a, cloud, cams, bg, dL, dev, rank, world):
+    """ShardedGaussianRasterizer(deterministic=True) under torch's deterministic flag: two identical fwd+bwd steps and
+    two identical traces (two views, CH = 1 binary and CH = 3 float masks) must give the same bits; at world 1 they must
+    also equal GaussianRasterizer(deterministic=True). Returns (ok, digest of every rank's results, message)."""
+    import hashlib
+    P = cloud.means3D.shape[0]
+    rs = settings_from(cams[0], bg, cloud.sh_degree, dev)
+    view_rs = [settings_from(cam, bg, cloud.sh_degree, dev) for cam in cams[:2]]
+    torch.use_deterministic_algorithms(True)
+    if a.no_fill:
+        from torch.utils import deterministic as torch_det
+        torch_det.fill_uninitialized_memory = False
+    rast = S.ShardedGaussianRasterizer(rs, P, p2p=(True if a.mode == 'sparse' else a.p2p), mode=a.mode,
+                                       deterministic=True)
+    plan = rast.plan
+    full = cloud_tensors(cloud, dev)
+
+    def step(r, tensors):
+        leaves = {k: v.detach().clone().requires_grad_(True) for k, v in tensors.items()}
+        m2 = torch.zeros_like(leaves["means3D"], requires_grad=True)
+        color, _, _ = r(means3D=leaves["means3D"], means2D=m2, opacities=leaves["opacities"], shs=leaves["shs"],
+                        scales=leaves["scales"], rotations=leaves["rotations"])
+        (color * dL).sum().backward()
+        out = {k: v.grad for k, v in leaves.items()}
+        out["means2D"] = m2.grad
+        for CH, binary in ((1, True), (3, False)):
+            n = tensors["means3D"].shape[0]
+            w = torch.zeros(n, CH, device=dev); c = torch.zeros(n, 1, dtype=torch.int32, device=dev)
+            for i, cam in enumerate(cams[:2]):
+                r.raster_settings = view_rs[i]
+                g = torch.Generator().manual_seed(100 * CH + i)
+                m = torch.rand(CH, cam.image_height, cam.image_width, generator=g)
+                iw = ((m > 0.5).float() if binary else m).to(dev)
+                r.apply_weights(tensors["means3D"], None, tensors["opacities"], None, w, tensors["scales"],
+                                tensors["rotations"], None, c, iw)
+            r.raster_settings = rs
+            out[f"weights{CH}"], out[f"cnt{CH}"] = w, c
+        torch.cuda.synchronize()
+        return {k: v.detach().cpu().clone() for k, v in out.items()}
+
+    loc = {k: S.shard_slice(v, plan) for k, v in full.items()}
+    runs = [step(rast, loc) for _ in range(2)]
+    bits = lambda d: {k: v.numpy().tobytes() for k, v in d.items()}
+    ok = bits(runs[0]) == bits(runs[1])
+    if world == 1:
+        ref = step(GaussianRasterizer(rs, deterministic=True), full)
+        ok = ok and all(torch.equal(runs[0][k], ref[k]) for k in ref)
+    mine = hashlib.sha256(b"".join(v for _, v in sorted(bits(runs[0]).items()))).hexdigest()
+    digests = [None] * world
+    dist.all_gather_object(digests, mine)
+    rast.close()
+    torch.use_deterministic_algorithms(False)
+    return ok, hashlib.sha256("".join(digests).encode()).hexdigest(), " deterministic=" + ("ok" if ok else "FAILED")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="c3")
@@ -65,6 +120,11 @@ def main():
     ap.add_argument("--mode", default="dense", choices=["dense", "sparse"])
     ap.add_argument("--apply-weights", action="store_true",
                     help="also check semantic tracing (CH = 1 and 3) and markVisible against the full cloud")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="also check deterministic=True under torch's deterministic flag (repeatable bits; at world 1 "
+                         "the single-GPU deterministic bits); prints DETERMINISTIC_DIGEST")
+    ap.add_argument("--no-fill", action="store_true",
+                    help="with --deterministic: torch.utils.deterministic.fill_uninitialized_memory = False")
     a = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     dev = torch.device("cuda", local)
@@ -129,6 +189,11 @@ def main():
     if a.apply_weights:
         aw_ok, aw_msg = check_apply_weights(rast, full, loc, cams, bg, cloud.sh_degree, dev)
         ok = ok and aw_ok
+    det_digest = None
+    if a.deterministic:
+        det_ok, det_digest, det_msg = check_deterministic(a, cloud, cams, bg, dL, dev, rank, world)
+        ok = ok and det_ok
+        aw_msg += det_msg
     flag = torch.tensor([1 if ok else 0], device=dev)
     dist.all_reduce(flag, op=dist.ReduceOp.MIN)
     if rank == 0:
@@ -139,6 +204,8 @@ def main():
         else:
             extra = f" R_rank0={S._ShardedRasterize.last_R}"
         print(f"world={world} mode={a.mode} p2p={a.p2p} P={P}{extra} worst_grad_rel_l2={worst:.2e}{aw_msg}")
+        if det_digest is not None:
+            print(f"DETERMINISTIC_DIGEST {det_digest}")
         print("SHARDED_CHECK_OK" if int(flag) == 1 else "SHARDED_CHECK_FAILED")
     del scolor, sradii, sdepth
     import gc
