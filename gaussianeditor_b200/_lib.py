@@ -33,6 +33,9 @@ SYMBOLS = [
     "gsr_apply_weights_deterministic",
     "gsr_shard_apply_weights", "gsr_sparse_apply_weights_gather",
     "gsr_shard_backward_render_deterministic", "gsr_shard_apply_weights_deterministic",
+    "gsr_shard_preprocess_raw", "gsr_shard_preprocess_p2p_raw", "gsr_sparse_preprocess_raw",
+    "gsr_shard_backward_render_depth", "gsr_shard_backward_preprocess_depth", "gsr_sparse_backward_preprocess_depth",
+    "gsr_shard_backward_preprocess_raw", "gsr_sparse_backward_preprocess_raw",
 ]
 
 
@@ -208,6 +211,17 @@ def load():
     lib.gsr_peer_free.restype = C.c_int; lib.gsr_peer_free.argtypes = [vp]
     lib.gsr_shard_preprocess_p2p.restype = C.c_int
     lib.gsr_shard_preprocess_p2p.argtypes = [S, Cl, i32, i32, i32, C.POINTER(vp), i32, i32, sz, vp, vp]
+    RC, RG = C.POINTER(RawCloud), C.POINTER(RawGrads)
+    lib.gsr_shard_preprocess_raw.restype = C.c_int
+    lib.gsr_shard_preprocess_raw.argtypes = [S, RC, i32, i32, i32, vp, sz, vp, vp]
+    lib.gsr_shard_preprocess_p2p_raw.restype = C.c_int
+    lib.gsr_shard_preprocess_p2p_raw.argtypes = [S, RC, i32, i32, i32, C.POINTER(vp), i32, i32, sz, vp, vp]
+    lib.gsr_shard_backward_render_depth.restype = C.c_int
+    lib.gsr_shard_backward_render_depth.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, sz, vp, sz, vp]
+    lib.gsr_shard_backward_preprocess_depth.restype = C.c_int
+    lib.gsr_shard_backward_preprocess_depth.argtypes = lib.gsr_shard_backward_preprocess.argtypes
+    lib.gsr_shard_backward_preprocess_raw.restype = C.c_int
+    lib.gsr_shard_backward_preprocess_raw.argtypes = [S, RC, i32, i32, vp, sz, vp, vp, RG, i32, vp]
     lib.gsr_forward_preprocess_raw.restype = C.c_int
     lib.gsr_forward_preprocess_raw.argtypes = [S, C.POINTER(RawCloud), vp, sz, vp, vp, vp]
     lib.gsr_backward_raw.restype = C.c_int
@@ -231,6 +245,12 @@ def load():
     lib.gsr_sparse_return.argtypes = [SP, vp, vp, C.POINTER(vp), vp]
     lib.gsr_sparse_backward_preprocess.restype = C.c_int
     lib.gsr_sparse_backward_preprocess.argtypes = [S, Cl, SP, vp, sz, vp, vp, sz, vp, sz, C.POINTER(Grads), vp]
+    lib.gsr_sparse_preprocess_raw.restype = C.c_int
+    lib.gsr_sparse_preprocess_raw.argtypes = [S, RC, SP, vp, sz, vp, C.POINTER(vp), sz, vp, vp]
+    lib.gsr_sparse_backward_preprocess_depth.restype = C.c_int
+    lib.gsr_sparse_backward_preprocess_depth.argtypes = lib.gsr_sparse_backward_preprocess.argtypes
+    lib.gsr_sparse_backward_preprocess_raw.restype = C.c_int
+    lib.gsr_sparse_backward_preprocess_raw.argtypes = [S, RC, SP, vp, sz, vp, vp, sz, vp, sz, RG, i32, vp]
     lib.gsr_sparse_apply_weights_gather.restype = C.c_int
     lib.gsr_sparse_apply_weights_gather.argtypes = [SP, vp, sz, vp, sz, i32, i32, vp, vp, vp]
     lib.gsr_peer_barrier.restype = C.c_int

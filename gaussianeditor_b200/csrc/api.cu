@@ -82,6 +82,46 @@ int validate_cloud(const gsr_settings* s, const gsr_cloud* c) {
   return GSR_OK;
 }
 
+// ---- fused activations (raw parameters): the checks shared by the single-GPU and the sharded entry points ----------
+int raw_to_cloud(const gsr_settings* s, const gsr_raw_cloud* r, gsr_cloud& c) {
+  if (!s || !r) { set_error("null settings/cloud"); return GSR_ERR_INVALID; }
+  c = gsr_cloud{};
+  c.P = r->P; c.means3D = r->means3D; c.opacities = r->opacity_logits; c.shs = r->features_dc;
+  c.scales = r->log_scales; c.rotations = r->raw_rotations;
+  int rc = validate_cloud(s, &c);
+  if (rc) return rc;
+  if (r->P > 0 && s->sh_coeffs > 1 && !r->features_rest) { set_error("features_rest is null but sh_coeffs = %d", s->sh_coeffs); return GSR_ERR_INVALID; }
+  if (r->features_rest && (reinterpret_cast<uintptr_t>(r->features_rest) & 15)) { set_error("features_rest must be 16-byte aligned"); return GSR_ERR_INVALID; }
+  return GSR_OK;
+}
+
+int check_raw_grads(const gsr_settings* s, const gsr_raw_grads* gr) {
+  if (!gr->dL_dmeans3D || !gr->dL_dmeans2D || !gr->dL_dopacity_logits || !gr->dL_dfeatures_dc || !gr->dL_dlog_scales ||
+      !gr->dL_draw_rotations || (s->sh_coeffs > 1 && !gr->dL_dfeatures_rest)) {
+    set_error("a gradient output pointer is null");
+    return GSR_ERR_INVALID;
+  }
+  if ((reinterpret_cast<uintptr_t>(gr->dL_draw_rotations) & 15) || (reinterpret_cast<uintptr_t>(gr->dL_dfeatures_rest) & 15)) {
+    set_error("dL_draw_rotations / dL_dfeatures_rest must be 16-byte aligned");
+    return GSR_ERR_INVALID;
+  }
+  return GSR_OK;
+}
+
+gsr_grads raw_grads_as_full(const gsr_raw_grads& gr) {
+  gsr_grads full{};
+  full.dL_dmeans3D = gr.dL_dmeans3D; full.dL_dmeans2D = gr.dL_dmeans2D; full.dL_dopacity = gr.dL_dopacity_logits;
+  full.dL_dsh = gr.dL_dfeatures_dc; full.dL_dscales = gr.dL_dlog_scales; full.dL_drotations = gr.dL_draw_rotations;
+  return full;
+}
+
+int shard_cloud(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw, gsr_cloud& c) {
+  if (raw) return raw_to_cloud(s, raw, c);
+  const int rc = validate_cloud(s, shard);
+  if (rc == GSR_OK) c = *shard;
+  return rc;
+}
+
 }  // namespace gsr
 
 using namespace gsr;
@@ -392,18 +432,6 @@ int gsr_apply_weights_deterministic(const gsr_settings* s, const gsr_cloud* c, i
 }
 
 // ---- fused activations (raw parameters) --------------------------------------------------------------------
-static int raw_to_cloud(const gsr_settings* s, const gsr_raw_cloud* r, gsr_cloud& c) {
-  if (!s || !r) { set_error("null settings/cloud"); return GSR_ERR_INVALID; }
-  c = gsr_cloud{};
-  c.P = r->P; c.means3D = r->means3D; c.opacities = r->opacity_logits; c.shs = r->features_dc;
-  c.scales = r->log_scales; c.rotations = r->raw_rotations;
-  int rc = validate_cloud(s, &c);
-  if (rc) return rc;
-  if (r->P > 0 && s->sh_coeffs > 1 && !r->features_rest) { set_error("features_rest is null but sh_coeffs = %d", s->sh_coeffs); return GSR_ERR_INVALID; }
-  if (r->features_rest && (reinterpret_cast<uintptr_t>(r->features_rest) & 15)) { set_error("features_rest must be 16-byte aligned"); return GSR_ERR_INVALID; }
-  return GSR_OK;
-}
-
 int gsr_forward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* r, void* geometry, size_t geometry_bytes,
                                int32_t* radii, int32_t* num_rendered_host, void* stream) {
   gsr_cloud c;
@@ -429,15 +457,7 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
   if (rc) return rc;
   if (!gr || !dL_dout_color) { set_error("grads / dL_dout_color is null"); return GSR_ERR_INVALID; }
   if (c.P == 0) return GSR_OK;
-  if (!gr->dL_dmeans3D || !gr->dL_dmeans2D || !gr->dL_dopacity_logits || !gr->dL_dfeatures_dc || !gr->dL_dlog_scales ||
-      !gr->dL_draw_rotations || (s->sh_coeffs > 1 && !gr->dL_dfeatures_rest)) {
-    set_error("a gradient output pointer is null");
-    return GSR_ERR_INVALID;
-  }
-  if ((reinterpret_cast<uintptr_t>(gr->dL_draw_rotations) & 15) || (reinterpret_cast<uintptr_t>(gr->dL_dfeatures_rest) & 15)) {
-    set_error("dL_draw_rotations / dL_dfeatures_rest must be 16-byte aligned");
-    return GSR_ERR_INVALID;
-  }
+  if ((rc = check_raw_grads(s, gr))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   GeometryWS g; BinningWS b; ImageWS im;
   rc = carve_all(s, &c, R, const_cast<void*>(geometry), geometry_bytes, const_cast<void*>(binning), binning_bytes,
@@ -459,9 +479,7 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
       if (rc) return rc;
     }
   }
-  gsr_grads full{};
-  full.dL_dmeans3D = gr->dL_dmeans3D; full.dL_dmeans2D = gr->dL_dmeans2D; full.dL_dopacity = gr->dL_dopacity_logits;
-  full.dL_dsh = gr->dL_dfeatures_dc; full.dL_dscales = gr->dL_dlog_scales; full.dL_drotations = gr->dL_draw_rotations;
+  const gsr_grads full = raw_grads_as_full(*gr);
   RawBackward raw{r->features_rest, gr->dL_dfeatures_rest};
   StageScope t(ST_PRE_BWD, st);
   return launch_preprocess_bwd(*s, c, g, radii, (const float*)scratch, full, st, &raw, nullptr, dL_dout_depth != nullptr);
@@ -524,12 +542,15 @@ int gsr_view_exchange(void* geometry, int32_t P_total, gsr_exchange_view* out) {
   return GSR_OK;
 }
 
-int gsr_shard_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
-                         int32_t slice_len, void* geometry, size_t geometry_bytes, int32_t* radii_total, void* stream) {
-  int rc = validate_cloud(s, shard);
+// gsr_shard_preprocess and, with `raw`, gsr_shard_preprocess_raw (`shard` unused)
+static int shard_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
+                                 int32_t P_total, int32_t index_base, int32_t slice_len, void* geometry,
+                                 size_t geometry_bytes, int32_t* radii_total, void* stream) {
+  gsr_cloud c;
+  int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
-  if (P_total <= 0 || index_base < 0 || slice_len < shard->P || (int64_t)index_base + slice_len > P_total) {
-    set_error("shard [%d, %d+%d) (P=%d) does not fit P_total=%d", index_base, index_base, slice_len, shard->P, P_total);
+  if (P_total <= 0 || index_base < 0 || slice_len < c.P || (int64_t)index_base + slice_len > P_total) {
+    set_error("shard [%d, %d+%d) (P=%d) does not fit P_total=%d", index_base, index_base, slice_len, c.P, P_total);
     return GSR_ERR_INVALID;
   }
   if (!radii_total || !geometry) { set_error("radii / geometry workspace is null"); return GSR_ERR_INVALID; }
@@ -538,16 +559,30 @@ int gsr_shard_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t 
   if (!carve_geometry(geometry, P_total, g)) return GSR_ERR_CUDA;
   if (g.total > geometry_bytes) { set_error("geometry workspace too small: %zu < %zu", geometry_bytes, g.total); return GSR_ERR_WORKSPACE; }
   StageScope t(ST_PRE_FWD, st);
-  if (shard->P > 0) {
-    rc = launch_preprocess_fwd(*s, *shard, slice_geometry(g, index_base), radii_total + index_base, st);
+  if (c.P > 0) {
+    rc = launch_preprocess_fwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, st, nullptr, 0,
+                               raw != nullptr, raw ? raw->features_rest : nullptr);
     if (rc) return rc;
   }
-  const int pad = slice_len - shard->P;  // slots of the slice behind the shard: culled (radius 0 in the record)
+  const int pad = slice_len - c.P;  // slots of the slice behind the shard: culled (radius 0 in the record)
   if (pad > 0) {
-    cudaError_t e = cudaMemsetAsync(g.records + index_base + shard->P, 0, (size_t)pad * sizeof(SplatRecord), st);
+    cudaError_t e = cudaMemsetAsync(g.records + index_base + c.P, 0, (size_t)pad * sizeof(SplatRecord), st);
     if (e != cudaSuccess) return check_cuda(e, "slice padding");
   }
   return GSR_OK;
+}
+
+int gsr_shard_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
+                         int32_t slice_len, void* geometry, size_t geometry_bytes, int32_t* radii_total, void* stream) {
+  return shard_preprocess_impl(s, shard, nullptr, P_total, index_base, slice_len, geometry, geometry_bytes, radii_total,
+                               stream);
+}
+
+int gsr_shard_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total, int32_t index_base,
+                             int32_t slice_len, void* geometry, size_t geometry_bytes, int32_t* radii_total,
+                             void* stream) {
+  return shard_preprocess_impl(s, nullptr, shard, P_total, index_base, slice_len, geometry, geometry_bytes, radii_total,
+                               stream);
 }
 
 int gsr_peer_alloc(size_t bytes, void** ptr_out, void* handle_out) {
@@ -577,17 +612,20 @@ int gsr_peer_open(const void* handle, void** ptr_out) {
 int gsr_peer_close(void* ptr) { return ptr ? check_cuda(cudaIpcCloseMemHandle(ptr), "cudaIpcCloseMemHandle") : GSR_OK; }
 int gsr_peer_free(void* ptr) { return ptr ? check_cuda(cudaFree(ptr), "peer_free") : GSR_OK; }
 
-int gsr_shard_preprocess_p2p(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
-                             int32_t slice_len, void* const* peer_geometry, int32_t world, int32_t rank,
-                             size_t geometry_bytes, int32_t* radii_total, void* stream) {
-  int rc = validate_cloud(s, shard);
+// gsr_shard_preprocess_p2p and, with `raw`, gsr_shard_preprocess_p2p_raw (`shard` unused)
+static int shard_preprocess_p2p_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
+                                     int32_t P_total, int32_t index_base, int32_t slice_len, void* const* peer_geometry,
+                                     int32_t world, int32_t rank, size_t geometry_bytes, int32_t* radii_total,
+                                     void* stream) {
+  gsr_cloud c;
+  int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
   if (world < 1 || world > GSR_MAX_PEERS || rank < 0 || rank >= world || !peer_geometry) {
     set_error("p2p preprocess: need 1 <= world <= %d, 0 <= rank < world", GSR_MAX_PEERS);
     return GSR_ERR_INVALID;
   }
-  if (P_total <= 0 || index_base < 0 || slice_len < shard->P || (int64_t)index_base + slice_len > P_total) {
-    set_error("shard [%d, %d+%d) (P=%d) does not fit P_total=%d", index_base, index_base, slice_len, shard->P, P_total);
+  if (P_total <= 0 || index_base < 0 || slice_len < c.P || (int64_t)index_base + slice_len > P_total) {
+    set_error("shard [%d, %d+%d) (P=%d) does not fit P_total=%d", index_base, index_base, slice_len, c.P, P_total);
     return GSR_ERR_INVALID;
   }
   if (!radii_total) { set_error("radii is null"); return GSR_ERR_INVALID; }
@@ -602,16 +640,31 @@ int gsr_shard_preprocess_p2p(const gsr_settings* s, const gsr_cloud* shard, int3
     dst[r] = gr.records + index_base;
   }
   StageScope t(ST_PRE_FWD, st);
-  if (shard->P > 0) {
-    rc = launch_preprocess_fwd(*s, *shard, slice_geometry(g, index_base), radii_total + index_base, st, dst, world);
+  if (c.P > 0) {
+    rc = launch_preprocess_fwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, st, dst, world,
+                               raw != nullptr, raw ? raw->features_rest : nullptr);
     if (rc) return rc;
   }
-  const int pad = slice_len - shard->P;
+  const int pad = slice_len - c.P;
   for (int r = 0; pad > 0 && r < world; r++) {
-    cudaError_t e = cudaMemsetAsync(dst[r] + shard->P, 0, (size_t)pad * sizeof(SplatRecord), st);
+    cudaError_t e = cudaMemsetAsync(dst[r] + c.P, 0, (size_t)pad * sizeof(SplatRecord), st);
     if (e != cudaSuccess) return check_cuda(e, "slice padding");
   }
   return GSR_OK;
+}
+
+int gsr_shard_preprocess_p2p(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
+                             int32_t slice_len, void* const* peer_geometry, int32_t world, int32_t rank,
+                             size_t geometry_bytes, int32_t* radii_total, void* stream) {
+  return shard_preprocess_p2p_impl(s, shard, nullptr, P_total, index_base, slice_len, peer_geometry, world, rank,
+                                   geometry_bytes, radii_total, stream);
+}
+
+int gsr_shard_preprocess_p2p_raw(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total, int32_t index_base,
+                                 int32_t slice_len, void* const* peer_geometry, int32_t world, int32_t rank,
+                                 size_t geometry_bytes, int32_t* radii_total, void* stream) {
+  return shard_preprocess_p2p_impl(s, nullptr, shard, P_total, index_base, slice_len, peer_geometry, world, rank,
+                                   geometry_bytes, radii_total, stream);
 }
 
 int gsr_shard_order(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, void* geometry,
@@ -665,7 +718,7 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
                                       const void* geometry, size_t geometry_bytes, const void* binning,
                                       size_t binning_bytes, const void* image, size_t image_bytes,
                                       const float* dL_dout_color, void* acc_total, size_t acc_bytes, void* stream,
-                                      const DetScratch* ds) {
+                                      const DetScratch* ds, const float* dL_dout_depth = nullptr) {
   int rc = check_settings(s);
   if (rc) return rc;
   TileOwner own;
@@ -689,8 +742,20 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
     if (e != cudaSuccess) return check_cuda(e, "accumulator memset");
   }
   if (R == 0) return GSR_OK;
-  return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own, nullptr, nullptr,
+  return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own, nullptr, dL_dout_depth,
                            ds ? &det : nullptr, P_total, R);
+}
+
+int gsr_shard_backward_render_depth(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                                    const void* geometry, size_t geometry_bytes, const void* binning,
+                                    size_t binning_bytes, const void* image, size_t image_bytes,
+                                    const float* dL_dout_color, const float* dL_dout_depth, void* acc_total,
+                                    size_t acc_bytes, void* det_scratch, size_t det_scratch_bytes, void* stream) {
+  if (!dL_dout_depth) { set_error("dL_dout_depth is null"); return GSR_ERR_INVALID; }
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  return shard_backward_render_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                    image_bytes, dL_dout_color, acc_total, acc_bytes, stream,
+                                    det_scratch ? &ds : nullptr, dL_dout_depth);
 }
 
 int gsr_shard_backward_render(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
@@ -774,28 +839,64 @@ int gsr_shard_apply_weights_deterministic(const gsr_settings* s, const gsr_tile_
                                   cnt_stride, stream, &ds);
 }
 
-int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
-                                  const void* geometry, size_t geometry_bytes, const int32_t* radii_total,
-                                  const void* acc_slice, const gsr_grads* gr, void* stream) {
-  int rc = validate_cloud(s, shard);
+// gsr_shard_backward_preprocess, its DEPTH form and, with `raw` / `rgr`, gsr_shard_backward_preprocess_raw (`shard` and
+// `gr` unused)
+static int shard_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
+                                          int32_t P_total, int32_t index_base, const void* geometry,
+                                          size_t geometry_bytes, const int32_t* radii_total, const void* acc_slice,
+                                          const gsr_grads* gr, const gsr_raw_grads* rgr, bool depth, void* stream) {
+  gsr_cloud c;
+  int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
-  if (P_total <= 0 || index_base < 0 || (int64_t)index_base + shard->P > P_total) { set_error("shard does not fit P_total"); return GSR_ERR_INVALID; }
-  if (shard->P == 0) return GSR_OK;
-  if (!gr || !acc_slice || !radii_total) { set_error("grads / accumulators / radii is null"); return GSR_ERR_INVALID; }
-  if (!gr->dL_dmeans3D || !gr->dL_dmeans2D || !gr->dL_dcolors || !gr->dL_dopacity || !gr->dL_dcov3D ||
-      !gr->dL_dscales || !gr->dL_drotations || (shard->shs && !gr->dL_dsh)) {
-    set_error("a gradient output pointer is null");
-    return GSR_ERR_INVALID;
+  if (P_total <= 0 || index_base < 0 || (int64_t)index_base + c.P > P_total) { set_error("shard does not fit P_total"); return GSR_ERR_INVALID; }
+  if (c.P == 0) return GSR_OK;
+  if ((raw ? !rgr : !gr) || !acc_slice || !radii_total) { set_error("grads / accumulators / radii is null"); return GSR_ERR_INVALID; }
+  if (raw) {
+    if ((rc = check_raw_grads(s, rgr))) return rc;
+  } else {
+    if (!gr->dL_dmeans3D || !gr->dL_dmeans2D || !gr->dL_dcolors || !gr->dL_dopacity || !gr->dL_dcov3D ||
+        !gr->dL_dscales || !gr->dL_drotations || (c.shs && !gr->dL_dsh)) {
+      set_error("a gradient output pointer is null");
+      return GSR_ERR_INVALID;
+    }
+    if (reinterpret_cast<uintptr_t>(gr->dL_drotations) & 15) { set_error("dL_drotations must be 16-byte aligned"); return GSR_ERR_INVALID; }
   }
-  if (reinterpret_cast<uintptr_t>(gr->dL_drotations) & 15) { set_error("dL_drotations must be 16-byte aligned"); return GSR_ERR_INVALID; }
   if (reinterpret_cast<uintptr_t>(acc_slice) & 15) { set_error("acc_slice must be 16-byte aligned"); return GSR_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   GeometryWS g;
   if (!carve_geometry(const_cast<void*>(geometry), P_total, g)) return GSR_ERR_CUDA;
   if (g.total > geometry_bytes) { set_error("geometry workspace too small: %zu < %zu", geometry_bytes, g.total); return GSR_ERR_WORKSPACE; }
   StageScope t(ST_PRE_BWD, st);
-  return launch_preprocess_bwd(*s, *shard, slice_geometry(g, index_base), radii_total + index_base,
-                               (const float*)acc_slice, *gr, st);
+  if (raw) {
+    const RawBackward rb{raw->features_rest, rgr->dL_dfeatures_rest};
+    return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, (const float*)acc_slice,
+                                 raw_grads_as_full(*rgr), st, &rb, nullptr, depth);
+  }
+  return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, (const float*)acc_slice,
+                               *gr, st, nullptr, nullptr, depth);
+}
+
+int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
+                                  const void* geometry, size_t geometry_bytes, const int32_t* radii_total,
+                                  const void* acc_slice, const gsr_grads* gr, void* stream) {
+  return shard_backward_preprocess_impl(s, shard, nullptr, P_total, index_base, geometry, geometry_bytes, radii_total,
+                                        acc_slice, gr, nullptr, false, stream);
+}
+
+int gsr_shard_backward_preprocess_depth(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                        int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                        const int32_t* radii_total, const void* acc_slice, const gsr_grads* gr,
+                                        void* stream) {
+  return shard_backward_preprocess_impl(s, shard, nullptr, P_total, index_base, geometry, geometry_bytes, radii_total,
+                                        acc_slice, gr, nullptr, true, stream);
+}
+
+int gsr_shard_backward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                      int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                      const int32_t* radii_total, const void* acc_slice, const gsr_raw_grads* gr,
+                                      int32_t depth, void* stream) {
+  return shard_backward_preprocess_impl(s, nullptr, shard, P_total, index_base, geometry, geometry_bytes, radii_total,
+                                        acc_slice, nullptr, gr, depth != 0, stream);
 }
 
 int gsr_view_geometry(const void* geometry, int32_t P, gsr_geometry_view* out) {

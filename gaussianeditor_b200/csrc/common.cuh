@@ -156,6 +156,12 @@ void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
 int check_launch(const char* what, bool debug, cudaStream_t st);
 int validate_cloud(const gsr_settings* s, const gsr_cloud* c);  // argument checks of the reference's Python/C++ glue
+// fused activations: the raw cloud checked and seen as a gsr_cloud (opacities = logits, shs = features_dc, ...)
+int raw_to_cloud(const gsr_settings* s, const gsr_raw_cloud* r, gsr_cloud& c);
+int check_raw_grads(const gsr_settings* s, const gsr_raw_grads* gr);  // gr must not be null
+gsr_grads raw_grads_as_full(const gsr_raw_grads& gr);  // the slots the RAW preprocess backward writes through gsr_grads
+// a shard of the sharded entry points: the activated cloud, or the raw one when `raw` is not null (then `shard` is unused)
+int shard_cloud(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw, gsr_cloud& c);
 
 // ---- stage entry points (host side; each file owns its kernels) ------------------------------------------
 // peer_records/npeers: fused all-gather of the sharded path (every rank's view of this shard's record slice), else 0

@@ -120,7 +120,8 @@ __device__ __forceinline__ float sigmoid_act(float x) { return __fdiv_rn(1.0f, _
 
 template <bool BULK_SH, bool P2P = false, bool RAW = false>
 __global__ void __launch_bounds__(PRE_THREADS) preprocess_fwd_kernel(const PreArgs a) {
-  static_assert(!(RAW && (BULK_SH || P2P)), "the RAW variant stages its SH block itself");
+  // RAW + P2P is fine: the features_rest block arrives in s_rest on `bar`, the records leave from s_rec without it
+  static_assert(!(RAW && BULK_SH), "the RAW variant stages its SH block itself");
   __shared__ __align__(16) float sh_rows[BULK_SH ? PRE_THREADS * SH_ROW_WORDS : 4];
   __shared__ __align__(128) float4 s_rec[P2P ? PRE_THREADS * 3 : 1];  // the CTA's records, contiguous like in HBM
   // RAW: the CTA's block of features_rest rows (128 x 12*(M-1) bytes, contiguous and 16-byte aligned in HBM although
@@ -474,7 +475,10 @@ int launch_preprocess_fwd(const gsr_settings& s, const gsr_cloud& c, const Geome
                     (s.sh_coeffs * 12) % 16 == 0 && (reinterpret_cast<uintptr_t>(c.shs) % 16) == 0 &&
                     (s.sh_coeffs * 12) <= 192;
   if (raw) {
-    preprocess_fwd_kernel<false, false, true><<<grid, PRE_THREADS, 0, st>>>(a);
+    if (npeers > 0)
+      preprocess_fwd_kernel<false, true, true><<<grid, PRE_THREADS, 0, st>>>(a);
+    else
+      preprocess_fwd_kernel<false, false, true><<<grid, PRE_THREADS, 0, st>>>(a);
   } else if (npeers > 0) {
     if (bulk)
       preprocess_fwd_kernel<true, true><<<grid, PRE_THREADS, 0, st>>>(a);

@@ -484,15 +484,20 @@ size_t gsr_sparse_candidate_bytes(int32_t world, int32_t seg_cap) {
   return sc.total;
 }
 
-int gsr_sparse_preprocess(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan, void* local_ws,
-                          size_t local_bytes, int32_t* radii_local, void* const* peer_cand, size_t cand_bytes,
-                          int32_t* counts_row, void* stream) {
+// gsr_sparse_preprocess and, with `raw`, gsr_sparse_preprocess_raw (`shard` unused)
+static int sparse_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
+                                  const gsr_sparse_plan* plan, void* local_ws, size_t local_bytes, int32_t* radii_local,
+                                  void* const* peer_cand, size_t cand_bytes, int32_t* counts_row, void* stream) {
   int rc = check_plan(plan);
   if (rc) return rc;
-  if (!s || !shard || shard->P < 0 || shard->P > plan->slice_len) { set_error("sparse_preprocess: shard does not fit slice_len"); return GSR_ERR_INVALID; }
+  const int32_t P = raw ? raw->P : (shard ? shard->P : -1);
+  if (!s || P < 0 || P > plan->slice_len) { set_error("sparse_preprocess: shard does not fit slice_len"); return GSR_ERR_INVALID; }
   if (!local_ws || !radii_local || !peer_cand || !counts_row) { set_error("sparse_preprocess: null buffer"); return GSR_ERR_INVALID; }
+  gsr_cloud c;
+  rc = shard_cloud(s, shard, raw, c);  // (P == 0 passes: nothing of the cloud is read)
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const int n = shard->P;
+  const int n = P;
   GeometryWS g;
   if (!carve_geometry(local_ws, plan->slice_len, g)) return GSR_ERR_CUDA;
   SparseLocal sl;
@@ -510,11 +515,9 @@ int gsr_sparse_preprocess(const gsr_settings* s, const gsr_cloud* shard, const g
   const int W = s->image_width, H = s->image_height;
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (n == 0) return check_cuda(cudaMemsetAsync(counts_row, 0, GSR_MAX_PEERS * sizeof(int32_t), st), "counts memset");
-  rc = validate_cloud(s, shard);
-  if (rc) return rc;
   {
     StageScope t(ST_PRE_FWD, st);
-    rc = launch_preprocess_fwd(*s, *shard, g, radii_local, st);
+    rc = launch_preprocess_fwd(*s, c, g, radii_local, st, nullptr, 0, raw != nullptr, raw ? raw->features_rest : nullptr);
     if (rc) return rc;
     const int nblocks = (n + SP_THREADS - 1) / SP_THREADS;
     sparse_mask_kernel<<<nblocks, SP_THREADS, 0, st>>>(n, g.records, gx, gy, plan->world, sl.dest_mask, sl.blk_base);
@@ -524,6 +527,20 @@ int gsr_sparse_preprocess(const gsr_settings* s, const gsr_cloud* shard, const g
     g_launches += 3;
   }
   return check_launch("sparse_preprocess", s->debug != 0, st);
+}
+
+int gsr_sparse_preprocess(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan, void* local_ws,
+                          size_t local_bytes, int32_t* radii_local, void* const* peer_cand, size_t cand_bytes,
+                          int32_t* counts_row, void* stream) {
+  return sparse_preprocess_impl(s, shard, nullptr, plan, local_ws, local_bytes, radii_local, peer_cand, cand_bytes,
+                                counts_row, stream);
+}
+
+int gsr_sparse_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, const gsr_sparse_plan* plan,
+                              void* local_ws, size_t local_bytes, int32_t* radii_local, void* const* peer_cand,
+                              size_t cand_bytes, int32_t* counts_row, void* stream) {
+  return sparse_preprocess_impl(s, nullptr, shard, plan, local_ws, local_bytes, radii_local, peer_cand, cand_bytes,
+                                counts_row, stream);
 }
 
 int gsr_sparse_order(const gsr_settings* s, const gsr_sparse_plan* plan, void* cand_ws, size_t cand_bytes,
@@ -582,27 +599,37 @@ int gsr_sparse_return(const gsr_sparse_plan* plan, const void* acc_cand, const i
   return check_launch("sparse_return", false, st);
 }
 
-int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
-                                   const void* local_ws, size_t local_bytes, const int32_t* radii_local,
-                                   const void* cand_ws, size_t cand_bytes, void* acc_slice, size_t acc_bytes,
-                                   const gsr_grads* gr, void* stream) {
+// gsr_sparse_backward_preprocess, its DEPTH form and, with `raw` / `rgr`, gsr_sparse_backward_preprocess_raw (`shard`
+// and `gr` unused)
+static int sparse_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
+                                           const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                           const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
+                                           void* acc_slice, size_t acc_bytes, const gsr_grads* gr,
+                                           const gsr_raw_grads* rgr, bool depth, void* stream) {
   int rc = check_plan(plan);
   if (rc) return rc;
-  if (!s || !shard || shard->P < 0 || shard->P > plan->slice_len) { set_error("sparse_backward: shard does not fit slice_len"); return GSR_ERR_INVALID; }
-  if (shard->P == 0) return GSR_OK;
-  rc = validate_cloud(s, shard);
+  const int32_t P = raw ? raw->P : (shard ? shard->P : -1);
+  if (!s || P < 0 || P > plan->slice_len) { set_error("sparse_backward: shard does not fit slice_len"); return GSR_ERR_INVALID; }
+  if (P == 0) return GSR_OK;
+  gsr_cloud c;
+  rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
-  if (!gr || !local_ws || !cand_ws || !radii_local || !acc_slice) { set_error("sparse_backward: null argument"); return GSR_ERR_INVALID; }
-  if (!gr->dL_dmeans3D || !gr->dL_dmeans2D || !gr->dL_dcolors || !gr->dL_dopacity || !gr->dL_dcov3D ||
-      !gr->dL_dscales || !gr->dL_drotations || (shard->shs && !gr->dL_dsh)) {
-    set_error("a gradient output pointer is null");
-    return GSR_ERR_INVALID;
+  if ((raw ? !rgr : !gr) || !local_ws || !cand_ws || !radii_local || !acc_slice) { set_error("sparse_backward: null argument"); return GSR_ERR_INVALID; }
+  if (raw) {
+    if ((rc = check_raw_grads(s, rgr))) return rc;
+    if (reinterpret_cast<uintptr_t>(acc_slice) & 15) { set_error("acc_slice must be 16-byte aligned"); return GSR_ERR_INVALID; }
+  } else {
+    if (!gr->dL_dmeans3D || !gr->dL_dmeans2D || !gr->dL_dcolors || !gr->dL_dopacity || !gr->dL_dcov3D ||
+        !gr->dL_dscales || !gr->dL_drotations || (c.shs && !gr->dL_dsh)) {
+      set_error("a gradient output pointer is null");
+      return GSR_ERR_INVALID;
+    }
+    if ((reinterpret_cast<uintptr_t>(gr->dL_drotations) & 15) || (reinterpret_cast<uintptr_t>(acc_slice) & 15)) {
+      set_error("dL_drotations / acc_slice must be 16-byte aligned");
+      return GSR_ERR_INVALID;
+    }
   }
-  if ((reinterpret_cast<uintptr_t>(gr->dL_drotations) & 15) || (reinterpret_cast<uintptr_t>(acc_slice) & 15)) {
-    set_error("dL_drotations / acc_slice must be 16-byte aligned");
-    return GSR_ERR_INVALID;
-  }
-  const int n = shard->P;
+  const int n = c.P;
   if (acc_bytes < (size_t)n * ACC_STRIDE * sizeof(float)) { set_error("acc_slice too small"); return GSR_ERR_WORKSPACE; }
   GeometryWS g;
   if (!carve_geometry(const_cast<void*>(local_ws), plan->slice_len, g)) return GSR_ERR_CUDA;
@@ -614,12 +641,42 @@ int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard
   if (sc.total > cand_bytes) { set_error("candidate workspace too small: %zu < %zu", cand_bytes, sc.total); return GSR_ERR_WORKSPACE; }
   cudaStream_t st = (cudaStream_t)stream;
   StageScope t(ST_PRE_BWD, st);
+  // the gather adds all 12 floats of each returned row, slot 9 (dL/dz of the depth gradient) included
   sparse_gather_kernel<<<(n + SP_THREADS - 1) / SP_THREADS, SP_THREADS, 0, st>>>(n, plan->world, plan->seg_cap, sl.dest_mask,
                                                                                  sl.blk_base, sc.ret, (float*)acc_slice);
   g_launches++;
   rc = check_launch("sparse_gather", s->debug != 0, st);
   if (rc) return rc;
-  return launch_preprocess_bwd(*s, *shard, g, radii_local, (const float*)acc_slice, *gr, st);
+  if (raw) {
+    const RawBackward rb{raw->features_rest, rgr->dL_dfeatures_rest};
+    return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, raw_grads_as_full(*rgr), st, &rb,
+                                 nullptr, depth);
+  }
+  return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, *gr, st, nullptr, nullptr, depth);
+}
+
+int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
+                                   const void* local_ws, size_t local_bytes, const int32_t* radii_local,
+                                   const void* cand_ws, size_t cand_bytes, void* acc_slice, size_t acc_bytes,
+                                   const gsr_grads* gr, void* stream) {
+  return sparse_backward_preprocess_impl(s, shard, nullptr, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
+                                         acc_slice, acc_bytes, gr, nullptr, false, stream);
+}
+
+int gsr_sparse_backward_preprocess_depth(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
+                                         const void* local_ws, size_t local_bytes, const int32_t* radii_local,
+                                         const void* cand_ws, size_t cand_bytes, void* acc_slice, size_t acc_bytes,
+                                         const gsr_grads* gr, void* stream) {
+  return sparse_backward_preprocess_impl(s, shard, nullptr, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
+                                         acc_slice, acc_bytes, gr, nullptr, true, stream);
+}
+
+int gsr_sparse_backward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, const gsr_sparse_plan* plan,
+                                       const void* local_ws, size_t local_bytes, const int32_t* radii_local,
+                                       const void* cand_ws, size_t cand_bytes, void* acc_slice, size_t acc_bytes,
+                                       const gsr_raw_grads* gr, int32_t depth, void* stream) {
+  return sparse_backward_preprocess_impl(s, nullptr, shard, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
+                                         acc_slice, acc_bytes, nullptr, gr, depth != 0, stream);
 }
 
 int gsr_sparse_apply_weights_gather(const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,

@@ -309,11 +309,13 @@ def exchange_view(buf: ShardBuffers) -> torch.Tensor:
 def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D, sh, colors_precomp, opacities,
                      scales, rotations, cov3Ds_precomp, *, geom: Optional[torch.Tensor] = None,
                      radii: Optional[torch.Tensor] = None, peer: Optional[PeerWorkspace] = None,
-                     ws: Optional[StepWorkspace] = None) -> ShardBuffers:
+                     ws: Optional[StepWorkspace] = None, raw_rest: Optional[torch.Tensor] = None) -> ShardBuffers:
     """Stage 1: project this rank's Gaussians into its slice of the global arrays. `geom` / `radii` may be passed
     in to share one set of global arrays between virtual ranks of a single process. With `peer` (a PeerWorkspace of
     gsr_geometry_bytes(P_pad) bytes) the kernel pushes its records into every rank's workspace itself: no all-gather
-    follows, only a barrier. `ws` (a StepWorkspace) supplies all scratch buffers persistently, its `peer` included."""
+    follows, only a barrier. `ws` (a StepWorkspace) supplies all scratch buffers persistently, its `peer` included.
+    With `raw_rest` (features_rest [n,K,3]) the shard is the scene model's raw parameters (fused activations): `sh` is
+    features_dc [n,1,3], `opacities` / `scales` / `rotations` are the logits, log-scales and raw rotations."""
     lib = _lib.load()
     if ws is not None and ws.peer is not None:
         peer = ws.peer
@@ -324,6 +326,8 @@ def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D
     device = means3D.device
     H, W = int(rs.image_height), int(rs.image_width)
     M = sh.size(1) if sh.numel() != 0 else 0
+    if raw_rest is not None:
+        M = 1 + raw_rest.size(1)
     buf = ShardBuffers()
     buf.plan, buf.M, buf.W, buf.H, buf.ws = plan, M, W, H, ws
     with torch.cuda.device(device):
@@ -332,6 +336,8 @@ def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D
         scales = _f32c(scales, device); rotations = _f32c(rotations, device)
         cov3Ds_precomp = _f32c(cov3Ds_precomp, device)
         buf.inputs = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+        if raw_rest is not None:   # a slice whose rows start off a 16-byte boundary is cloned by _f32c
+            buf.inputs = buf.inputs + (_f32c(raw_rest, device),)
         gbytes = _geometry_bytes(lib, plan.P_pad)
         buf.peer = peer
         if peer is not None:
@@ -343,16 +349,55 @@ def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D
         buf.keep = []
         s = buf.s = _make_settings(rs, M, device, buf.keep)   # one settings struct for all five stage calls
         buf.own = plan.owner()
-        c = _make_cloud(plan.count, means3D, opacities, sh, colors_precomp, scales, rotations, cov3Ds_precomp)
+        c = _shard_cloud(plan.count, buf.inputs)
+        raw = "_raw" if len(buf.inputs) == 8 else ""
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         if peer is not None:
-            _lib.check(lib.gsr_shard_preprocess_p2p(C.byref(s), C.byref(c), plan.P_pad, plan.base, plan.slice_len,
-                                                    peer.ptr_array, plan.world, plan.rank, peer.nbytes,
-                                                    _ptr(buf.radii), st), "gsr_shard_preprocess_p2p")
+            _lib.check(getattr(lib, "gsr_shard_preprocess_p2p" + raw)(
+                C.byref(s), C.byref(c), plan.P_pad, plan.base, plan.slice_len, peer.ptr_array, plan.world, plan.rank,
+                peer.nbytes, _ptr(buf.radii), st), "gsr_shard_preprocess_p2p" + raw)
         else:
-            _lib.check(lib.gsr_shard_preprocess(C.byref(s), C.byref(c), plan.P_pad, plan.base, plan.slice_len,
-                                                _ptr(buf.geom), gbytes, _ptr(buf.radii), st), "gsr_shard_preprocess")
+            _lib.check(getattr(lib, "gsr_shard_preprocess" + raw)(
+                C.byref(s), C.byref(c), plan.P_pad, plan.base, plan.slice_len, _ptr(buf.geom), gbytes,
+                _ptr(buf.radii), st), "gsr_shard_preprocess" + raw)
     return buf
+
+
+def _shard_cloud(n: int, inputs):
+    """The C struct of a shard's inputs: gsr_cloud, or gsr_raw_cloud when `inputs` carries features_rest (8 entries)."""
+    (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp) = inputs[:7]
+    if len(inputs) == 8:
+        return _lib.RawCloud(n, _ptr(means3D), _ptr(opacities), _ptr(sh), _ptr(inputs[7]), _ptr(scales), _ptr(rotations))
+    return _make_cloud(n, means3D, opacities, sh, colors_precomp, scales, rotations, cov3Ds_precomp)
+
+
+def preprocess_grads(lib, n: int, M: int, inputs, device, call):
+    """Gradient buffers of a shard's fused preprocess backward; `call(cloud, grads, raw)` runs the entry point (not for
+    n == 0). Activated inputs: the 8 tensors of the reference's slot order (means3D, means2D, sh, colors, opacity,
+    scales, rotations, cov3D). Raw inputs (features_rest present): means3D, means2D, opacity_logits, features_dc,
+    features_rest, log_scales, raw_rotations."""
+    f32 = dict(dtype=torch.float32, device=device)
+    raw = len(inputs) == 8
+    with torch.cuda.device(device):
+        if raw:
+            d_m3 = torch.empty(n, 3, **f32); d_m2 = torch.empty(n, 3, **f32); d_op = torch.empty(n, 1, **f32)
+            d_dc = torch.empty(n, 1, 3, **f32); d_rest = torch.empty(n, M - 1, 3, **f32)
+            d_sc = torch.empty(n, 3, **f32); d_ro = torch.empty(n, 4, **f32)
+            if n > 0:
+                call(_shard_cloud(n, inputs), _lib.RawGrads(_ptr(d_m3), _ptr(d_m2), _ptr(d_op), _ptr(d_dc),
+                                                            _ptr(d_rest), _ptr(d_sc), _ptr(d_ro)), True)
+            return (d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro)
+        dL_dmeans3D = torch.empty(n, 3, **f32); dL_dmeans2D = torch.empty(n, 3, **f32)
+        dL_dcolors = torch.empty(n, 3, **f32); dL_dopacity = torch.empty(n, 1, **f32)
+        dL_dcov3D = torch.empty(n, 6, **f32); dL_dsh = torch.empty(n, M, 3, **f32)
+        dL_dscales = torch.empty(n, 3, **f32); dL_drotations = torch.empty(n, 4, **f32)
+        if n > 0:
+            call(_shard_cloud(n, inputs), _lib.Grads(_ptr(dL_dmeans3D), _ptr(dL_dmeans2D), _ptr(dL_dcolors),
+                                                     _ptr(dL_dopacity), _ptr(dL_dcov3D), _ptr(dL_dsh),
+                                                     _ptr(dL_dscales), _ptr(dL_drotations)), False)
+            if inputs[4].numel() == 0:
+                dL_dscales.zero_(); dL_drotations.zero_()
+    return (dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D)
 
 
 def shard_order(buf: ShardBuffers) -> int:
@@ -390,14 +435,27 @@ def shard_render(buf: ShardBuffers, color: torch.Tensor, depth: torch.Tensor):
 
 
 def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: torch.Tensor, img: torch.Tensor,
-                          grad_out_color: torch.Tensor, acc: torch.Tensor, deterministic: bool, get):
+                          grad_out_color: torch.Tensor, acc: torch.Tensor, deterministic: bool, get,
+                          grad_depth: Optional[torch.Tensor] = None):
     """gsr_shard_backward_render (or its deterministic form) of the owned tiles of a P-record workspace into
-    acc [P, 12]; `get(name, numel, dtype, grow)` supplies the deterministic scratch."""
+    acc [P, 12]; `get(name, numel, dtype, grow)` supplies the deterministic scratch. With `grad_depth` [1,H,W]
+    (gsr_shard_backward_render_depth) float 9 of each row also gets dL/dz."""
     lib = _lib.load()
     device = geom.device
     with torch.cuda.device(device):
         grad_out_color = _f32c(grad_out_color, device)
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        if grad_depth is not None:
+            grad_depth = _f32c(grad_depth, device)
+            args = (C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), binning.numel(),
+                    _ptr(img), img.numel(), _ptr(grad_out_color), _ptr(grad_depth), _ptr(acc), acc.numel() * 4)
+            det, dbytes = None, 0
+            if deterministic:
+                dbytes = lib.gsr_deterministic_scratch_bytes(P, R, 0)
+                det = get("det", dbytes, torch.uint8, 1.25)
+            _lib.check(lib.gsr_shard_backward_render_depth(*args, _ptr(det), dbytes, st),
+                       "gsr_shard_backward_render_depth")
+            return
         args = (C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), binning.numel(), _ptr(img),
                 img.numel(), _ptr(grad_out_color), _ptr(acc), acc.numel() * 4)
         if deterministic:
@@ -409,41 +467,38 @@ def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: t
             _lib.check(lib.gsr_shard_backward_render(*args, st), "gsr_shard_backward_render")
 
 
-def shard_backward_render(buf: ShardBuffers, grad_out_color: torch.Tensor, deterministic: bool = False) -> torch.Tensor:
+def shard_backward_render(buf: ShardBuffers, grad_out_color: torch.Tensor, deterministic: bool = False,
+                          grad_depth: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Backward stage 1: this rank's tiles -> partial accumulators [P_pad, 12] (zero for untouched Gaussians). With
-    `deterministic` each row is the same bits on every call (no float atomics)."""
+    `deterministic` each row is the same bits on every call (no float atomics). With `grad_depth` [1,H,W] the depth
+    image's gradient enters too (dL/dz in float 9)."""
     device = buf.geom.device
     acc = buf.alloc("acc", buf.plan.P_pad * ACC_STRIDE, torch.float32, device).view(buf.plan.P_pad, ACC_STRIDE)
     owner_backward_render(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.binning, buf.img, grad_out_color, acc,
-                          deterministic, lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow))
+                          deterministic, lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow),
+                          grad_depth)
     return acc
 
 
-def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor):
-    """Backward stage 2 (after the reduce-scatter): gradients of this rank's Gaussians, reference slot order."""
+def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor, depth: bool = False):
+    """Backward stage 2 (after the reduce-scatter): gradients of this rank's Gaussians, reference slot order (or the
+    raw parameters' order of GaussianRasterizer.forward_raw for a raw shard). `depth`: the rows carry dL/dz (the
+    blending backward had a depth gradient)."""
     lib = _lib.load()
     device = buf.geom.device
-    plan, M = buf.plan, buf.M
-    n = plan.count
-    (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp) = buf.inputs
-    with torch.cuda.device(device):
-        f32 = dict(dtype=torch.float32, device=device)
-        dL_dmeans3D = torch.empty(n, 3, **f32); dL_dmeans2D = torch.empty(n, 3, **f32)
-        dL_dcolors = torch.empty(n, 3, **f32); dL_dopacity = torch.empty(n, 1, **f32)
-        dL_dcov3D = torch.empty(n, 6, **f32); dL_dsh = torch.empty(n, M, 3, **f32)
-        dL_dscales = torch.empty(n, 3, **f32); dL_drotations = torch.empty(n, 4, **f32)
-        if n > 0:
-            s = buf.s
-            c = _make_cloud(n, means3D, opacities, sh, colors_precomp, scales, rotations, cov3Ds_precomp)
-            gr = _lib.Grads(_ptr(dL_dmeans3D), _ptr(dL_dmeans2D), _ptr(dL_dcolors), _ptr(dL_dopacity),
-                            _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations))
-            st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-            _lib.check(lib.gsr_shard_backward_preprocess(C.byref(s), C.byref(c), plan.P_pad, plan.base, _ptr(buf.geom),
-                                                         buf.geom.numel(), _ptr(buf.radii), _ptr(acc_slice),
-                                                         C.byref(gr), st), "gsr_shard_backward_preprocess")
-            if scales.numel() == 0:
-                dL_dscales.zero_(); dL_drotations.zero_()
-    return (dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D)
+    plan = buf.plan
+
+    def call(c, gr, raw):
+        st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        args = (C.byref(buf.s), C.byref(c), plan.P_pad, plan.base, _ptr(buf.geom), buf.geom.numel(), _ptr(buf.radii),
+                _ptr(acc_slice), C.byref(gr))
+        if raw:
+            _lib.check(lib.gsr_shard_backward_preprocess_raw(*args, int(depth), st), "gsr_shard_backward_preprocess_raw")
+        elif depth:
+            _lib.check(lib.gsr_shard_backward_preprocess_depth(*args, st), "gsr_shard_backward_preprocess_depth")
+        else:
+            _lib.check(lib.gsr_shard_backward_preprocess(*args, st), "gsr_shard_backward_preprocess")
+    return preprocess_grads(lib, plan.count, buf.M, buf.inputs, device, call)
 
 
 def owner_apply_weights(s, own, P: int, R: int, geom: torch.Tensor, radii: torch.Tensor, image_weights: torch.Tensor,
@@ -548,13 +603,26 @@ def dense_apply_weights(plan: ShardPlan, exchange: "Exchange", pool: "WorkspaceP
 # ---------------------------------------------------------------------------------------------------------
 # autograd + module (one process per GPU)
 # ---------------------------------------------------------------------------------------------------------
+def grads_in_slots(grads, raw: bool):
+    """The step functions' gradient tuple in the input slots of _ShardedRasterize / _SparseShardedRasterize:
+    (means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp) and, last, features_rest. A raw
+    shard has features_dc in the sh slot, the logits / log-scales / raw rotations in theirs and no colour or cov3D."""
+    if raw:
+        d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro = grads
+        return (d_m3, d_m2, d_dc, None, d_op, d_sc, d_ro, None), d_rest
+    return grads, None
+
+
 class _ShardedRasterize(torch.autograd.Function):
+    """Dense exchange. `raw_rest` (features_rest) makes it the fused-activation call (see shard_preprocess);
+    `depth_grad` makes the depth output differentiable, with GaussianRasterizer(depth_grad=True)'s semantics."""
+
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, plan,
-                exchange, pool, deterministic=False):
+                exchange, pool, deterministic=False, depth_grad=False, raw_rest=None):
         ws = pool.take(means3D.device) if pool is not None else None
         buf = shard_preprocess(plan, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                               ws=ws)
+                               ws=ws, raw_rest=raw_rest)
         if ws is not None:
             weakref.finalize(buf, pool.give, ws)     # back to the pool when the last user of this forward is gone
         if buf.peer is not None:
@@ -565,7 +633,11 @@ class _ShardedRasterize(torch.autograd.Function):
         frame = torch.zeros(4, buf.H, buf.W, dtype=torch.float32, device=means3D.device)
         shard_render(buf, frame[:3], frame[3:])
         exchange.all_reduce_sum(frame)
-        ctx.buf, ctx.exchange, ctx.deterministic = buf, exchange, deterministic
+        ctx.buf, ctx.exchange, ctx.deterministic, ctx.depth_grad = buf, exchange, deterministic, bool(depth_grad)
+        if ctx.depth_grad:
+            # outputs without a gradient arrive as None: no depth gradient -> the ordinary backward, and a loss on the
+            # depth alone leaves the colour gradient None (treated as zeros)
+            ctx.set_materialize_grads(False)
         # a fresh tensor, like the single-GPU path and the reference: buf.radii lives in the pooled StepWorkspace and is
         # overwritten by the next forward that takes that workspace
         radii = shard_slice(buf.radii, plan).clone()
@@ -576,12 +648,16 @@ class _ShardedRasterize(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out_color, grad_radii, grad_depth):
         buf, exchange, det = ctx.buf, ctx.exchange, ctx.deterministic
-        acc = shard_backward_render(buf, grad_out_color, det)
+        grad_depth = grad_depth if ctx.depth_grad else None
+        if grad_out_color is None:   # depth_grad: a loss on the depth alone
+            grad_out_color = torch.zeros(3, buf.H, buf.W, dtype=torch.float32, device=buf.geom.device)
+        acc = shard_backward_render(buf, grad_out_color, det, grad_depth)
         acc_slice = buf.alloc("acc_slice", buf.plan.slice_len * ACC_STRIDE, torch.float32,
                               acc.device).view(buf.plan.slice_len, ACC_STRIDE)
         (exchange.reduce_scatter_ordered if det else exchange.reduce_scatter_sum)(acc, acc_slice)
-        grads = shard_backward_preprocess(buf, acc_slice)
-        return (*grads, None, None, None, None, None)
+        grads, d_rest = grads_in_slots(shard_backward_preprocess(buf, acc_slice, grad_depth is not None),
+                                       len(buf.inputs) == 8)
+        return (*grads, None, None, None, None, None, None, d_rest)
 
 
 def p2p_available(exchange: "Exchange") -> bool:
@@ -635,14 +711,19 @@ class ShardedGaussianRasterizer(nn.Module):
     number of ranks, and the dense and sparse modes give the same bits; at one rank they equal
     ``GaussianRasterizer(deterministic=True)``. With more ranks they are not the single-GPU bits (the sums are grouped
     per rank). ``None`` / ``False``: float atomics, and torch's deterministic flag raises (or warns).
+    ``depth_grad``: ``True`` makes the depth output of ``forward`` and ``forward_raw`` differentiable, exactly as
+    ``GaussianRasterizer(depth_grad=True)``: when the depth gets no gradient the ordinary backward runs, and a loss on
+    the depth alone works (the colour gradient is then zeros). It combines with both modes and ``deterministic``.
+    ``forward_raw`` is ``GaussianRasterizer.forward_raw`` (fused activations) on this rank's rows.
     """
 
     def __init__(self, raster_settings: GaussianRasterizationSettings, P_total: int, group=None,
                  p2p: Optional[bool] = None, mode: Optional[str] = None, max_in_flight: int = 3,
-                 deterministic: Optional[bool] = None):
+                 deterministic: Optional[bool] = None, depth_grad: bool = False):
         super().__init__()
         self.raster_settings = raster_settings
         self.deterministic = bool(deterministic)
+        self.depth_grad = bool(depth_grad)
         self.exchange = Exchange(group)
         self.plan = ShardPlan(int(P_total), self.exchange.world, self.exchange.rank)
         can_p2p = p2p_available(self.exchange) if (p2p is None or p2p or mode == "sparse") else False
@@ -688,17 +769,35 @@ class ShardedGaussianRasterizer(nn.Module):
         scales = empty if scales is None else scales
         rotations = empty if rotations is None else rotations
         cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
+        return self._apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, None)
+
+    def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations):
+        """``GaussianRasterizer.forward_raw`` of a sharded cloud (collective): THIS RANK's rows of the scene model's raw
+        parameters (``_xyz, _opacity, _features_dc, _features_rest, _scaling, _rotation``); the activations and the SH
+        concatenation happen inside the preprocess kernels. Returns ``(color, radii_local, depth)`` as ``forward``;
+        gradients land on the raw local leaves (``means2D`` included)."""
+        if not getattr(self, "deterministic", False):
+            _check_deterministic_flag()
+        if means3D.dim() != 2 or means3D.size(1) != 3:
+            raise RuntimeError("means3D must have dimensions (num_points, 3)")
+        empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
+        return self._apply(means3D, means2D, features_dc, empty, opacity_logits, log_scales, raw_rotations, empty,
+                           features_rest)
+
+    def _apply(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest):
         rs = self.raster_settings
+        depth_grad = getattr(self, "depth_grad", False)
         if self.mode == "sparse":
             from . import sparse_sharded as SS
             rk0 = self.sparse_pool.all[0]
             if int(rs.image_width) != rk0.W or int(rs.image_height) != rk0.H:
                 raise RuntimeError("sparse mode: the image size is fixed at construction (peer-mapped frames)")
-            return SS._SparseShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
+            return SS._SparseShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                                     cov3D_precomp, rs, self.sparse_pool, self.exchange,
-                                                    self.deterministic)
-        return _ShardedRasterize.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
-                                       cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic)
+                                                    self.deterministic, depth_grad, raw_rest)
+        return _ShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                       cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic,
+                                       depth_grad, raw_rest)
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):

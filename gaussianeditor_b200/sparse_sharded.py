@@ -31,8 +31,9 @@ import torch
 import torch.nn as nn
 
 from . import _lib
-from .rasterizer import GaussianRasterizationSettings, _f32c, _make_cloud, _make_settings, _ptr, _wait_count
-from .sharded import ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, shard_slice
+from .rasterizer import GaussianRasterizationSettings, _f32c, _make_settings, _ptr, _wait_count
+from .sharded import (ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, _shard_cloud, grads_in_slots, preprocess_grads,
+                      shard_slice)
 
 MAXP = 8  # GSR_MAX_PEERS
 CTRL_BYTES, CTRL_MATRIX_OFFSET, CTRL_ERROR_OFFSET = 512, 64, 32   # GSR_PEER_CTRL_{BYTES,MATRIX_OFFSET,ERROR_OFFSET}
@@ -147,9 +148,10 @@ def _cplan(plan: ShardPlan, cap: int) -> "_lib.SparsePlan":
 
 
 def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D, sh, colors_precomp, opacities, scales,
-                      rotations, cov3Ds_precomp, cap: int) -> SparseStep:
+                      rotations, cov3Ds_precomp, cap: int, raw_rest: Optional[torch.Tensor] = None) -> SparseStep:
     """Owner side: preprocess the shard and push every record to the candidate arrays of the ranks it touches. Writes
-    row `rank` of ``rk.matrix`` (the other rows must be zero before the all-reduce that follows)."""
+    row `rank` of ``rk.matrix`` (the other rows must be zero before the all-reduce that follows). `raw_rest`: a raw
+    shard, as in sharded.shard_preprocess."""
     lib = _lib.load()
     plan, device = rk.plan, rk.device
     if not means3D.is_cuda:
@@ -161,24 +163,29 @@ def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D
     st = SparseStep()
     st.rk, st.cap, st.n = rk, int(cap), plan.count
     st.M = sh.size(1) if sh.numel() != 0 else 0
+    if raw_rest is not None:
+        st.M = 1 + raw_rest.size(1)
     with torch.cuda.device(device):
         means3D = _f32c(means3D, device); opacities = _f32c(opacities, device)
         sh = _f32c(sh, device); colors_precomp = _f32c(colors_precomp, device)
         scales = _f32c(scales, device); rotations = _f32c(rotations, device)
         cov3Ds_precomp = _f32c(cov3Ds_precomp, device)
         st.inputs = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+        if raw_rest is not None:   # a slice whose rows start off a 16-byte boundary is cloned by _f32c
+            st.inputs = st.inputs + (_f32c(raw_rest, device),)
+        raw = "_raw" if raw_rest is not None else ""
         st.keep = []
         st.s = _make_settings(rs, st.M, device, st.keep)
         st.cplan = _cplan(plan, cap)
-        c = _make_cloud(plan.count, *[st.inputs[i] for i in (0, 3, 1, 2, 4, 5, 6)])
+        c = _shard_cloud(plan.count, st.inputs)
         stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         # (the count matrix is never zeroed: every step each rank rewrites its whole row, here and -- through
         # peer_barrier(with_row=True) -- in every peer's copy; a zero-fill could wipe a faster peer's fresh row)
         cand_bytes = lib.gsr_sparse_candidate_bytes(plan.world, cap)
-        _lib.check(lib.gsr_sparse_preprocess(C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local), rk.local_bytes,
-                                             _ptr(rk.radii_local), rk.cand_ptr_array, cand_bytes,
-                                             C.c_void_p(rk.matrix[plan.rank].data_ptr()), stream),
-                   "gsr_sparse_preprocess")
+        _lib.check(getattr(lib, "gsr_sparse_preprocess" + raw)(
+            C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local), rk.local_bytes, _ptr(rk.radii_local),
+            rk.cand_ptr_array, cand_bytes, C.c_void_p(rk.matrix[plan.rank].data_ptr()), stream),
+            "gsr_sparse_preprocess" + raw)
     return st
 
 
@@ -241,9 +248,10 @@ def peer_barrier(rk: SparseRank, with_row: bool = False):
                                         1 if with_row else 0, stream), "gsr_peer_barrier")
 
 
-def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, deterministic: bool = False) -> torch.Tensor:
+def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, deterministic: bool = False,
+                           grad_depth: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Blend backward of the owned tiles into the candidate accumulators [world*cap, 12] (deterministic: no float
-    atomics, every row written)."""
+    atomics, every row written; `grad_depth`: dL/dz in float 9 too)."""
     from .sharded import owner_backward_render
     lib = _lib.load()
     rk = st.rk
@@ -251,7 +259,7 @@ def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, determi
     acc = rk.get("acc", M * ACC_STRIDE, torch.float32, grow=1.25).view(M, ACC_STRIDE)
     gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
     owner_backward_render(st.s, rk.plan.owner(), M, st.R, rk.cand[:gb], st.binning, st.img, grad_out_color, acc,
-                          deterministic, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow))
+                          deterministic, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow), grad_depth)
     return acc
 
 
@@ -265,32 +273,27 @@ def sparse_return(st: SparseStep, acc: torch.Tensor):
                    "gsr_sparse_return")
 
 
-def sparse_backward_preprocess(st: SparseStep):
-    """Owner side: add the returned rows of every Gaussian (ascending rank) and run the fused preprocess backward."""
+def sparse_backward_preprocess(st: SparseStep, depth: bool = False):
+    """Owner side: add the returned rows of every Gaussian (ascending rank) and run the fused preprocess backward
+    (`depth`: the rows carry dL/dz). Gradients in the order of sharded.shard_backward_preprocess."""
     lib = _lib.load()
     rk = st.rk
-    device, n, M = rk.device, st.n, st.M
-    (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp) = st.inputs
-    with torch.cuda.device(device):
-        f32 = dict(dtype=torch.float32, device=device)
-        dL_dmeans3D = torch.empty(n, 3, **f32); dL_dmeans2D = torch.empty(n, 3, **f32)
-        dL_dcolors = torch.empty(n, 3, **f32); dL_dopacity = torch.empty(n, 1, **f32)
-        dL_dcov3D = torch.empty(n, 6, **f32); dL_dsh = torch.empty(n, M, 3, **f32)
-        dL_dscales = torch.empty(n, 3, **f32); dL_drotations = torch.empty(n, 4, **f32)
-        if n > 0:
-            c = _make_cloud(n, means3D, opacities, sh, colors_precomp, scales, rotations, cov3Ds_precomp)
-            gr = _lib.Grads(_ptr(dL_dmeans3D), _ptr(dL_dmeans2D), _ptr(dL_dcolors), _ptr(dL_dopacity),
-                            _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations))
-            acc_slice = rk.get("acc_slice", n * ACC_STRIDE, torch.float32)
-            stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-            gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
-            _lib.check(lib.gsr_sparse_backward_preprocess(C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local),
-                                                          rk.local_bytes, _ptr(rk.radii_local), _ptr(rk.cand), gb,
-                                                          _ptr(acc_slice), acc_slice.numel() * 4, C.byref(gr), stream),
-                       "gsr_sparse_backward_preprocess")
-            if scales.numel() == 0:
-                dL_dscales.zero_(); dL_drotations.zero_()
-    return (dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D)
+    n = st.n
+
+    def call(c, gr, raw):
+        acc_slice = rk.get("acc_slice", n * ACC_STRIDE, torch.float32)
+        stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
+        gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
+        args = (C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local), rk.local_bytes, _ptr(rk.radii_local),
+                _ptr(rk.cand), gb, _ptr(acc_slice), acc_slice.numel() * 4, C.byref(gr))
+        if raw:
+            _lib.check(lib.gsr_sparse_backward_preprocess_raw(*args, int(depth), stream),
+                       "gsr_sparse_backward_preprocess_raw")
+        elif depth:
+            _lib.check(lib.gsr_sparse_backward_preprocess_depth(*args, stream), "gsr_sparse_backward_preprocess_depth")
+        else:
+            _lib.check(lib.gsr_sparse_backward_preprocess(*args, stream), "gsr_sparse_backward_preprocess")
+    return preprocess_grads(lib, n, st.M, st.inputs, rk.device, call)
 
 
 def next_capacity(max_count: int, cap_alloc: int) -> int:
@@ -347,12 +350,12 @@ def _mark(name: str):
 
 
 def _preprocess_and_order(rk: SparseRank, pool: SparsePool, rs, means3D, sh, colors_precomp, opacities, scales, rotations,
-                          cov3Ds_precomp):
+                          cov3Ds_precomp, raw_rest=None):
     """preprocess + push -- barrier with the count row -- order, redone with the exact capacity while a segment
     overflows; then the capacity of the next step. Returns (step, num_rendered of this rank, largest segment)."""
     while True:
         st = sparse_preprocess(rk, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                               pool.cap)
+                               pool.cap, raw_rest)
         _mark("preprocess+push")
         peer_barrier(rk, with_row=True)                # counts + barrier: every push has landed
         rk.queue_barrier_check()                       # sticky error word (this and earlier barriers) -> pinned
@@ -427,15 +430,17 @@ def sparse_apply_weights(pool: SparsePool, rs, means3D, opacities, scales, rotat
 
 
 class _SparseShardedRasterize(torch.autograd.Function):
+    """Sparse exchange; `depth_grad` and `raw_rest` as in sharded._ShardedRasterize."""
+
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange,
-                deterministic=False):
+                deterministic=False, depth_grad=False, raw_rest=None):
         rk = pool.take()
         device = means3D.device
         _mark("start")
         try:
             st, R, max_count = _preprocess_and_order(rk, pool, rs, means3D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp)
+                                                     rotations, cov3Ds_precomp, raw_rest)
         except BaseException:
             pool.give(rk)                                       # a failed forward must not leak its workspace
             raise
@@ -449,7 +454,9 @@ class _SparseShardedRasterize(torch.autograd.Function):
         peer_barrier(rk)
         out = frame.clone()                                 # the peer-visible frame is overwritten by the next step
         _mark("frame broadcast+barrier")
-        ctx.st, ctx.exchange, ctx.deterministic = st, exchange, deterministic
+        ctx.st, ctx.exchange, ctx.deterministic, ctx.depth_grad = st, exchange, deterministic, bool(depth_grad)
+        if ctx.depth_grad:   # None = no gradient for that output (see sharded._ShardedRasterize)
+            ctx.set_materialize_grads(False)
         radii = rk.radii_local[:rk.plan.count].clone()
         ctx.mark_non_differentiable(radii)
         _SparseShardedRasterize.last = dict(R=R, cap=st.cap, max_count=max_count)
@@ -461,12 +468,15 @@ class _SparseShardedRasterize(torch.autograd.Function):
         if st is None:
             raise RuntimeError("the sharded rasterizer's backward can run once (its workspace went back to the pool)")
         _mark("loss")
-        acc = sparse_backward_render(st, grad_out_color, ctx.deterministic)
+        grad_depth = grad_depth if ctx.depth_grad else None
+        if grad_out_color is None:   # depth_grad: a loss on the depth alone
+            grad_out_color = torch.zeros(3, st.rk.H, st.rk.W, dtype=torch.float32, device=st.rk.device)
+        acc = sparse_backward_render(st, grad_out_color, ctx.deterministic, grad_depth)
         _mark("blend backward")
         sparse_return(st, acc)
         peer_barrier(st.rk)
         _mark("return push+barrier")
-        grads = sparse_backward_preprocess(st)
+        grads, d_rest = grads_in_slots(sparse_backward_preprocess(st, grad_depth is not None), len(st.inputs) == 8)
         _mark("gather+preprocess backward")
         ctx.st = None   # the workspace goes back to the pool now, not when the output tensors die
-        return (*grads, None, None, None, None)
+        return (*grads, None, None, None, None, None, d_rest)

@@ -186,7 +186,9 @@ GSR_API int gsr_backward_camera(const gsr_settings* s, const gsr_cloud* c, int32
  * dL_dout_alpha may be NULL (as gsr_backward_alpha), `camera` may be NULL (as gsr_backward_camera). Pass a zero
  * dL_dout_color for a loss on the depth alone. The blending backward always runs render_bwd variant 15 here.
  * gsr_backward_raw_depth is the same for gsr_backward_raw (fused activations, below).
- * Single-GPU only: the Gaussian-sharded entry points take no depth gradient. */
+ * The Gaussian-sharded path has its own depth entry points (gsr_shard_backward_render_depth,
+ * gsr_shard_backward_preprocess_depth / _raw and gsr_sparse_backward_preprocess_depth / _raw, below); they take no
+ * alpha or camera gradient. */
 GSR_API int gsr_backward_depth(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered, const void* geometry,
                        size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                        size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
@@ -268,7 +270,9 @@ GSR_API int gsr_view_image(const void* image, int32_t image_width, int32_t image
  * gsr_forward_render (pass a gsr_cloud with P and any non-null pointers); gsr_backward_raw replaces gsr_backward and
  * returns gradients w.r.t. the raw parameters (chain rule through the activations included). settings.sh_coeffs is
  * M = 1 + K, the coefficients allocated over both arrays. Results agree with the PyTorch-activated path to rounding
- * (not bit-for-bit: torch's normalize reduces in a different order); the default entry points keep exact parity. */
+ * (not bit-for-bit: torch's normalize reduces in a different order); the default entry points keep exact parity.
+ * The Gaussian-sharded path takes raw shards too: gsr_shard_preprocess_raw, gsr_shard_preprocess_p2p_raw,
+ * gsr_sparse_preprocess_raw, gsr_shard_backward_preprocess_raw and gsr_sparse_backward_preprocess_raw (below). */
 typedef struct gsr_raw_cloud {
   int32_t P;
   const float* means3D;        /* [P,3] */
@@ -326,7 +330,12 @@ GSR_API int gsr_backward_raw_deterministic(const gsr_settings* s, const gsr_raw_
  * All P_total-sized arrays (geometry workspace, radii, accumulators) are indexed by GLOBAL Gaussian index, so
  * the gathered state is exactly the single-GPU state and the images are bit-identical to gsr_forward_render's.
  * Every rank must pass the same P_total and slice_len (= ceil(P_total / world)); slots of a slice beyond
- * shard.P are marked culled. */
+ * shard.P are marked culled.
+ * Depth gradient (see gsr_backward_depth): gsr_shard_backward_render_depth also writes dL/dz into float 9 of every
+ * accumulator row, which the reduce-scatter (and the sparse return / gather) carries with the other eleven; then
+ * gsr_shard_backward_preprocess_depth (or gsr_shard_backward_preprocess_raw with depth = 1) takes it into dL/dmeans3D.
+ * Fused activations (see gsr_forward_preprocess_raw): the *_raw entry points take this rank's rows of the raw
+ * parameters (gsr_raw_cloud, features_rest 16-byte aligned) and return gradients w.r.t. them (gsr_raw_grads). */
 typedef struct gsr_tile_owner {
   int32_t row_stride; /* >= 1 */
   int32_t row_phase;  /* 0 .. row_stride-1 */
@@ -352,6 +361,30 @@ GSR_API int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud
                                   int32_t index_base, const void* geometry, size_t geometry_bytes,
                                   const int32_t* radii_total, const void* acc_slice, const gsr_grads* grads,
                                   void* stream);
+/* gsr_shard_preprocess on a raw shard (fused activations). */
+GSR_API int gsr_shard_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                     int32_t index_base, int32_t slice_len, void* geometry, size_t geometry_bytes,
+                                     int32_t* radii_total, void* stream);
+/* gsr_shard_backward_render with the depth image's upstream gradient dL_dout_depth [H*W] (must not be NULL; pass a zero
+ * dL_dout_color for a loss on the depth alone). det_scratch NULL: float atomics, as gsr_shard_backward_render;
+ * otherwise the deterministic form, as gsr_shard_backward_render_deterministic (gsr_deterministic_scratch_bytes(P_total,
+ * num_rendered, 0) bytes). */
+GSR_API int gsr_shard_backward_render_depth(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                            int32_t num_rendered, const void* geometry, size_t geometry_bytes,
+                                            const void* binning, size_t binning_bytes, const void* image,
+                                            size_t image_bytes, const float* dL_dout_color, const float* dL_dout_depth,
+                                            void* acc_total, size_t acc_bytes, void* det_scratch /* may be NULL */,
+                                            size_t det_scratch_bytes, void* stream);
+/* gsr_shard_backward_preprocess with dL/dz (float 9 of the reduced rows) taken into dL/dmeans3D. */
+GSR_API int gsr_shard_backward_preprocess_depth(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                                int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                                const int32_t* radii_total, const void* acc_slice,
+                                                const gsr_grads* grads, void* stream);
+/* gsr_shard_backward_preprocess on a raw shard: gradients w.r.t. the raw parameters; depth != 0 as the DEPTH form. */
+GSR_API int gsr_shard_backward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                              int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                              const int32_t* radii_total, const void* acc_slice,
+                                              const gsr_raw_grads* grads, int32_t depth, void* stream);
 /* Semantic tracing (gsr_apply_weights) of a sharded cloud. After gsr_shard_order (with the same owner and workspaces),
  * bins the owned tile rows and walks them: every hit of splat i (GLOBAL index) adds the pixel's mask value to
  * weights_total[i*weights_stride + ch] (ch < num_channels, float atomics) and num_channels to
@@ -413,6 +446,11 @@ GSR_API int gsr_peer_free(void* ptr);
 GSR_API int gsr_shard_preprocess_p2p(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
                              int32_t slice_len, void* const* peer_geometry /* [world] host array */, int32_t world,
                              int32_t rank, size_t geometry_bytes, int32_t* radii_total, void* stream);
+/* gsr_shard_preprocess_p2p on a raw shard (fused activations). */
+GSR_API int gsr_shard_preprocess_p2p_raw(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                         int32_t index_base, int32_t slice_len,
+                                         void* const* peer_geometry /* [world] host array */, int32_t world,
+                                         int32_t rank, size_t geometry_bytes, int32_t* radii_total, void* stream);
 
 /* ---- sparse exchange for the Gaussian-sharded path -------------------------------------------------------------
  * The dense scheme above moves, sorts and reduces P_total-sized arrays on every rank. Here a splat record travels only
@@ -462,6 +500,24 @@ GSR_API int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_clou
                                    const void* local_ws, size_t local_bytes, const int32_t* radii_local,
                                    const void* cand_ws, size_t cand_bytes, void* acc_slice /* [shard.P,12] scratch */,
                                    size_t acc_bytes, const gsr_grads* grads, void* stream);
+/* Depth gradient and fused activations with the sparse exchange: gsr_sparse_preprocess_raw replaces
+ * gsr_sparse_preprocess for a raw shard; the blending backward is gsr_shard_backward_render_depth on the candidates
+ * (the returned rows carry float 9 like the others); gsr_sparse_backward_preprocess_depth (activated) and
+ * gsr_sparse_backward_preprocess_raw (raw, depth != 0 for the DEPTH form) replace gsr_sparse_backward_preprocess. */
+GSR_API int gsr_sparse_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, const gsr_sparse_plan* plan,
+                                      void* local_ws, size_t local_bytes, int32_t* radii_local,
+                                      void* const* peer_cand /* [world] host */, size_t cand_bytes,
+                                      int32_t* counts_row, void* stream);
+GSR_API int gsr_sparse_backward_preprocess_depth(const gsr_settings* s, const gsr_cloud* shard,
+                                                 const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                                 const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
+                                                 void* acc_slice, size_t acc_bytes, const gsr_grads* grads,
+                                                 void* stream);
+GSR_API int gsr_sparse_backward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard,
+                                               const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                               const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
+                                               void* acc_slice, size_t acc_bytes, const gsr_raw_grads* grads,
+                                               int32_t depth, void* stream);
 /* Semantic tracing with the sparse exchange. The candidate rows carry the hits: weights in floats 0..CH-1 and the
  * count as int32 BITS in float GSR_SPARSE_AW_CNT_SLOT (never converted), and gsr_sparse_return copies rows bit for bit.
  *   gsr_sparse_preprocess -- gsr_peer_barrier(with_matrix_row) -- gsr_sparse_order   (as in the forward, overflow redo

@@ -112,6 +112,59 @@ def check_deterministic(a, cloud, cams, bg, dL, dev, rank, world):
     return ok, hashlib.sha256("".join(digests).encode()).hexdigest(), " deterministic=" + ("ok" if ok else "FAILED")
 
 
+def raw_params(t):
+    """The scene model's raw parameters of a cloud (the inverse activations; rotations left unnormalised)."""
+    o = t["opacities"].clamp(1e-6, 1 - 1e-6)
+    return dict(means3D=t["means3D"], opacity_logits=torch.log(o / (1 - o)), features_dc=t["shs"][:, :1].contiguous(),
+                features_rest=t["shs"][:, 1:].contiguous(), log_scales=torch.log(t["scales"]),
+                raw_rotations=t["rotations"] * 1.7)
+
+
+def check_fused_depth(a, cloud, cam, bg, dL, dev):
+    """--raw (forward_raw on the local rows) and/or --depth-grad (depth_grad=True with a colour + depth loss, then a
+    depth-only loss) against GaussianRasterizer with the same options on the full cloud: frames and radii bit-identical,
+    every gradient (means2D included) within 2e-5 relative L2."""
+    P = cloud.means3D.shape[0]
+    rs = settings_from(cam, bg, cloud.sh_degree, dev)
+    dD = torch.from_numpy(np.random.default_rng(5).random((1, cam.image_height, cam.image_width),
+                                                          dtype=np.float32)).to(dev)
+    t = cloud_tensors(cloud, dev)
+    params = raw_params(t) if a.raw else dict(means3D=t["means3D"], opacities=t["opacities"], shs=t["shs"],
+                                              scales=t["scales"], rotations=t["rotations"])
+    rast = S.ShardedGaussianRasterizer(rs, P, p2p=(True if a.mode == 'sparse' else a.p2p), mode=a.mode,
+                                       depth_grad=a.depth_grad)
+    ref_rast = GaussianRasterizer(rs, depth_grad=a.depth_grad)
+
+    def run(r, tensors, loss):
+        leaves = {k: v.detach().clone().requires_grad_(True) for k, v in tensors.items()}
+        m2 = torch.zeros_like(leaves["means3D"], requires_grad=True)
+        if a.raw:
+            color, radii, depth = r.forward_raw(leaves["means3D"], m2, leaves["opacity_logits"], leaves["features_dc"],
+                                                leaves["features_rest"], leaves["log_scales"], leaves["raw_rotations"])
+        else:
+            color, radii, depth = r(means3D=leaves["means3D"], means2D=m2, opacities=leaves["opacities"],
+                                    shs=leaves["shs"], scales=leaves["scales"], rotations=leaves["rotations"])
+        {"color": (color * dL).sum(), "both": (color * dL).sum() + (depth * dD).sum(),
+         "depth": (depth * dD).sum()}[loss].backward()
+        grads = {k: v.grad for k, v in leaves.items()}
+        grads["means2D"] = m2.grad
+        return color.detach(), radii, depth.detach(), grads
+
+    ok, worst = True, 0.0
+    for loss in (("both", "depth") if a.depth_grad else ("color",)):
+        ref = run(ref_rast, params, loss)
+        mine = run(rast, {k: S.shard_slice(v, rast.plan) for k, v in params.items()}, loss)
+        torch.cuda.synchronize()
+        ok = ok and torch.equal(mine[0], ref[0]) and torch.equal(mine[2], ref[2])
+        ok = ok and torch.equal(mine[1], S.shard_slice(ref[1], rast.plan))
+        for k, g in mine[3].items():
+            worst = max(worst, rel_l2(g.cpu().numpy(), S.shard_slice(ref[3][k], rast.plan).cpu().numpy()))
+    rast.close()
+    ok = ok and worst <= 2e-5
+    return ok, f" raw={a.raw} depth_grad={a.depth_grad} fused_depth_worst_rel_l2={worst:.2e}" + \
+        (" fused_depth=ok" if ok else " fused_depth=FAILED")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="c3")
@@ -123,6 +176,10 @@ def main():
     ap.add_argument("--deterministic", action="store_true",
                     help="also check deterministic=True under torch's deterministic flag (repeatable bits; at world 1 "
                          "the single-GPU deterministic bits); prints DETERMINISTIC_DIGEST")
+    ap.add_argument("--raw", action="store_true",
+                    help="also check forward_raw (fused activations) on the local rows against the single-GPU one")
+    ap.add_argument("--depth-grad", action="store_true",
+                    help="also check depth_grad=True with a colour + depth loss and a depth-only loss")
     ap.add_argument("--no-fill", action="store_true",
                     help="with --deterministic: torch.utils.deterministic.fill_uninitialized_memory = False")
     a = ap.parse_args()
@@ -189,6 +246,10 @@ def main():
     if a.apply_weights:
         aw_ok, aw_msg = check_apply_weights(rast, full, loc, cams, bg, cloud.sh_degree, dev)
         ok = ok and aw_ok
+    if a.raw or a.depth_grad:
+        fd_ok, fd_msg = check_fused_depth(a, cloud, cam, bg, dL, dev)
+        ok = ok and fd_ok
+        aw_msg += fd_msg
     det_digest = None
     if a.deterministic:
         det_ok, det_digest, det_msg = check_deterministic(a, cloud, cams, bg, dL, dev, rank, world)
