@@ -5,8 +5,8 @@
 // (pixel, splat) pair that WOULD be blended adds the pixel's 2-D mask value to the splat:
 //     weights[id*CH + ch] += image_weights[ch, pixel];   cnt[id] += 1      (once per channel, :331-334)
 // No image is written.  The reference issues 2*CH global atomics per hit; here the hits of a warp on the same
-// splat are summed with shuffles first (one atomic pair per warp and splat) and the same opacity-aware tile
-// culling as the render kernels drops splats that cannot reach alpha >= 1/255 inside the tile.
+// splat are summed with shuffles first (one atomic pair per warp and splat). There is no tile culling: every
+// pixel tests every splat of its tile's list with the reference's per-pixel alpha >= 1/255 test.
 // Integer counts are exact; float sums differ from the reference only in summation order.
 #include "common.cuh"
 

@@ -320,6 +320,104 @@ def opacity_edge_cloud(seed: int = 0, stacks: int = 48):
     return Cloud(xyz, scales, _random_quats(rng, P), opac, _sh_dc(rng, P, 1), 1), cam
 
 
+# ---- list-structure scenes ---------------------------------------------------------------------------------------
+# Inputs that shape the per-tile instance lists rather than the splats: one tile holding more instances than a sort tile
+# (4096) and than 2^16, depth keys shared by thousands of Gaussians, and instance counts at the kernels' block sizes.
+# All three put the camera at the origin looking down +z, so the view depth of a Gaussian is its world z exactly.
+
+def _origin_camera(W: int, H: int) -> Camera:
+    return look_at_camera((0, 0, 0), (0, 0, 1), (0, -1, 0), W, H, fovx_deg=60.0)   # view (x, y, z) = world (-x, -y, z)
+
+
+def _at_pixels(cam: Camera, px, py, z):
+    """World centres that project to pixel coordinates (px, py) at view depth z (inverse of ndc2Pix and the
+    projection of _origin_camera)."""
+    W, H = cam.image_width, cam.image_height
+    ndc_x = (2.0 * px + 1.0) / W - 1.0
+    ndc_y = (2.0 * py + 1.0) / H - 1.0
+    return np.stack([-ndc_x * cam.tanfovx * z, -ndc_y * cam.tanfovy * z, z], axis=1)
+
+
+def _tiny_splats(rng, n):
+    """Scales of 1e-5 (sub-pixel at depths 2..6): only the 0.3 px^2 dilation is left, and with the reference's 0.1 floor
+    under the eigenvalue spread the radius is ceil(3 sqrt(0.3 + sqrt(0.1))) = 3 px."""
+    return np.full((n, 3), 1e-5) * rng.uniform(0.8, 1.2, (n, 3))
+
+
+def hotspot_cloud(P: int = 70_000, seed: int = 0, extra: int = 200):
+    """One hot tile at 64x64 -> (Cloud, Camera). ``P`` near-isotropic sub-pixel Gaussians (radius 3 px) with centres
+    uniform inside tile (1, 1) at depths 2..6 and opacities in [1.05/255, 3/255], so no pixel reaches the T < 1e-4 stop
+    and every pixel of the tile walks the whole list: that tile's list holds about P instances (more than a sort tile of
+    4096 and than 2^16 at the default P), and n_contrib reaches P. ``extra`` ordinary Gaussians elsewhere keep the other
+    tiles from being empty. SH degree 0."""
+    rng = np.random.default_rng(seed)
+    cam = _origin_camera(64, 64)
+    px, py = rng.uniform(16.0, 32.0, P), rng.uniform(16.0, 32.0, P)
+    hot = _at_pixels(cam, px, py, rng.uniform(2.0, 6.0, P))
+    other = _at_pixels(cam, rng.uniform(0.0, 64.0, extra), rng.uniform(0.0, 64.0, extra), rng.uniform(2.0, 6.0, extra))
+    xyz = np.concatenate([hot, other]).astype(np.float32)
+    scales = np.concatenate([_tiny_splats(rng, P), np.exp(rng.uniform(np.log(0.01), np.log(0.05), (extra, 3)))])
+    opac = np.concatenate([rng.uniform(1.05 / 255.0, 3.0 / 255.0, P), rng.uniform(0.1, 0.9, extra)])
+    n = P + extra
+    return Cloud(xyz, scales.astype(np.float32), _random_quats(rng, n), opac.astype(np.float32)[:, None],
+                 _sh_dc(rng, n, 0), 0), cam
+
+
+def clone_rows(cloud: Cloud, seed: int = 0, fraction: float = 0.3) -> Cloud:
+    """What GaussianEditor's densify_and_clone does to the list order: a random ``fraction`` of the rows copied 1..3
+    times and the exact copies appended at the end (densification_postfix). A copy shares its original's depth key but
+    sits far from it in index."""
+    rng = np.random.default_rng(seed)
+    P = cloud.means3D.shape[0]
+    picked = rng.permutation(P)[: int(fraction * P)]
+    rows = np.sort(np.repeat(picked, rng.integers(1, 4, picked.size)))
+    cat = lambda a: np.ascontiguousarray(np.concatenate([a, a[rows]]))
+    return Cloud(cat(cloud.means3D), cat(cloud.scales), cat(cloud.rotations), cat(cloud.opacities), cat(cloud.shs),
+                 cloud.sh_degree)
+
+
+def tied_depth_cloud(seed: int = 0, layer: int = 20_000, ordinary: int = 10_000):
+    """A planar layer at 128x128 -> (Cloud, Camera): ``layer`` Gaussians at world z = 4 (one depth key, so equal keys
+    span warps and CTAs of the depth sort) with their indices interleaved with ``ordinary`` Gaussians at depths 2..8, then
+    clone_rows: a third of the rows copied 1..3 times and appended, so copies share keys with rows far away in index.
+    Splats of a few pixels, opacities 0.05..0.5. SH degree 1."""
+    rng = np.random.default_rng(seed)
+    W = H = 128
+    cam = _origin_camera(W, H)
+    P = layer + ordinary
+    z = np.where(np.arange(P) < layer, 4.0, rng.uniform(2.0, 8.0, P))
+    z = z[rng.permutation(P)]
+    xyz = _at_pixels(cam, rng.uniform(-8.0, W + 8.0, P), rng.uniform(-8.0, H + 8.0, P), z).astype(np.float32)
+    xyz[:, 2] = z       # exactly 4.0 for the layer
+    scales = np.exp(rng.uniform(np.log(0.005), np.log(0.03), (P, 3))).astype(np.float32)
+    opac = rng.uniform(0.05, 0.5, (P, 1)).astype(np.float32)
+    base = Cloud(xyz, scales, _random_quats(rng, P), opac, _sh_dc(rng, P, 1), 1)
+    return clone_rows(base, seed=seed + 1), cam
+
+
+ONE_TILE_COUNTS = (1, 2, 31, 32, 33, 127, 128, 129, 511, 512, 513, 4095, 4096, 4097, 8191, 8192, 8193)
+
+
+def one_tile_cloud(P: int, W: int = 1024, H: int = 1024, seed: int = 0):
+    """``P`` Gaussians that touch exactly one tile each -> (Cloud, Camera), so the instance count R equals P: sub-pixel
+    splats (radius 3 px) whose centres lie 4..12 px into their tile. Depths are distinct (a permutation of an evenly
+    spaced grid in 2..6). Half of the Gaussians go to four hot tiles, the rest to tiles drawn at random; at 1024x1024
+    there are 4096 tiles, so both digits of the tile sort are used. SH degree 0. P in ONE_TILE_COUNTS puts R at and
+    next to the multiples of the warp (32), the preprocess block (128), a warp's 512 sort slots and the sort tile
+    (4096)."""
+    rng = np.random.default_rng(seed)
+    cam = _origin_camera(W, H)
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    hot = rng.choice(gx * gy, 4, replace=False)
+    tile = np.where(rng.uniform(size=P) < 0.5, hot[rng.integers(0, 4, P)], rng.integers(0, gx * gy, P))
+    px = 16.0 * (tile % gx) + rng.uniform(4.0, 12.0, P)
+    py = 16.0 * (tile // gx) + rng.uniform(4.0, 12.0, P)
+    z = np.linspace(2.0, 6.0, P, dtype=np.float32)[rng.permutation(P)]
+    xyz = _at_pixels(cam, px, py, z.astype(np.float64)).astype(np.float32)
+    opac = rng.uniform(0.2, 0.9, (P, 1)).astype(np.float32)
+    return Cloud(xyz, _tiny_splats(rng, P).astype(np.float32), _random_quats(rng, P), opac, _sh_dc(rng, P, 0), 0), cam
+
+
 CONFIGS = {
     # name: (P, sh_degree, W, H)
     "c1": dict(P=10_000, sh_degree=0, W=256, H=256),

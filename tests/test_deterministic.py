@@ -91,14 +91,20 @@ def _slots_from_oracle(f, gx, gy):
     return slot, g, tile_of, order, excl
 
 
-@pytest.mark.parametrize("scene", ["c3_small", "frustum_edge", "needle"])
+@pytest.mark.parametrize("scene", ["c3_small", "frustum_edge", "needle", "hotspot", "tied_depth"])
 def test_emission_slots_are_a_bijection_in_emission_order(scene):
+    """hotspot: one tile list of ~70 000 instances; tied_depth: ~27 000 visible Gaussians sharing one depth key (excl
+    follows the index order inside the tie) and exact copies far apart in index."""
     from oracle import cpu_oracle
     if scene == "c3_small":
         cloud, cams = synth.make_config("c3", P=3000)
         cam = cams[0]
     elif scene == "frustum_edge":
         cloud, cam = synth.frustum_edge_cloud()
+    elif scene == "hotspot":
+        cloud, cam = synth.hotspot_cloud()
+    elif scene == "tied_depth":
+        cloud, cam = synth.tied_depth_cloud()
     else:
         cloud, cam = synth.needle_cloud(P=300)
     f = cpu_oracle.forward_from(cloud, cam)
@@ -123,9 +129,8 @@ def test_emission_slots_are_a_bijection_in_emission_order(scene):
         assert np.all(np.diff(tile_by_slot)[same] > 0)
         # relative position of every instance inside its Gaussian's run equals the reference's emission position
         ref_pos = np.zeros(R, np.int64)
-        for gi in np.unique(g):
-            m = np.nonzero(g == gi)[0]
-            ref_pos[m[np.argsort(tile[m], kind="stable")]] = np.arange(len(m))
+        by_g = np.lexsort((tile, g))      # per Gaussian, its instances by tile
+        ref_pos[by_g] = np.arange(R) - np.searchsorted(g[by_g], g[by_g], side="left")
         assert np.array_equal(slot - excl[g], ref_pos)
         assert np.all(off_excl[g] + ref_pos < f.point_offsets[g])
         if scene == "frustum_edge":   # clamped rectangles are part of this scene

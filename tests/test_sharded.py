@@ -215,9 +215,14 @@ def _case():
 def test_virtual_ranks_tile_the_single_gpu_result(world):
     """Drive the sharded C-ABI for `world` virtual ranks on one GPU (the all-gather is a shared buffer, the
     all-reduce / reduce-scatter are explicit sums) and compare with the single-GPU rasterizer."""
+    virtual_dense(_case(), world)
+
+
+def virtual_dense(case, world):
+    """The dense sharded path on `world` virtual ranks against `case` (cloud, cam, bg, dL and the single-GPU result
+    `ref` of util.run_ours): frames, depth and radii bit-identical, instance total equal, gradients to 2e-5."""
     from util import cloud_tensors, settings_from, rel_l2
     dev = torch.device("cuda")
-    case = _case()
     cloud, cam, bg, dL, ref = case["cloud"], case["cam"], case["bg"], case["dL"], case["ref"]
     H, W = cam.image_height, cam.image_width
     rs = settings_from(cam, bg, cloud.sh_degree, dev)
@@ -276,10 +281,15 @@ def test_sparse_exchange_virtual_ranks_match_single_gpu(world, cap_mode):
     whose tile rows they touch, yet frames, depth, radii and the instance total must equal the single-GPU result bit for
     bit and the gathered gradients must match to summation order. `tight` uses the smallest legal segment capacity
     (exactly the largest segment), `overflow` starts too small and must be detected through the count matrix."""
+    virtual_sparse(_case(), world, cap_mode)
+
+
+def virtual_sparse(case, world, cap_mode):
+    """The sparse sharded path on `world` virtual ranks against `case` (as for virtual_dense), with the segment
+    capacity of `cap_mode`."""
     from gaussianeditor_b200 import sparse_sharded as SS
     from util import cloud_tensors, settings_from, rel_l2
     dev = torch.device("cuda")
-    case = _case()
     cloud, cam, bg, dL, ref = case["cloud"], case["cam"], case["bg"], case["dL"], case["ref"]
     H, W = cam.image_height, cam.image_width
     rs = settings_from(cam, bg, cloud.sh_degree, dev)

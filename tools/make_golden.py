@@ -3,7 +3,7 @@
 Needs a GPU and the built oracle/_ref:   python tools/make_golden.py OUT_DIR   (writes OUT_DIR/*.npz; copy them to
 tests/golden/ and commit).  The reference has no tests or fixtures of its own (SURVEY.md section 4); these files
 are what pins the CPU oracle and our kernels to the reference's actual outputs when no GPU reference is at hand:
-  * <case>.npz                    inputs and full reference outputs of three tiny scenes (tests/test_golden.py);
+  * <case>.npz                    inputs and full reference outputs of four tiny scenes (tests/test_golden.py);
   * small_cases_reference.npz     (goes to tests/golden/parity/) for test_parity_gpu's small cases: SHA-256 digests of every forward output and a
                                   seeded sample of every gradient with its noise floor and max |value|;
   * reference_outputs.npz         (goes to tests/golden/parity/) every other reference value test_parity_gpu compares
@@ -23,9 +23,9 @@ import torch
 from gaussianeditor_b200 import synth
 import test_parity_gpu as T
 
-OUT = sys.argv[1]
-os.makedirs(OUT, exist_ok=True)
-assert T.ref_cuda.available(), "oracle/_ref/libdgr_ref.so is not built"
+import test_list_edges as LE
+
+OUT = None
 
 
 def case(name, cloud, cam, bg, colors_precomp=None, scale_modifier=1.0, seed=0):
@@ -54,48 +54,74 @@ def case(name, cloud, cam, bg, colors_precomp=None, scale_modifier=1.0, seed=0):
     print(name, "R", ref["R"], "visible", int((ref["radii"] > 0).sum()), "noise", max(noise.values()))
 
 
-c3, _ = synth.make_config("c3", P=400)
-case("c3_p400_deg3", c3, synth.ring_cameras(8, 4.5, 15.0, 72, 56, 61.0)[2], (0.1, 0.3, 0.6), seed=1)
-c1, _ = synth.make_config("c1", P=300)
-case("c1_p300_deg0", c1, synth.look_at_camera((0, 0, -3.5), (0, 0, 0), (0, -1, 0), 64, 48, fovy_deg=50.0), (0, 0, 0), seed=2)
-c2, _ = synth.make_config("c2", P=300)
-cp = np.random.default_rng(5).uniform(size=(300, 3)).astype(np.float32)
-case("c2_p300_colors_mod07", c2, synth.look_at_camera((0, 0, -3.5), (0, 0, 0), (0, -1, 0), 50, 35, fovy_deg=50.0),
-     (1, 1, 1), colors_precomp=cp, scale_modifier=0.7, seed=3)
-small = {}
-for name, cloud, cam, bg in T._small_cases():
-    dL = T._small_case_dL(cam)
-    ref = T._ref_run(cloud, cam, bg, dL=dL)
-    ref2 = T._ref_run(cloud, cam, bg, dL=dL)
-    for k, x in T._ref_forward_fields(ref).items():
-        small[f"{name}/fwd/{k}"] = np.array(T._digest(x))
-    for _, b in T.GRAD_PAIRS:
-        r = ref["grads"][b].cpu().numpy().ravel()
-        small[f"{name}/bwd/{b}"] = r[T._sample_index(r.size)]
-        small[f"{name}/bwd/{b}/noise"] = np.float64(T.rel_l2(ref2["grads"][b].cpu().numpy().ravel(), r))
-        small[f"{name}/bwd/{b}/absmax"] = np.float64(np.abs(r).max())
-np.savez_compressed(os.path.join(OUT, "small_cases_reference.npz"), **small)
-
-
 def parametrizations(fn):
-    marks = [m for m in getattr(fn, "pytestmark", []) if m.name == "parametrize"]
-    if not marks:
-        return [()]
-    return [v if isinstance(v, tuple) else (v,) for v in marks[0].args[1]]
+    """Keyword arguments of every parameter set of a test (the product of its parametrize marks)."""
+    combos = [{}]
+    for m in [m for m in getattr(fn, "pytestmark", []) if m.name == "parametrize"]:
+        names = [n.strip() for n in m.args[0].split(",")]
+        combos = [dict(c, **dict(zip(names, v if isinstance(v, tuple) else (v,)))) for c in combos for v in m.args[1]]
+    return combos
 
 
-T.RECORD = {}
-for fn in (T.test_precomputed_colors_and_scale_modifier, T.test_mark_visible_and_apply_weights_match_reference,
-           T.test_apply_weights_channels_and_float_masks,
-           T.test_alpha_output_matches_reference_accum_alpha_and_is_differentiable,
-           T.test_binning_variants_match_reference_lists, T.test_edit_loop_matches_the_reference_rasterizer_step_by_step,
-           T.test_sh_degrees_and_coefficient_counts, T.test_precomputed_covariance_path,
-           T.test_hd_frame_partial_tile_row_and_debug_flag, T.test_full_size_configs_match_reference_cuda,
-           T.test_needle_forward_bit_exact_every_variant, T.test_needle_backward_blend_weights_every_variant,
-           T.test_frustum_edge_forward_and_preprocess_backward, T.test_opacity_edge_forward_and_backward,
-           T.test_frame_size_edges):
-    for args in parametrizations(fn):
-        fn(*args)
-        print("recorded", fn.__name__, args)
-np.savez_compressed(os.path.join(OUT, "reference_outputs.npz"), **T.RECORD)
-print("golden written to", OUT)
+def main():
+    global OUT
+    OUT = sys.argv[1]
+    os.makedirs(OUT, exist_ok=True)
+    assert T.ref_cuda.available(), "oracle/_ref/libdgr_ref.so is not built"
+    c3, _ = synth.make_config("c3", P=400)
+    case("c3_p400_deg3", c3, synth.ring_cameras(8, 4.5, 15.0, 72, 56, 61.0)[2], (0.1, 0.3, 0.6), seed=1)
+    c1, _ = synth.make_config("c1", P=300)
+    case("c1_p300_deg0", c1, synth.look_at_camera((0, 0, -3.5), (0, 0, 0), (0, -1, 0), 64, 48, fovy_deg=50.0), (0, 0, 0), seed=2)
+    c2, _ = synth.make_config("c2", P=300)
+    cp = np.random.default_rng(5).uniform(size=(300, 3)).astype(np.float32)
+    case("c2_p300_colors_mod07", c2, synth.look_at_camera((0, 0, -3.5), (0, 0, 0), (0, -1, 0), 50, 35, fovy_deg=50.0),
+         (1, 1, 1), colors_precomp=cp, scale_modifier=0.7, seed=3)
+    hotspot_case()
+    small = {}
+    for name, cloud, cam, bg in T._small_cases():
+        dL = T._small_case_dL(cam)
+        ref = T._ref_run(cloud, cam, bg, dL=dL)
+        ref2 = T._ref_run(cloud, cam, bg, dL=dL)
+        for k, x in T._ref_forward_fields(ref).items():
+            small[f"{name}/fwd/{k}"] = np.array(T._digest(x))
+        for _, b in T.GRAD_PAIRS:
+            r = ref["grads"][b].cpu().numpy().ravel()
+            small[f"{name}/bwd/{b}"] = r[T._sample_index(r.size)]
+            small[f"{name}/bwd/{b}/noise"] = np.float64(T.rel_l2(ref2["grads"][b].cpu().numpy().ravel(), r))
+            small[f"{name}/bwd/{b}/absmax"] = np.float64(np.abs(r).max())
+    np.savez_compressed(os.path.join(OUT, "small_cases_reference.npz"), **small)
+    np.savez_compressed(os.path.join(OUT, "reference_outputs.npz"), **record(RECORDED))
+    print("golden written to", OUT)
+
+
+def hotspot_case():
+    """A hot tile of 1500 sub-pixel splats plus densify_and_clone copies (tests/golden/hotspot_p1500_clones.npz)."""
+    cloud, cam = synth.hotspot_cloud(P=1500, extra=50)
+    case("hotspot_p1500_clones", synth.clone_rows(cloud), cam, (0.1, 0.2, 0.3), seed=4)
+
+
+# the tests that use test_parity_gpu._Ref: run against the live reference (their assertions included), and what they
+# computed from it is recorded
+RECORDED = (T.test_precomputed_colors_and_scale_modifier, T.test_mark_visible_and_apply_weights_match_reference,
+            T.test_apply_weights_channels_and_float_masks,
+            T.test_alpha_output_matches_reference_accum_alpha_and_is_differentiable,
+            T.test_binning_variants_match_reference_lists, T.test_edit_loop_matches_the_reference_rasterizer_step_by_step,
+            T.test_sh_degrees_and_coefficient_counts, T.test_precomputed_covariance_path,
+            T.test_hd_frame_partial_tile_row_and_debug_flag, T.test_full_size_configs_match_reference_cuda,
+            T.test_needle_forward_bit_exact_every_variant, T.test_needle_backward_blend_weights_every_variant,
+            T.test_frustum_edge_forward_and_preprocess_backward, T.test_opacity_edge_forward_and_backward,
+            T.test_frame_size_edges, LE.test_forward_bit_exact_binning_and_depth_sort_variants,
+            LE.test_backward_against_reference_and_fp64, LE.test_apply_weights_matches_reference)
+
+
+def record(tests):
+    T.RECORD = {}
+    for fn in tests:
+        for kw in parametrizations(fn):
+            fn(**kw)
+            print("recorded", fn.__name__, kw)
+    return T.RECORD
+
+
+if __name__ == "__main__":
+    main()
