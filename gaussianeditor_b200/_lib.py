@@ -36,6 +36,8 @@ SYMBOLS = [
     "gsr_shard_preprocess_raw", "gsr_shard_preprocess_p2p_raw", "gsr_sparse_preprocess_raw",
     "gsr_shard_backward_render_depth", "gsr_shard_backward_preprocess_depth", "gsr_sparse_backward_preprocess_depth",
     "gsr_shard_backward_preprocess_raw", "gsr_sparse_backward_preprocess_raw",
+    "gsr_shard_alpha_image", "gsr_shard_backward_render_alpha", "gsr_shard_backward_preprocess_camera",
+    "gsr_sparse_backward_preprocess_camera", "gsr_frame_broadcast_planes", "gsr_peer_row_put",
 ]
 
 
@@ -257,6 +259,21 @@ def load():
     lib.gsr_peer_barrier.argtypes = [i32, i32, C.POINTER(vp), C.c_uint32, i32, vp]
     lib.gsr_frame_broadcast.restype = C.c_int
     lib.gsr_frame_broadcast.argtypes = [TO, i32, i32, vp, C.POINTER(vp), vp]
+    CG = C.POINTER(CameraGrads)
+    lib.gsr_shard_alpha_image.restype = C.c_int
+    lib.gsr_shard_alpha_image.argtypes = [TO, vp, sz, i32, i32, vp, vp]
+    lib.gsr_shard_backward_render_alpha.restype = C.c_int
+    lib.gsr_shard_backward_render_alpha.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, sz, vp, sz,
+                                                    vp]
+    lib.gsr_shard_backward_preprocess_camera.restype = C.c_int
+    lib.gsr_shard_backward_preprocess_camera.argtypes = [S, Cl, i32, i32, vp, sz, vp, vp, C.POINTER(Grads), i32, CG, vp]
+    lib.gsr_sparse_backward_preprocess_camera.restype = C.c_int
+    lib.gsr_sparse_backward_preprocess_camera.argtypes = [S, Cl, SP, vp, sz, vp, vp, sz, vp, sz, C.POINTER(Grads), i32,
+                                                          CG, vp]
+    lib.gsr_frame_broadcast_planes.restype = C.c_int
+    lib.gsr_frame_broadcast_planes.argtypes = [TO, i32, i32, i32, vp, C.POINTER(vp), vp]
+    lib.gsr_peer_row_put.restype = C.c_int
+    lib.gsr_peer_row_put.argtypes = [i32, i32, vp, i32, C.POINTER(vp), vp]
     if lib.gsr_abi_version() != 2:
         raise RuntimeError("libgsr_b200.so ABI version mismatch")
     _lib = lib

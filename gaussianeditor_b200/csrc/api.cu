@@ -122,6 +122,26 @@ int shard_cloud(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_clo
   return rc;
 }
 
+int check_shard_camera(const gsr_camera_grads* cam, int P) {
+  if (!cam || !cam->dL_dviewmatrix || !cam->dL_dprojmatrix || !cam->dL_dcampos) {
+    set_error("camera gradients: null struct or output");
+    return GSR_ERR_INVALID;
+  }
+  const size_t need = camera_scratch_bytes(P > 0 ? P : 1);
+  if (!cam->scratch || cam->scratch_bytes < need) {
+    set_error("camera scratch too small: %zu < %zu (gsr_camera_scratch_bytes(shard.P))", cam->scratch_bytes, need);
+    return GSR_ERR_WORKSPACE;
+  }
+  return GSR_OK;
+}
+
+int zero_shard_camera(const gsr_camera_grads* cam, cudaStream_t st) {
+  cudaError_t e = cudaMemsetAsync(cam->dL_dviewmatrix, 0, 16 * sizeof(float), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(cam->dL_dprojmatrix, 0, 16 * sizeof(float), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(cam->dL_dcampos, 0, 3 * sizeof(float), st);
+  return e == cudaSuccess ? GSR_OK : check_cuda(e, "camera gradient memset");
+}
+
 }  // namespace gsr
 
 using namespace gsr;
@@ -718,7 +738,8 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
                                       const void* geometry, size_t geometry_bytes, const void* binning,
                                       size_t binning_bytes, const void* image, size_t image_bytes,
                                       const float* dL_dout_color, void* acc_total, size_t acc_bytes, void* stream,
-                                      const DetScratch* ds, const float* dL_dout_depth = nullptr) {
+                                      const DetScratch* ds, const float* dL_dout_depth = nullptr,
+                                      const float* dL_dout_alpha = nullptr) {
   int rc = check_settings(s);
   if (rc) return rc;
   TileOwner own;
@@ -742,8 +763,33 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
     if (e != cudaSuccess) return check_cuda(e, "accumulator memset");
   }
   if (R == 0) return GSR_OK;
-  return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own, nullptr, dL_dout_depth,
+  return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own, dL_dout_alpha, dL_dout_depth,
                            ds ? &det : nullptr, P_total, R);
+}
+
+int gsr_shard_backward_render_alpha(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                                    const void* geometry, size_t geometry_bytes, const void* binning,
+                                    size_t binning_bytes, const void* image, size_t image_bytes,
+                                    const float* dL_dout_color, const float* dL_dout_alpha, const float* dL_dout_depth,
+                                    void* acc_total, size_t acc_bytes, void* det_scratch, size_t det_scratch_bytes,
+                                    void* stream) {
+  if (!dL_dout_alpha) { set_error("dL_dout_alpha is null"); return GSR_ERR_INVALID; }
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  return shard_backward_render_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                    image_bytes, dL_dout_color, acc_total, acc_bytes, stream,
+                                    det_scratch ? &ds : nullptr, dL_dout_depth, dL_dout_alpha);
+}
+
+int gsr_shard_alpha_image(const gsr_tile_owner* owner, const void* image, size_t image_bytes, int32_t W, int32_t H,
+                          float* out_alpha, void* stream) {
+  TileOwner own;
+  int rc = check_owner(owner, own);
+  if (rc) return rc;
+  if (W < 0 || H < 0 || !out_alpha || !image) { set_error("shard_alpha_image: bad arguments"); return GSR_ERR_INVALID; }
+  ImageWS im;
+  carve_image(const_cast<void*>(image), W, H, im);
+  if (im.total > image_bytes) { set_error("image workspace too small: %zu < %zu", image_bytes, im.total); return GSR_ERR_WORKSPACE; }
+  return launch_alpha_image_owner(im.final_T, W, H, own, out_alpha, (cudaStream_t)stream);
 }
 
 int gsr_shard_backward_render_depth(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
@@ -844,12 +890,14 @@ int gsr_shard_apply_weights_deterministic(const gsr_settings* s, const gsr_tile_
 static int shard_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
                                           int32_t P_total, int32_t index_base, const void* geometry,
                                           size_t geometry_bytes, const int32_t* radii_total, const void* acc_slice,
-                                          const gsr_grads* gr, const gsr_raw_grads* rgr, bool depth, void* stream) {
+                                          const gsr_grads* gr, const gsr_raw_grads* rgr, bool depth, void* stream,
+                                          const gsr_camera_grads* cam = nullptr) {
   gsr_cloud c;
   int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
   if (P_total <= 0 || index_base < 0 || (int64_t)index_base + c.P > P_total) { set_error("shard does not fit P_total"); return GSR_ERR_INVALID; }
-  if (c.P == 0) return GSR_OK;
+  if (cam && (rc = check_shard_camera(cam, c.P))) return rc;
+  if (c.P == 0) return cam ? zero_shard_camera(cam, (cudaStream_t)stream) : GSR_OK;
   if ((raw ? !rgr : !gr) || !acc_slice || !radii_total) { set_error("grads / accumulators / radii is null"); return GSR_ERR_INVALID; }
   if (raw) {
     if ((rc = check_raw_grads(s, rgr))) return rc;
@@ -872,8 +920,22 @@ static int shard_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud
     return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, (const float*)acc_slice,
                                  raw_grads_as_full(*rgr), st, &rb, nullptr, depth);
   }
+  if (cam) {
+    const CameraBackward cb{cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos, (float*)cam->scratch};
+    return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base,
+                                 (const float*)acc_slice, *gr, st, nullptr, &cb, depth);
+  }
   return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, (const float*)acc_slice,
                                *gr, st, nullptr, nullptr, depth);
+}
+
+int gsr_shard_backward_preprocess_camera(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                         int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                         const int32_t* radii_total, const void* acc_slice, const gsr_grads* gr,
+                                         int32_t depth, const gsr_camera_grads* camera, void* stream) {
+  if (!camera) { set_error("camera gradients: null struct"); return GSR_ERR_INVALID; }
+  return shard_backward_preprocess_impl(s, shard, nullptr, P_total, index_base, geometry, geometry_bytes, radii_total,
+                                        acc_slice, gr, nullptr, depth != 0, stream, camera);
 }
 
 int gsr_shard_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,

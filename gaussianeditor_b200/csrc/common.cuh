@@ -162,6 +162,10 @@ int check_raw_grads(const gsr_settings* s, const gsr_raw_grads* gr);  // gr must
 gsr_grads raw_grads_as_full(const gsr_raw_grads& gr);  // the slots the RAW preprocess backward writes through gsr_grads
 // a shard of the sharded entry points: the activated cloud, or the raw one when `raw` is not null (then `shard` is unused)
 int shard_cloud(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw, gsr_cloud& c);
+// the camera arrays of a sharded preprocess backward of a P-Gaussian shard: outputs and scratch checked (no device work)
+int check_shard_camera(const gsr_camera_grads* cam, int P);
+// writes this rank's zero partial (a shard without Gaussians: no preprocess backward runs)
+int zero_shard_camera(const gsr_camera_grads* cam, cudaStream_t st);
 
 // ---- stage entry points (host side; each file owns its kernels) ------------------------------------------
 // peer_records/npeers: fused all-gather of the sharded path (every rank's view of this shard's record slice), else 0
@@ -217,6 +221,9 @@ int launch_preprocess_bwd(const gsr_settings& s, const gsr_cloud& c, const Geome
                           const CameraBackward* cam = nullptr, bool depth = false);
 // out_alpha[i] = 1 - final_T[i]  (the reference keeps final_T as ImageState::accum_alpha, rasterizer_impl.h:50)
 int launch_alpha_image(const float* final_T, size_t n, float* out_alpha, cudaStream_t st);
+// the same on the tile rows `own` owns only (the sharded forward writes final_T there and nowhere else)
+int launch_alpha_image_owner(const float* final_T, int W, int H, const TileOwner& own, float* out_alpha,
+                             cudaStream_t st);
 int launch_mark_visible(int P, const float* means3D, const float* viewmatrix, uint8_t* present, cudaStream_t st);
 int launch_apply_weights(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                          const float* image_weights, int CH, float* weights, int32_t* cnt, cudaStream_t st,

@@ -413,6 +413,22 @@ __global__ void frame_broadcast_kernel(const FrameArgs a) {
   }
 }
 
+// ---- small row all-gather: this rank's row -> slot [me] of every rank's slots (a barrier must follow) ----------------
+struct RowPutArgs {
+  const float* row;
+  int n, me, world;
+  float* peer_slots[GSR_MAX_PEERS];  // rank r's [GSR_MAX_PEERS][GSR_PEER_ROW_FLOATS] slots as mapped here
+};
+__global__ void peer_row_put_kernel(const RowPutArgs a) {
+  // threadIdx.x = float of the row (plain copy: the bits travel unchanged); the unrolled loop over the destinations
+  // indexes the parameter array with constants, so it is not copied to local memory
+  if ((int)threadIdx.x >= a.n) return;
+  const float v = a.row[threadIdx.x];
+#pragma unroll
+  for (int r = 0; r < GSR_MAX_PEERS; r++)
+    if (r < a.world) a.peer_slots[r][a.me * GSR_PEER_ROW_FLOATS + threadIdx.x] = v;
+}
+
 // ---- cross-rank barrier over peer memory ---------------------------------------------------------------------------
 // 512 bytes at the start of every rank's peer-visible block. flags[r] is written by rank r only (the number of the last
 // barrier it has reached); matrix row s is written by rank s only (n[s -> d], the segment sizes of the sparse exchange).
@@ -605,12 +621,14 @@ static int sparse_backward_preprocess_impl(const gsr_settings* s, const gsr_clou
                                            const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
                                            const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
                                            void* acc_slice, size_t acc_bytes, const gsr_grads* gr,
-                                           const gsr_raw_grads* rgr, bool depth, void* stream) {
+                                           const gsr_raw_grads* rgr, bool depth, void* stream,
+                                           const gsr_camera_grads* cam = nullptr) {
   int rc = check_plan(plan);
   if (rc) return rc;
   const int32_t P = raw ? raw->P : (shard ? shard->P : -1);
   if (!s || P < 0 || P > plan->slice_len) { set_error("sparse_backward: shard does not fit slice_len"); return GSR_ERR_INVALID; }
-  if (P == 0) return GSR_OK;
+  if (cam && (rc = check_shard_camera(cam, P))) return rc;
+  if (P == 0) return cam ? zero_shard_camera(cam, (cudaStream_t)stream) : GSR_OK;
   gsr_cloud c;
   rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
@@ -652,7 +670,21 @@ static int sparse_backward_preprocess_impl(const gsr_settings* s, const gsr_clou
     return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, raw_grads_as_full(*rgr), st, &rb,
                                  nullptr, depth);
   }
+  if (cam) {
+    const CameraBackward cb{cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos, (float*)cam->scratch};
+    return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, *gr, st, nullptr, &cb, depth);
+  }
   return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, *gr, st, nullptr, nullptr, depth);
+}
+
+int gsr_sparse_backward_preprocess_camera(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
+                                          const void* local_ws, size_t local_bytes, const int32_t* radii_local,
+                                          const void* cand_ws, size_t cand_bytes, void* acc_slice, size_t acc_bytes,
+                                          const gsr_grads* gr, int32_t depth, const gsr_camera_grads* camera,
+                                          void* stream) {
+  if (!camera) { set_error("camera gradients: null struct"); return GSR_ERR_INVALID; }
+  return sparse_backward_preprocess_impl(s, shard, nullptr, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
+                                         acc_slice, acc_bytes, gr, nullptr, depth != 0, stream, camera);
 }
 
 int gsr_sparse_backward_preprocess(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
@@ -728,11 +760,15 @@ int gsr_peer_barrier(int32_t world, int32_t rank, void* const* peer_ctrl, uint32
   return check_launch("peer_barrier", false, (cudaStream_t)stream);
 }
 
-int gsr_frame_broadcast(const gsr_tile_owner* owner, int32_t W, int32_t H, const float* frame, void* const* peer_frames,
-                        void* stream) {
+int gsr_frame_broadcast_planes(const gsr_tile_owner* owner, int32_t W, int32_t H, int32_t planes, const float* frame,
+                               void* const* peer_frames, void* stream) {
   if (!owner || owner->row_stride < 1 || owner->row_stride > GSR_MAX_PEERS || owner->row_phase < 0 ||
       owner->row_phase >= owner->row_stride || !frame || !peer_frames || W < 0 || H < 0) {
     set_error("frame_broadcast: bad arguments");
+    return GSR_ERR_INVALID;
+  }
+  if (planes < 1 || planes > GSR_FRAME_MAX_PLANES) {
+    set_error("frame_broadcast: planes = %d outside 1..%d", planes, GSR_FRAME_MAX_PLANES);
     return GSR_ERR_INVALID;
   }
   FrameArgs a;
@@ -744,10 +780,31 @@ int gsr_frame_broadcast(const gsr_tile_owner* owner, int32_t W, int32_t H, const
   for (int r = 0; r < a.world; r++)
     if (!a.peer_frame[r]) { set_error("frame_broadcast: peer frame %d is null", r); return GSR_ERR_INVALID; }
   if (a.nrows == 0 || a.world == 1 || W * H == 0) return GSR_OK;
-  dim3 grid(4, a.nrows, 4 * a.world);
+  dim3 grid(4, a.nrows, planes * a.world);
   frame_broadcast_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a);
   g_launches++;
   return check_launch("frame_broadcast", false, (cudaStream_t)stream);
+}
+
+int gsr_frame_broadcast(const gsr_tile_owner* owner, int32_t W, int32_t H, const float* frame, void* const* peer_frames,
+                        void* stream) {
+  return gsr_frame_broadcast_planes(owner, W, H, 4, frame, peer_frames, stream);
+}
+
+int gsr_peer_row_put(int32_t world, int32_t rank, const float* row, int32_t n, void* const* peer_slots, void* stream) {
+  if (world < 1 || world > GSR_MAX_PEERS || rank < 0 || rank >= world || !row || !peer_slots) {
+    set_error("peer_row_put: bad arguments");
+    return GSR_ERR_INVALID;
+  }
+  if (n < 1 || n > GSR_PEER_ROW_FLOATS) { set_error("peer_row_put: n = %d outside 1..%d", n, GSR_PEER_ROW_FLOATS); return GSR_ERR_INVALID; }
+  RowPutArgs a;
+  for (int r = 0; r < GSR_MAX_PEERS; r++) a.peer_slots[r] = r < world ? (float*)peer_slots[r] : nullptr;
+  for (int r = 0; r < world; r++)
+    if (!a.peer_slots[r]) { set_error("peer_row_put: peer slots %d are null", r); return GSR_ERR_INVALID; }
+  a.row = row; a.n = n; a.me = rank; a.world = world;
+  peer_row_put_kernel<<<1, GSR_PEER_ROW_FLOATS, 0, (cudaStream_t)stream>>>(a);
+  g_launches++;
+  return check_launch("peer_row_put", false, (cudaStream_t)stream);
 }
 
 }  // extern "C"

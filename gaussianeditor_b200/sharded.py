@@ -434,17 +434,40 @@ def shard_render(buf: ShardBuffers, color: torch.Tensor, depth: torch.Tensor):
                                         _ptr(color), _ptr(depth), st), "gsr_shard_render")
 
 
+def shard_alpha(buf: ShardBuffers, alpha: torch.Tensor):
+    """After shard_render: alpha = 1 - final_T on the owned tile rows of `alpha` [1,H,W] (other rows untouched)."""
+    lib = _lib.load()
+    device = buf.geom.device
+    with torch.cuda.device(device):
+        st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(lib.gsr_shard_alpha_image(C.byref(buf.own), _ptr(buf.img), buf.img.numel(), buf.W, buf.H, _ptr(alpha),
+                                             st), "gsr_shard_alpha_image")
+
+
 def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: torch.Tensor, img: torch.Tensor,
                           grad_out_color: torch.Tensor, acc: torch.Tensor, deterministic: bool, get,
-                          grad_depth: Optional[torch.Tensor] = None):
+                          grad_depth: Optional[torch.Tensor] = None, grad_alpha: Optional[torch.Tensor] = None):
     """gsr_shard_backward_render (or its deterministic form) of the owned tiles of a P-record workspace into
     acc [P, 12]; `get(name, numel, dtype, grow)` supplies the deterministic scratch. With `grad_depth` [1,H,W]
-    (gsr_shard_backward_render_depth) float 9 of each row also gets dL/dz."""
+    (gsr_shard_backward_render_depth) float 9 of each row also gets dL/dz. With `grad_alpha` [1,H,W]
+    (gsr_shard_backward_render_alpha, `grad_depth` optional) the alpha image's gradient enters too."""
     lib = _lib.load()
     device = geom.device
     with torch.cuda.device(device):
         grad_out_color = _f32c(grad_out_color, device)
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        if grad_alpha is not None:
+            grad_alpha = _f32c(grad_alpha, device)
+            grad_depth = None if grad_depth is None else _f32c(grad_depth, device)
+            det, dbytes = None, 0
+            if deterministic:
+                dbytes = lib.gsr_deterministic_scratch_bytes(P, R, 0)
+                det = get("det", dbytes, torch.uint8, 1.25)
+            _lib.check(lib.gsr_shard_backward_render_alpha(
+                C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), binning.numel(), _ptr(img),
+                img.numel(), _ptr(grad_out_color), _ptr(grad_alpha), _ptr(grad_depth), _ptr(acc), acc.numel() * 4,
+                _ptr(det), dbytes, st), "gsr_shard_backward_render_alpha")
+            return
         if grad_depth is not None:
             grad_depth = _f32c(grad_depth, device)
             args = (C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), binning.numel(),
@@ -468,22 +491,56 @@ def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: t
 
 
 def shard_backward_render(buf: ShardBuffers, grad_out_color: torch.Tensor, deterministic: bool = False,
-                          grad_depth: Optional[torch.Tensor] = None) -> torch.Tensor:
+                          grad_depth: Optional[torch.Tensor] = None,
+                          grad_alpha: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Backward stage 1: this rank's tiles -> partial accumulators [P_pad, 12] (zero for untouched Gaussians). With
     `deterministic` each row is the same bits on every call (no float atomics). With `grad_depth` [1,H,W] the depth
-    image's gradient enters too (dL/dz in float 9)."""
+    image's gradient enters too (dL/dz in float 9), with `grad_alpha` [1,H,W] the alpha image's."""
     device = buf.geom.device
     acc = buf.alloc("acc", buf.plan.P_pad * ACC_STRIDE, torch.float32, device).view(buf.plan.P_pad, ACC_STRIDE)
     owner_backward_render(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.binning, buf.img, grad_out_color, acc,
                           deterministic, lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow),
-                          grad_depth)
+                          grad_depth, grad_alpha)
     return acc
 
 
-def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor, depth: bool = False):
+CAM_ROW = 35   # one rank's camera-gradient partial: dL/dviewmatrix [16], dL/dprojmatrix [16], dL/dcampos [3]
+
+
+def camera_row(n: int, device):
+    """(row, gsr_camera_grads) of a shard of n Gaussians: the entry points write the partial into the zeroed `row`
+    [CAM_ROW] (an empty shard is not called and keeps its zero row). The struct keeps its scratch alive in `_keep`."""
+    lib = _lib.load()
+    row = torch.zeros(CAM_ROW, dtype=torch.float32, device=device)
+    cbytes = lib.gsr_camera_scratch_bytes(n)
+    scratch = torch.empty(cbytes, dtype=torch.uint8, device=device)
+    cam = _lib.CameraGrads(_ptr(row[:16]), _ptr(row[16:32]), _ptr(row[32:]), _ptr(scratch), cbytes)
+    cam._keep = scratch
+    return row, cam
+
+
+def combine_camera_rows(rows: torch.Tensor) -> torch.Tensor:
+    """The camera gradients of the whole cloud from the ranks' partials `rows` [world, CAM_ROW]: plain fp32 adds in
+    ascending rank order, so every rank that holds the same rows gets the same bits (an all-reduce fixes no order). At
+    world 1 the result is row 0 itself."""
+    out = rows[0].clone()
+    for r in range(1, rows.size(0)):
+        out.add_(rows[r])
+    return out
+
+
+def camera_grads_like(total: torch.Tensor, rs) -> tuple:
+    """A combined row as (dL/dviewmatrix, dL/dprojmatrix, dL/dcampos) shaped like the settings' camera arrays."""
+    return (total[:16].reshape(rs.viewmatrix.shape), total[16:32].reshape(rs.projmatrix.shape),
+            total[32:CAM_ROW].reshape(rs.campos.shape))
+
+
+def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor, depth: bool = False,
+                              camera: Optional[_lib.CameraGrads] = None):
     """Backward stage 2 (after the reduce-scatter): gradients of this rank's Gaussians, reference slot order (or the
     raw parameters' order of GaussianRasterizer.forward_raw for a raw shard). `depth`: the rows carry dL/dz (the
-    blending backward had a depth gradient)."""
+    blending backward had a depth gradient). `camera` (from camera_row, activated shards only): this rank's camera
+    partial is written too (gsr_shard_backward_preprocess_camera)."""
     lib = _lib.load()
     device = buf.geom.device
     plan = buf.plan
@@ -492,7 +549,10 @@ def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor, depth:
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         args = (C.byref(buf.s), C.byref(c), plan.P_pad, plan.base, _ptr(buf.geom), buf.geom.numel(), _ptr(buf.radii),
                 _ptr(acc_slice), C.byref(gr))
-        if raw:
+        if camera is not None:
+            _lib.check(lib.gsr_shard_backward_preprocess_camera(*args, int(depth), C.byref(camera), st),
+                       "gsr_shard_backward_preprocess_camera")
+        elif raw:
             _lib.check(lib.gsr_shard_backward_preprocess_raw(*args, int(depth), st), "gsr_shard_backward_preprocess_raw")
         elif depth:
             _lib.check(lib.gsr_shard_backward_preprocess_depth(*args, st), "gsr_shard_backward_preprocess_depth")
@@ -615,11 +675,14 @@ def grads_in_slots(grads, raw: bool):
 
 class _ShardedRasterize(torch.autograd.Function):
     """Dense exchange. `raw_rest` (features_rest) makes it the fused-activation call (see shard_preprocess);
-    `depth_grad` makes the depth output differentiable, with GaussianRasterizer(depth_grad=True)'s semantics."""
+    `depth_grad` makes the depth output differentiable, with GaussianRasterizer(depth_grad=True)'s semantics;
+    `return_alpha` adds the alpha output (a fifth frame plane); `viewmatrix` / `projmatrix` / `campos` (the settings'
+    camera arrays, or None) are the camera inputs of camera_grad."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, plan,
-                exchange, pool, deterministic=False, depth_grad=False, raw_rest=None):
+                exchange, pool, deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False,
+                viewmatrix=None, projmatrix=None, campos=None):
         ws = pool.take(means3D.device) if pool is not None else None
         buf = shard_preprocess(plan, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                ws=ws, raw_rest=raw_rest)
@@ -630,34 +693,48 @@ class _ShardedRasterize(torch.autograd.Function):
         else:
             exchange.all_gather_inplace(exchange_view(buf))
         shard_order(buf)
-        frame = torch.zeros(4, buf.H, buf.W, dtype=torch.float32, device=means3D.device)
-        shard_render(buf, frame[:3], frame[3:])
+        frame = torch.zeros(5 if return_alpha else 4, buf.H, buf.W, dtype=torch.float32, device=means3D.device)
+        shard_render(buf, frame[:3], frame[3:4])
+        if return_alpha:
+            shard_alpha(buf, frame[4:])
         exchange.all_reduce_sum(frame)
         ctx.buf, ctx.exchange, ctx.deterministic, ctx.depth_grad = buf, exchange, deterministic, bool(depth_grad)
-        if ctx.depth_grad:
-            # outputs without a gradient arrive as None: no depth gradient -> the ordinary backward, and a loss on the
-            # depth alone leaves the colour gradient None (treated as zeros)
+        ctx.return_alpha, ctx.camera_grad, ctx.rs = bool(return_alpha), viewmatrix is not None, rs
+        if ctx.depth_grad or ctx.return_alpha:
+            # outputs without a gradient arrive as None: no depth / alpha gradient -> the ordinary backward, and a loss
+            # on the depth or alpha alone leaves the colour gradient None (treated as zeros)
             ctx.set_materialize_grads(False)
         # a fresh tensor, like the single-GPU path and the reference: buf.radii lives in the pooled StepWorkspace and is
         # overwritten by the next forward that takes that workspace
         radii = shard_slice(buf.radii, plan).clone()
         ctx.mark_non_differentiable(radii)
         _ShardedRasterize.last_R = buf.R  # instrumentation only (no reference to the buffers: they must be free to die)
-        return frame[:3], radii, frame[3:]
+        if return_alpha:
+            return frame[:3], radii, frame[3:4], frame[4:]
+        return frame[:3], radii, frame[3:4]
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth):
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
         buf, exchange, det = ctx.buf, ctx.exchange, ctx.deterministic
         grad_depth = grad_depth if ctx.depth_grad else None
-        if grad_out_color is None:   # depth_grad: a loss on the depth alone
+        if grad_out_color is None:   # depth_grad / return_alpha: a loss on the depth or alpha alone
             grad_out_color = torch.zeros(3, buf.H, buf.W, dtype=torch.float32, device=buf.geom.device)
-        acc = shard_backward_render(buf, grad_out_color, det, grad_depth)
+        acc = shard_backward_render(buf, grad_out_color, det, grad_depth, grad_alpha)
         acc_slice = buf.alloc("acc_slice", buf.plan.slice_len * ACC_STRIDE, torch.float32,
                               acc.device).view(buf.plan.slice_len, ACC_STRIDE)
         (exchange.reduce_scatter_ordered if det else exchange.reduce_scatter_sum)(acc, acc_slice)
-        grads, d_rest = grads_in_slots(shard_backward_preprocess(buf, acc_slice, grad_depth is not None),
-                                       len(buf.inputs) == 8)
-        return (*grads, None, None, None, None, None, None, d_rest)
+        cam_grads = (None, None, None)
+        if ctx.camera_grad:
+            row, cam = camera_row(buf.plan.count, acc.device)
+            grads = shard_backward_preprocess(buf, acc_slice, grad_depth is not None, cam)
+            rows = torch.empty(exchange.world, CAM_ROW, dtype=torch.float32, device=acc.device)
+            rows[exchange.rank].copy_(row)
+            exchange.all_gather_inplace(rows)
+            cam_grads = camera_grads_like(combine_camera_rows(rows), ctx.rs)
+        else:
+            grads = shard_backward_preprocess(buf, acc_slice, grad_depth is not None)
+        grads, d_rest = grads_in_slots(grads, len(buf.inputs) == 8)
+        return (*grads, None, None, None, None, None, None, d_rest, None, *cam_grads)
 
 
 def p2p_available(exchange: "Exchange") -> bool:
@@ -676,6 +753,16 @@ def p2p_available(exchange: "Exchange") -> bool:
     flag = torch.tensor([1 if ok else 0], dtype=torch.int32, device=torch.device("cuda", torch.cuda.current_device()))
     exchange.dist.all_reduce(flag, op=exchange.dist.ReduceOp.MIN, group=exchange.group)
     return bool(int(flag[0]))
+
+
+def check_forward_raw_flags(module):
+    """forward_raw has neither the alpha output nor camera gradients (the fused-activation preprocess backward has no
+    camera form, and the single-GPU forward_raw offers neither). Raised before any collective, so that the peers are
+    not left waiting."""
+    flags = [f for f in ("return_alpha", "camera_grad") if getattr(module, f, False)]
+    if flags:
+        raise ValueError(f"ShardedGaussianRasterizer.forward_raw is not available on a module built with "
+                         f"{' and '.join(f + '=True' for f in flags)}: use forward with the activated parameters")
 
 
 def _check_deterministic_flag():
@@ -715,15 +802,24 @@ class ShardedGaussianRasterizer(nn.Module):
     ``GaussianRasterizer(depth_grad=True)``: when the depth gets no gradient the ordinary backward runs, and a loss on
     the depth alone works (the colour gradient is then zeros). It combines with both modes and ``deterministic``.
     ``forward_raw`` is ``GaussianRasterizer.forward_raw`` (fused activations) on this rank's rows.
+    ``return_alpha``: ``True`` makes ``forward`` return ``(color, radii_local, depth, alpha)``, alpha = 1 - final_T
+    [1,H,W] (the full frame on every rank, bit-identical to ``GaussianRasterizer(return_alpha=True)``), differentiable.
+    ``camera_grad``: ``True`` makes ``raster_settings.viewmatrix / projmatrix / campos`` autograd inputs, as on one GPU;
+    their ``.grad`` on every rank is the gradient of the whole cloud (the ranks' partials added in ascending rank
+    order), the same bits on every rank. Both combine with both modes, ``deterministic`` and ``depth_grad``; neither is
+    available on ``forward_raw``.
     """
 
     def __init__(self, raster_settings: GaussianRasterizationSettings, P_total: int, group=None,
                  p2p: Optional[bool] = None, mode: Optional[str] = None, max_in_flight: int = 3,
-                 deterministic: Optional[bool] = None, depth_grad: bool = False):
+                 deterministic: Optional[bool] = None, depth_grad: bool = False, return_alpha: bool = False,
+                 camera_grad: bool = False):
         super().__init__()
         self.raster_settings = raster_settings
         self.deterministic = bool(deterministic)
         self.depth_grad = bool(depth_grad)
+        self.return_alpha = bool(return_alpha)
+        self.camera_grad = bool(camera_grad)
         self.exchange = Exchange(group)
         self.plan = ShardPlan(int(P_total), self.exchange.world, self.exchange.rank)
         can_p2p = p2p_available(self.exchange) if (p2p is None or p2p or mode == "sparse") else False
@@ -741,7 +837,8 @@ class ShardedGaussianRasterizer(nn.Module):
             from . import sparse_sharded as SS
             dev = torch.device("cuda", torch.cuda.current_device())
             self.sparse_pool = SS.SparsePool(self.plan, dev, int(raster_settings.image_width),
-                                             int(raster_settings.image_height), self.exchange, depth=max_in_flight)
+                                             int(raster_settings.image_height), self.exchange, depth=max_in_flight,
+                                             alpha=self.return_alpha, camera=self.camera_grad)
         else:
             # fused preprocess + all-gather through peer-mapped workspaces (faster than the NCCL all-gather)
             self.pool = WorkspacePool(self.exchange, _geometry_bytes(_lib.load(), self.plan.P_pad),
@@ -776,6 +873,7 @@ class ShardedGaussianRasterizer(nn.Module):
         parameters (``_xyz, _opacity, _features_dc, _features_rest, _scaling, _rotation``); the activations and the SH
         concatenation happen inside the preprocess kernels. Returns ``(color, radii_local, depth)`` as ``forward``;
         gradients land on the raw local leaves (``means2D`` included)."""
+        check_forward_raw_flags(self)
         if not getattr(self, "deterministic", False):
             _check_deterministic_flag()
         if means3D.dim() != 2 or means3D.size(1) != 3:
@@ -787,6 +885,8 @@ class ShardedGaussianRasterizer(nn.Module):
     def _apply(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest):
         rs = self.raster_settings
         depth_grad = getattr(self, "depth_grad", False)
+        return_alpha = getattr(self, "return_alpha", False)
+        cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if getattr(self, "camera_grad", False) else (None, None, None)
         if self.mode == "sparse":
             from . import sparse_sharded as SS
             rk0 = self.sparse_pool.all[0]
@@ -794,10 +894,10 @@ class ShardedGaussianRasterizer(nn.Module):
                 raise RuntimeError("sparse mode: the image size is fixed at construction (peer-mapped frames)")
             return SS._SparseShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                                     cov3D_precomp, rs, self.sparse_pool, self.exchange,
-                                                    self.deterministic, depth_grad, raw_rest)
+                                                    self.deterministic, depth_grad, raw_rest, return_alpha, *cam)
         return _ShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                        cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic,
-                                       depth_grad, raw_rest)
+                                       depth_grad, raw_rest, return_alpha, *cam)
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):

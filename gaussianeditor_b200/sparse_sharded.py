@@ -38,6 +38,8 @@ from .sharded import (ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, _shard_clo
 MAXP = 8  # GSR_MAX_PEERS
 CTRL_BYTES, CTRL_MATRIX_OFFSET, CTRL_ERROR_OFFSET = 512, 64, 32   # GSR_PEER_CTRL_{BYTES,MATRIX_OFFSET,ERROR_OFFSET}
 AW_CNT_SLOT = 11   # GSR_SPARSE_AW_CNT_SLOT: float of an apply_weights candidate row that carries the int32 count bits
+ROW_FLOATS = 64    # GSR_PEER_ROW_FLOATS: floats per slot of gsr_peer_row_put
+CAM_SLOT_BYTES = 4 * MAXP * ROW_FLOATS   # the camera-gradient slots of a block (only with camera_grad)
 
 
 def _align(n: int, a: int = 256) -> int:
@@ -48,15 +50,21 @@ class SparseRank:
     """Buffers of one rank for ONE in-flight forward/backward: local (owner-side) workspace, the peer-visible block
     ``[control words 512 B | frame 4*H*W floats | candidate workspace]`` and small bookkeeping tensors. ``seg_cap`` may
     change from step to step (it only selects how much of the allocated candidate workspace is used); ``cap_alloc`` is
-    fixed. ``matrix`` (the [world, 8] segment counts) is a view into the control words: peers write their rows there."""
+    fixed. ``matrix`` (the [world, 8] segment counts) is a view into the control words: peers write their rows there.
+    ``alpha``: the frame has a fifth plane (the alpha image). ``camera``: the camera-gradient slots
+    [GSR_MAX_PEERS, GSR_PEER_ROW_FLOATS] floats follow the frame (slot r is written by rank r, gsr_peer_row_put)."""
 
     def __init__(self, plan: ShardPlan, device, W: int, H: int, cap_alloc: Optional[int] = None,
-                 exchange: Optional[Exchange] = None):
+                 exchange: Optional[Exchange] = None, alpha: bool = False, camera: bool = False):
         lib = _lib.load()
         self.plan, self.device, self.W, self.H = plan, device, int(W), int(H)
         self.cap_alloc = int(cap_alloc if cap_alloc is not None else max(plan.slice_len, 1))
+        self.planes = 5 if alpha else 4
         self.frame_off = CTRL_BYTES
-        self.frame_bytes = CTRL_BYTES + _align(16 * self.W * self.H)   # offset of the candidate workspace in the block
+        self.cam_off = CTRL_BYTES + _align(4 * self.planes * self.W * self.H)
+        # offset of the candidate workspace in the block
+        self.frame_bytes = self.cam_off + (CAM_SLOT_BYTES if camera else 0)
+        self.camera = bool(camera)
         self.cand_bytes_alloc = lib.gsr_sparse_candidate_bytes(plan.world, self.cap_alloc)
         if self.cand_bytes_alloc == 0:
             _lib.check(-2, "gsr_sparse_candidate_bytes")
@@ -93,6 +101,7 @@ class SparseRank:
         self.cand_ptr_array = (C.c_void_p * w)(*[(p + self.frame_bytes) if p is not None else None for p in self.base_ptrs])
         self.frame_ptr_array = (C.c_void_p * w)(*[(p + self.frame_off) if p is not None else None for p in self.base_ptrs])
         self.ctrl_ptr_array = (C.c_void_p * w)(*self.base_ptrs)
+        self.cam_ptr_array = (C.c_void_p * w)(*[(p + self.cam_off) if p is not None else None for p in self.base_ptrs])
 
     @property
     def cand(self) -> torch.Tensor:
@@ -100,7 +109,16 @@ class SparseRank:
 
     @property
     def frame(self) -> torch.Tensor:
-        return self.block[self.frame_off:self.frame_off + 16 * self.W * self.H].view(torch.float32).view(4, self.H, self.W)
+        n = self.planes * self.W * self.H
+        return self.block[self.frame_off:self.frame_off + 4 * n].view(torch.float32).view(self.planes, self.H, self.W)
+
+    @property
+    def cam_slots(self) -> torch.Tensor:
+        """[world, ROW_FLOATS] float32: slot r holds rank r's camera partial after the barrier that follows the puts."""
+        if not self.camera:
+            raise RuntimeError("this SparseRank was built without camera slots")
+        v = self.block[self.cam_off:self.cam_off + CAM_SLOT_BYTES].view(torch.float32).view(MAXP, ROW_FLOATS)
+        return v[:self.plan.world]
 
     def get(self, name: str, numel: int, dtype, grow: float = 1.0) -> torch.Tensor:
         t = self.scratch.get(name)
@@ -226,14 +244,42 @@ def sparse_render(st: SparseStep, color: torch.Tensor, depth: torch.Tensor):
                    "gsr_shard_render")
 
 
+def sparse_alpha(st: SparseStep, alpha: torch.Tensor):
+    """After sparse_render: alpha = 1 - final_T on the owned tile rows of `alpha` [1,H,W] (other rows untouched)."""
+    lib = _lib.load()
+    rk = st.rk
+    with torch.cuda.device(rk.device):
+        own = rk.plan.owner()
+        stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
+        _lib.check(lib.gsr_shard_alpha_image(C.byref(own), _ptr(st.img), st.img.numel(), rk.W, rk.H, _ptr(alpha),
+                                             stream), "gsr_shard_alpha_image")
+
+
 def frame_broadcast(rk: SparseRank):
-    """Peer stores of this rank's owned rows of ``rk.frame`` into every other rank's frame (barrier must follow)."""
+    """Peer stores of this rank's owned rows of ``rk.frame`` (all its planes) into every other rank's frame (barrier
+    must follow)."""
     lib = _lib.load()
     with torch.cuda.device(rk.device):
         own = rk.plan.owner()
         stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
-        _lib.check(lib.gsr_frame_broadcast(C.byref(own), rk.W, rk.H, _ptr(rk.frame), rk.frame_ptr_array, stream),
-                   "gsr_frame_broadcast")
+        if rk.planes == 4:
+            _lib.check(lib.gsr_frame_broadcast(C.byref(own), rk.W, rk.H, _ptr(rk.frame), rk.frame_ptr_array, stream),
+                       "gsr_frame_broadcast")
+        else:
+            _lib.check(lib.gsr_frame_broadcast_planes(C.byref(own), rk.W, rk.H, rk.planes, _ptr(rk.frame),
+                                                      rk.frame_ptr_array, stream), "gsr_frame_broadcast_planes")
+
+
+def camera_put(rk: SparseRank, row: torch.Tensor):
+    """Peer stores of this rank's camera partial `row` [CAM_ROW] into slot `rank` of every rank's camera slots
+    (gsr_peer_row_put). A peer_barrier must follow, and the slots must be read (combine_camera_rows on
+    ``rk.cam_slots``) before this rank's next barrier on the block."""
+    from .sharded import CAM_ROW
+    lib = _lib.load()
+    with torch.cuda.device(rk.device):
+        stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
+        _lib.check(lib.gsr_peer_row_put(rk.plan.world, rk.plan.rank, _ptr(row), CAM_ROW, rk.cam_ptr_array, stream),
+                   "gsr_peer_row_put")
 
 
 def peer_barrier(rk: SparseRank, with_row: bool = False):
@@ -249,9 +295,10 @@ def peer_barrier(rk: SparseRank, with_row: bool = False):
 
 
 def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, deterministic: bool = False,
-                           grad_depth: Optional[torch.Tensor] = None) -> torch.Tensor:
+                           grad_depth: Optional[torch.Tensor] = None,
+                           grad_alpha: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Blend backward of the owned tiles into the candidate accumulators [world*cap, 12] (deterministic: no float
-    atomics, every row written; `grad_depth`: dL/dz in float 9 too)."""
+    atomics, every row written; `grad_depth`: dL/dz in float 9 too; `grad_alpha`: the alpha image's gradient too)."""
     from .sharded import owner_backward_render
     lib = _lib.load()
     rk = st.rk
@@ -259,7 +306,8 @@ def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, determi
     acc = rk.get("acc", M * ACC_STRIDE, torch.float32, grow=1.25).view(M, ACC_STRIDE)
     gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
     owner_backward_render(st.s, rk.plan.owner(), M, st.R, rk.cand[:gb], st.binning, st.img, grad_out_color, acc,
-                          deterministic, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow), grad_depth)
+                          deterministic, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow), grad_depth,
+                          grad_alpha)
     return acc
 
 
@@ -273,9 +321,10 @@ def sparse_return(st: SparseStep, acc: torch.Tensor):
                    "gsr_sparse_return")
 
 
-def sparse_backward_preprocess(st: SparseStep, depth: bool = False):
+def sparse_backward_preprocess(st: SparseStep, depth: bool = False, camera: Optional[_lib.CameraGrads] = None):
     """Owner side: add the returned rows of every Gaussian (ascending rank) and run the fused preprocess backward
-    (`depth`: the rows carry dL/dz). Gradients in the order of sharded.shard_backward_preprocess."""
+    (`depth`: the rows carry dL/dz). Gradients in the order of sharded.shard_backward_preprocess. `camera` (from
+    sharded.camera_row): this rank's camera partial is written too (gsr_sparse_backward_preprocess_camera)."""
     lib = _lib.load()
     rk = st.rk
     n = st.n
@@ -286,7 +335,10 @@ def sparse_backward_preprocess(st: SparseStep, depth: bool = False):
         gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
         args = (C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local), rk.local_bytes, _ptr(rk.radii_local),
                 _ptr(rk.cand), gb, _ptr(acc_slice), acc_slice.numel() * 4, C.byref(gr))
-        if raw:
+        if camera is not None:
+            _lib.check(lib.gsr_sparse_backward_preprocess_camera(*args, int(depth), C.byref(camera), stream),
+                       "gsr_sparse_backward_preprocess_camera")
+        elif raw:
             _lib.check(lib.gsr_sparse_backward_preprocess_raw(*args, int(depth), stream),
                        "gsr_sparse_backward_preprocess_raw")
         elif depth:
@@ -313,10 +365,11 @@ class SparsePool:
     given back when that forward's state dies; every rank runs the same sequence, so workspace k here is always paired
     with workspace k on the peers. Also holds the adaptive segment capacity shared by all ranks."""
 
-    def __init__(self, plan: ShardPlan, device, W, H, exchange: Exchange, depth: int = 2):
+    def __init__(self, plan: ShardPlan, device, W, H, exchange: Exchange, depth: int = 2, alpha: bool = False,
+                 camera: bool = False):
         self.all = []
         for k in range(depth):
-            rk = SparseRank(plan, device, W, H, exchange=exchange)
+            rk = SparseRank(plan, device, W, H, exchange=exchange, alpha=alpha, camera=camera)
             rk.index = k
             self.all.append(rk)
         self.free = list(self.all)
@@ -430,11 +483,16 @@ def sparse_apply_weights(pool: SparsePool, rs, means3D, opacities, scales, rotat
 
 
 class _SparseShardedRasterize(torch.autograd.Function):
-    """Sparse exchange; `depth_grad` and `raw_rest` as in sharded._ShardedRasterize."""
+    """Sparse exchange; `depth_grad`, `raw_rest`, `return_alpha` and the camera inputs as in sharded._ShardedRasterize
+    (the pool must have been built with the alpha plane / camera slots)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange,
-                deterministic=False, depth_grad=False, raw_rest=None):
+                deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False, viewmatrix=None,
+                projmatrix=None, campos=None):
+        rk0 = pool.all[0]
+        if (return_alpha and rk0.planes != 5) or (viewmatrix is not None and not rk0.camera):
+            raise RuntimeError("return_alpha / camera gradients need a SparsePool built with alpha=True / camera=True")
         rk = pool.take()
         device = means3D.device
         _mark("start")
@@ -448,35 +506,52 @@ class _SparseShardedRasterize(torch.autograd.Function):
         # Every pixel has exactly one writer (the owner of its tile row; empty tiles are written too), so the frame needs
         # no zero-fill -- and must not get one: a faster peer may already have stored its rows here.
         frame = rk.frame
-        sparse_render(st, frame[:3], frame[3:])
+        sparse_render(st, frame[:3], frame[3:4])
+        if return_alpha:   # every pixel of the alpha plane has one writer too: the owner of its tile row
+            sparse_alpha(st, frame[4:5])
         _mark("bin+blend")
         frame_broadcast(rk)
         peer_barrier(rk)
         out = frame.clone()                                 # the peer-visible frame is overwritten by the next step
         _mark("frame broadcast+barrier")
         ctx.st, ctx.exchange, ctx.deterministic, ctx.depth_grad = st, exchange, deterministic, bool(depth_grad)
-        if ctx.depth_grad:   # None = no gradient for that output (see sharded._ShardedRasterize)
+        ctx.return_alpha, ctx.camera_grad, ctx.rs = bool(return_alpha), viewmatrix is not None, rs
+        if ctx.depth_grad or ctx.return_alpha:   # None = no gradient for that output (see sharded._ShardedRasterize)
             ctx.set_materialize_grads(False)
         radii = rk.radii_local[:rk.plan.count].clone()
         ctx.mark_non_differentiable(radii)
         _SparseShardedRasterize.last = dict(R=R, cap=st.cap, max_count=max_count)
-        return out[:3], radii, out[3:]
+        if return_alpha:
+            return out[:3], radii, out[3:4], out[4:5]
+        return out[:3], radii, out[3:4]
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth):
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
+        from .sharded import CAM_ROW, camera_grads_like, camera_row, combine_camera_rows
         st, exchange = ctx.st, ctx.exchange
         if st is None:
             raise RuntimeError("the sharded rasterizer's backward can run once (its workspace went back to the pool)")
         _mark("loss")
         grad_depth = grad_depth if ctx.depth_grad else None
-        if grad_out_color is None:   # depth_grad: a loss on the depth alone
+        if grad_out_color is None:   # depth_grad / return_alpha: a loss on the depth or alpha alone
             grad_out_color = torch.zeros(3, st.rk.H, st.rk.W, dtype=torch.float32, device=st.rk.device)
-        acc = sparse_backward_render(st, grad_out_color, ctx.deterministic, grad_depth)
+        acc = sparse_backward_render(st, grad_out_color, ctx.deterministic, grad_depth, grad_alpha)
         _mark("blend backward")
         sparse_return(st, acc)
         peer_barrier(st.rk)
         _mark("return push+barrier")
-        grads, d_rest = grads_in_slots(sparse_backward_preprocess(st, grad_depth is not None), len(st.inputs) == 8)
+        cam_grads = (None, None, None)
+        if ctx.camera_grad:
+            row, cam = camera_row(st.n, st.rk.device)
+            grads = sparse_backward_preprocess(st, grad_depth is not None, cam)
+            camera_put(st.rk, row)
+            peer_barrier(st.rk)
+            # read before this rank's next barrier on the block: no peer can store into the slots again until then
+            cam_grads = camera_grads_like(combine_camera_rows(st.rk.cam_slots[:, :CAM_ROW]), ctx.rs)
+            _mark("camera put+barrier")
+        else:
+            grads = sparse_backward_preprocess(st, grad_depth is not None)
+        grads, d_rest = grads_in_slots(grads, len(st.inputs) == 8)
         _mark("gather+preprocess backward")
         ctx.st = None   # the workspace goes back to the pool now, not when the output tensors die
-        return (*grads, None, None, None, None, None, d_rest)
+        return (*grads, None, None, None, None, None, d_rest, None, *cam_grads)

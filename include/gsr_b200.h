@@ -187,8 +187,9 @@ GSR_API int gsr_backward_camera(const gsr_settings* s, const gsr_cloud* c, int32
  * dL_dout_color for a loss on the depth alone. The blending backward always runs render_bwd variant 15 here.
  * gsr_backward_raw_depth is the same for gsr_backward_raw (fused activations, below).
  * The Gaussian-sharded path has its own depth entry points (gsr_shard_backward_render_depth,
- * gsr_shard_backward_preprocess_depth / _raw and gsr_sparse_backward_preprocess_depth / _raw, below); they take no
- * alpha or camera gradient. */
+ * gsr_shard_backward_preprocess_depth / _raw and gsr_sparse_backward_preprocess_depth / _raw, below). Its alpha and
+ * camera gradients go through gsr_shard_backward_render_alpha and gsr_shard_backward_preprocess_camera /
+ * gsr_sparse_backward_preprocess_camera, which take the depth gradient too. */
 GSR_API int gsr_backward_depth(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered, const void* geometry,
                        size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                        size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
@@ -385,6 +386,32 @@ GSR_API int gsr_shard_backward_preprocess_raw(const gsr_settings* s, const gsr_r
                                               int32_t index_base, const void* geometry, size_t geometry_bytes,
                                               const int32_t* radii_total, const void* acc_slice,
                                               const gsr_raw_grads* grads, int32_t depth, void* stream);
+/* Alpha image and camera gradients of a sharded cloud (see gsr_alpha_image and gsr_backward_camera).
+ *   gsr_shard_alpha_image: after gsr_shard_render, out_alpha [H*W] = 1 - final_T on the tile rows `owner` owns only
+ *       (final_T elsewhere in a shard's image workspace is not written); every other pixel is left untouched, so the
+ *       alpha plane travels with the frame (all-reduce of a zero-filled [5,H,W] frame, or gsr_frame_broadcast_planes).
+ *   gsr_shard_backward_render_alpha: gsr_shard_backward_render_depth with the alpha image's upstream gradient
+ *       dL_dout_alpha [H*W] (must not be NULL). dL_dout_depth may be NULL (no depth gradient) and det_scratch may be
+ *       NULL (float atomics), so one entry covers alpha x depth x deterministic.
+ *   gsr_shard_backward_preprocess_camera: gsr_shard_backward_preprocess (depth = 0) or its DEPTH form (depth != 0) that
+ *       also writes THIS RANK'S PARTIAL camera gradients (its Gaussians only; zeros for an empty shard) into `camera`
+ *       (scratch: gsr_camera_scratch_bytes(shard.P)). The host sums the ranks' partials in ascending rank order on every
+ *       rank (not with an all-reduce, whose order is not fixed), which gives every rank the same bits; at world 1 the
+ *       partial is the single-GPU gsr_backward_camera result. */
+GSR_API int gsr_shard_alpha_image(const gsr_tile_owner* owner, const void* image, size_t image_bytes,
+                                  int32_t image_width, int32_t image_height, float* out_alpha, void* stream);
+GSR_API int gsr_shard_backward_render_alpha(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                            int32_t num_rendered, const void* geometry, size_t geometry_bytes,
+                                            const void* binning, size_t binning_bytes, const void* image,
+                                            size_t image_bytes, const float* dL_dout_color, const float* dL_dout_alpha,
+                                            const float* dL_dout_depth /* may be NULL */, void* acc_total,
+                                            size_t acc_bytes, void* det_scratch /* may be NULL */,
+                                            size_t det_scratch_bytes, void* stream);
+GSR_API int gsr_shard_backward_preprocess_camera(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                                 int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                                 const int32_t* radii_total, const void* acc_slice,
+                                                 const gsr_grads* grads, int32_t depth, const gsr_camera_grads* camera,
+                                                 void* stream);
 /* Semantic tracing (gsr_apply_weights) of a sharded cloud. After gsr_shard_order (with the same owner and workspaces),
  * bins the owned tile rows and walks them: every hit of splat i (GLOBAL index) adds the pixel's mask value to
  * weights_total[i*weights_stride + ch] (ch < num_channels, float atomics) and num_channels to
@@ -553,6 +580,30 @@ GSR_API int gsr_peer_barrier(int32_t world, int32_t rank, void* const* peer_ctrl
  * must follow before the frames are read. */
 GSR_API int gsr_frame_broadcast(const gsr_tile_owner* owner, int32_t image_width, int32_t image_height, const float* frame,
                         void* const* peer_frames /* [world] host */, void* stream);
+/* gsr_frame_broadcast of a [planes,H,W] frame, 1 <= planes <= GSR_FRAME_MAX_PLANES (the same kernel; gsr_frame_broadcast
+ * is the 4-plane call). The sharded alpha output uses 5: colour, depth, then alpha from gsr_shard_alpha_image. */
+#define GSR_FRAME_MAX_PLANES 5
+GSR_API int gsr_frame_broadcast_planes(const gsr_tile_owner* owner, int32_t image_width, int32_t image_height,
+                                       int32_t planes, const float* frame, void* const* peer_frames /* [world] host */,
+                                       void* stream);
+/* All-gather of one small float row over peer memory: row[0..n) (device, 1 <= n <= GSR_PEER_ROW_FLOATS) is stored bit for
+ * bit into slot `rank` of every rank's [GSR_MAX_PEERS][GSR_PEER_ROW_FLOATS] float slots (peer_slots[r] = rank r's slots
+ * as mapped here, own entry included). A gsr_peer_barrier must follow before the slots are read, and every rank must
+ * read its slots before it enters the next barrier on the same block (then no peer can store into them again before
+ * they are read). The sparse exchange gathers the ranks' camera-gradient partials this way. */
+#define GSR_PEER_ROW_FLOATS 64
+GSR_API int gsr_peer_row_put(int32_t world, int32_t rank, const float* row, int32_t n,
+                             void* const* peer_slots /* [world] host */, void* stream);
+/* Camera gradients with the sparse exchange: gsr_sparse_backward_preprocess (depth = 0) or its DEPTH form (depth != 0)
+ * that also runs the CAM preprocess backward on this rank's shard and writes THIS RANK'S PARTIAL camera gradients (its
+ * Gaussians only; zeros for an empty shard) into `camera` (scratch: gsr_camera_scratch_bytes(shard.P)). Summing the
+ * ranks' partials in ascending rank order on every rank gives every rank the same bits; at world 1 the partial is the
+ * single-GPU gsr_backward_camera result. */
+GSR_API int gsr_sparse_backward_preprocess_camera(const gsr_settings* s, const gsr_cloud* shard,
+                                                  const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                                  const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
+                                                  void* acc_slice, size_t acc_bytes, const gsr_grads* grads,
+                                                  int32_t depth, const gsr_camera_grads* camera, void* stream);
 
 /* ---- tuning / instrumentation ---------------------------------------------------------------------------
  * gsr_set_option("render_variant", v) etc.; unknown names return GSR_ERR_INVALID.

@@ -165,6 +165,67 @@ def check_fused_depth(a, cloud, cam, bg, dL, dev):
         (" fused_depth=ok" if ok else " fused_depth=FAILED")
 
 
+def check_alpha_camera(a, cloud, cam, bg, dL, dev, world):
+    """--alpha and/or --camera-grad (with depth_grad=True) against GaussianRasterizer with the same options on the full
+    cloud, for a colour + alpha + depth loss (the alpha term only with --alpha): colour, depth, alpha and radii
+    bit-identical; per-Gaussian gradients within 2e-5 relative L2; each camera array within 1e-4 relative L2 (or 10x
+    the single-GPU call-to-call spread if larger) and the same bits on every rank."""
+    import hashlib
+    P = cloud.means3D.shape[0]
+    base = settings_from(cam, bg, cloud.sh_degree, dev)
+    g = np.random.default_rng(11)
+    dD = torch.from_numpy(g.random((1, cam.image_height, cam.image_width), dtype=np.float32) * 0.1).to(dev)
+    dA = torch.from_numpy(g.random((1, cam.image_height, cam.image_width), dtype=np.float32) - 0.5).to(dev)
+    t = cloud_tensors(cloud, dev)
+    cam_keys = ("viewmatrix", "projmatrix", "campos")
+    opts = dict(return_alpha=a.alpha, camera_grad=a.camera_grad, depth_grad=True)
+
+    def settings():
+        if not a.camera_grad:
+            return base
+        return base._replace(**{k: getattr(base, k).clone().requires_grad_(True) for k in cam_keys})
+
+    def run(make, tensors):
+        rs = settings()
+        r = make(rs)
+        leaves = {k: v.detach().clone().requires_grad_(True) for k, v in tensors.items()}
+        m2 = torch.zeros_like(leaves["means3D"], requires_grad=True)
+        out = r(means3D=leaves["means3D"], means2D=m2, opacities=leaves["opacities"], shs=leaves["shs"],
+                scales=leaves["scales"], rotations=leaves["rotations"])
+        loss = (out[0] * dL).sum() + (out[2] * dD).sum() + ((out[3] * dA).sum() if a.alpha else 0.0)
+        loss.backward()
+        grads = {k: v.grad for k, v in leaves.items()}
+        grads["means2D"] = m2.grad
+        cams = {k: getattr(rs, k).grad for k in cam_keys} if a.camera_grad else {}
+        torch.cuda.synchronize()
+        return [o.detach() for o in out], grads, cams
+
+    rast = S.ShardedGaussianRasterizer(base, P, p2p=(True if a.mode == 'sparse' else a.p2p), mode=a.mode, **opts)
+    ref_out, ref_g, ref_c = run(lambda rs: GaussianRasterizer(rs, **opts), t)
+    _, _, ref_c2 = run(lambda rs: GaussianRasterizer(rs, **opts), t)
+    out, grads, cams = run(lambda rs: (setattr(rast, "raster_settings", rs), rast)[1],
+                           {k: S.shard_slice(v, rast.plan) for k, v in t.items()})
+    ok = all(torch.equal(out[i], ref_out[i]) for i in (0, 2) + ((3,) if a.alpha else ()))
+    ok = ok and torch.equal(out[1], S.shard_slice(ref_out[1], rast.plan))
+    worst = max(rel_l2(v.cpu().numpy(), S.shard_slice(ref_g[k], rast.plan).cpu().numpy()) for k, v in grads.items())
+    ok = ok and worst <= 2e-5
+    cworst, spread = 0.0, 0.0
+    for k in cams:
+        spread = max(spread, rel_l2(ref_c2[k].cpu().numpy(), ref_c[k].cpu().numpy()))
+        cworst = max(cworst, rel_l2(cams[k].cpu().numpy(), ref_c[k].cpu().numpy()))
+    ok = ok and cworst <= max(1e-4, 10 * spread)
+    if a.camera_grad:
+        ok = ok and not cams["viewmatrix"][:, 3].any() and not cams["projmatrix"][:, 2].any()
+        mine = hashlib.sha256(b"".join(cams[k].cpu().numpy().tobytes() for k in cam_keys)).hexdigest()
+        digests = [None] * world
+        dist.all_gather_object(digests, mine)
+        ok = ok and len(set(digests)) == 1
+    rast.close()
+    return ok, (f" alpha={a.alpha} camera_grad={a.camera_grad} alpha_camera_worst_rel_l2={worst:.2e}"
+                f" camera_worst_rel_l2={cworst:.2e} camera_spread={spread:.2e}") + \
+        (" alpha_camera=ok" if ok else " alpha_camera=FAILED")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="c3")
@@ -180,6 +241,10 @@ def main():
                     help="also check forward_raw (fused activations) on the local rows against the single-GPU one")
     ap.add_argument("--depth-grad", action="store_true",
                     help="also check depth_grad=True with a colour + depth loss and a depth-only loss")
+    ap.add_argument("--alpha", action="store_true",
+                    help="also check return_alpha=True (alpha frame and a loss on it) against the single-GPU one")
+    ap.add_argument("--camera-grad", action="store_true",
+                    help="also check camera_grad=True: camera gradients of the whole cloud, the same bits on every rank")
     ap.add_argument("--no-fill", action="store_true",
                     help="with --deterministic: torch.utils.deterministic.fill_uninitialized_memory = False")
     a = ap.parse_args()
@@ -250,6 +315,10 @@ def main():
         fd_ok, fd_msg = check_fused_depth(a, cloud, cam, bg, dL, dev)
         ok = ok and fd_ok
         aw_msg += fd_msg
+    if a.alpha or a.camera_grad:
+        ac_ok, ac_msg = check_alpha_camera(a, cloud, cam, bg, dL, dev, world)
+        ok = ok and ac_ok
+        aw_msg += ac_msg
     det_digest = None
     if a.deterministic:
         det_ok, det_digest, det_msg = check_deterministic(a, cloud, cams, bg, dL, dev, rank, world)
