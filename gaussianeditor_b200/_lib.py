@@ -38,6 +38,7 @@ SYMBOLS = [
     "gsr_shard_backward_preprocess_raw", "gsr_sparse_backward_preprocess_raw",
     "gsr_shard_alpha_image", "gsr_shard_backward_render_alpha", "gsr_shard_backward_preprocess_camera",
     "gsr_sparse_backward_preprocess_camera", "gsr_frame_broadcast_planes", "gsr_peer_row_put",
+    "gsr_forward_static", "gsr_forward_static_raw",
 ]
 
 
@@ -226,6 +227,10 @@ def load():
     lib.gsr_shard_backward_preprocess_raw.argtypes = [S, RC, i32, i32, vp, sz, vp, vp, RG, i32, vp]
     lib.gsr_forward_preprocess_raw.restype = C.c_int
     lib.gsr_forward_preprocess_raw.argtypes = [S, C.POINTER(RawCloud), vp, sz, vp, vp, vp]
+    lib.gsr_forward_static.restype = C.c_int
+    lib.gsr_forward_static.argtypes = [S, Cl, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp]
+    lib.gsr_forward_static_raw.restype = C.c_int
+    lib.gsr_forward_static_raw.argtypes = [S, RC, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp]
     lib.gsr_backward_raw.restype = C.c_int
     lib.gsr_backward_raw.argtypes = [S, C.POINTER(RawCloud), i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, sz,
                                      C.POINTER(RawGrads), vp]

@@ -189,7 +189,8 @@ static int carve_det_checked(const DetScratch& ds, int P, int64_t R, int CH, Det
 
 // First forward half on a carved workspace: preprocess, depth order, tile-count scan, and the copy of num_rendered to
 // the host. With the tile-binning path (tile_binning.cu) the preprocess kernel accumulates the count itself, so the copy
-// is issued right behind it and the host learns R while the GPU is still sorting.
+// is issued right behind it and the host learns R while the GPU is still sorting. num_rendered_host == nullptr (the
+// static-capacity forward): no copy at all, R stays on the device.
 static int first_half(const gsr_settings& s, const gsr_cloud& c, const GeometryWS& g, int32_t* radii,
                       int32_t* num_rendered_host, cudaStream_t st, bool raw, const float* features_rest) {
   const int gx = (s.image_width + TILE - 1) / TILE, gy = (s.image_height + TILE - 1) / TILE;
@@ -202,8 +203,10 @@ static int first_half(const gsr_settings& s, const gsr_cloud& c, const GeometryW
     if (rc) return rc;
     if (v2) {
       if ((rc = launch_tile_count(g, gx, gy, TileOwner(), st))) return rc;
-      cudaError_t e = cudaMemcpyAsync(num_rendered_host, g.R_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
-      if (e != cudaSuccess) return check_cuda(e, "num_rendered readback");
+      if (num_rendered_host) {
+        cudaError_t e = cudaMemcpyAsync(num_rendered_host, g.R_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
+        if (e != cudaSuccess) return check_cuda(e, "num_rendered readback");
+      }
     }
   }
   StageScope t(ST_DEPTH_SCAN, st);
@@ -272,6 +275,55 @@ int gsr_forward_render_speculative(const gsr_settings* s, const gsr_cloud* c, in
   if (capacity <= 0) { set_error("speculative capacity must be positive"); return GSR_ERR_INVALID; }
   return forward_render_impl(s, c, capacity, true, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes,
                              radii, out_color, out_depth, stream);
+}
+
+// Both forward halves for a caller-given capacity, with R kept on the device (gsr_forward_static and, with `raw`,
+// gsr_forward_static_raw; `c` is then the raw cloud seen through raw_to_cloud). Every argument is checked before the
+// first launch; the second half is the speculative one, and launch_static_status reports R and empties an overflowing
+// frame.
+static int forward_static_impl(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
+                               size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                               size_t image_bytes, int32_t* radii, float* out_color, float* out_depth, int32_t* status,
+                               void* stream, bool raw, const float* features_rest) {
+  if (capacity <= 0) { set_error("static capacity must be positive"); return GSR_ERR_INVALID; }
+  if (!status) { set_error("status is null"); return GSR_ERR_INVALID; }
+  if (!out_color || !out_depth) { set_error("output images are null"); return GSR_ERR_INVALID; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t npix = (size_t)s->image_width * s->image_height;
+  if (c->P == 0) {  // as forward_render_impl: outputs stay zero, and so do R and the overflow flag
+    cudaError_t e = cudaMemsetAsync(status, 0, 2 * sizeof(int32_t), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(out_color, 0, 3 * npix * sizeof(float), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(out_depth, 0, npix * sizeof(float), st);
+    return check_cuda(e, "zero outputs");
+  }
+  if (!radii || !geometry) { set_error("radii / geometry workspace is null"); return GSR_ERR_INVALID; }
+  GeometryWS g; BinningWS b; ImageWS im;
+  int rc = carve_all(s, c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, g, b, im);
+  if (rc) return rc;
+  if ((rc = first_half(*s, *c, g, radii, nullptr, st, raw, features_rest))) return rc;
+  if ((rc = run_binning(*s, *c, capacity, true, g, b, im, radii, st))) return rc;
+  if ((rc = launch_static_status(*s, c->P, (uint32_t)capacity, g, im, status, st))) return rc;
+  StageScope t(ST_RENDER_FWD, st);
+  return launch_render_fwd(*s, g, b, im, out_color, out_depth, st);
+}
+
+int gsr_forward_static(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
+                       size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                       int32_t* radii, float* out_color, float* out_depth, int32_t* status, void* stream) {
+  const int rc = validate_cloud(s, c);
+  if (rc) return rc;
+  return forward_static_impl(s, c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                             out_color, out_depth, status, stream, false, nullptr);
+}
+
+int gsr_forward_static_raw(const gsr_settings* s, const gsr_raw_cloud* r, int32_t capacity, void* geometry,
+                           size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                           int32_t* radii, float* out_color, float* out_depth, int32_t* status, void* stream) {
+  gsr_cloud c;
+  const int rc = raw_to_cloud(s, r, c);
+  if (rc) return rc;
+  return forward_static_impl(s, &c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes,
+                             radii, out_color, out_depth, status, stream, true, r->features_rest);
 }
 
 static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry, size_t geometry_bytes,

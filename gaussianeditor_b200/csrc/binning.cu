@@ -200,6 +200,29 @@ __global__ void tile_ranges_kernel(int cap, const uint32_t* __restrict__ R_dev, 
   }
 }
 
+// Static-capacity forward: the host never learns R, so the device reports it. When R exceeds the capacity the lists
+// were sized for, the tile-binning path has already left every range empty (tile_prefix_kernel) but the CUB path holds
+// the first `cap` instances in sorted order; both are reduced to the same empty frame here, before the render: zero
+// ranges (colour = background, depth = 0, alpha = 0) and zero per-Gaussian tile counts, so that the deterministic
+// reduction, whose runs [excl, excl + tiles_touched) would reach past the capacity, has nothing to read.
+constexpr int STATUS_THREADS = 256;
+__global__ void __launch_bounds__(STATUS_THREADS)
+static_status_kernel(int P, int ntile, uint32_t cap, const uint32_t* __restrict__ R_dev, uint2* __restrict__ ranges,
+                     uint32_t* __restrict__ tiles_touched, int32_t* __restrict__ status) {
+  const uint32_t R = __ldg(R_dev);
+  const bool overflow = R > cap;
+  const int i0 = blockIdx.x * STATUS_THREADS + threadIdx.x;
+  if (i0 == 0) {
+    status[0] = (int32_t)R;
+    status[1] = overflow ? 1 : 0;
+  }
+  if (!overflow) return;
+  for (int i = i0; i < max(P, ntile); i += gridDim.x * STATUS_THREADS) {
+    if (i < ntile) ranges[i] = make_uint2(0u, 0u);
+    if (i < P) tiles_touched[i] = 0u;
+  }
+}
+
 // CUB's temp-size queries depend only on the item count but cost several runtime calls each; every C-ABI entry point
 // re-derives the workspace layout, so they are memoised (single-threaded callers per the ABI; a mutex keeps it safe).
 struct SizeCache {
@@ -404,6 +427,18 @@ int run_binning(const gsr_settings& s, const gsr_cloud& c, int R, bool speculati
   if ((int64_t)gx * gy < 65536 && g_opt.tile_key_bits == 16)
     return bin_typed<uint16_t>(c, R, speculative, gx, gy, g, b, im, radii, st, debug, own);
   return bin_typed<uint32_t>(c, R, speculative, gx, gy, g, b, im, radii, st, debug, own);
+}
+
+int launch_static_status(const gsr_settings& s, int P, uint32_t capacity, const GeometryWS& g, const ImageWS& im,
+                         int32_t* status, cudaStream_t st) {
+  const int gx = (s.image_width + TILE - 1) / TILE, gy = (s.image_height + TILE - 1) / TILE;
+  // the count run_binning compared against the capacity: tile_count_kernel's on the tile-binning path, else the scan's
+  const uint32_t* R_dev = tile_binning_supported(gx, gy) ? g.R_dev : g.offsets + (P - 1);
+  const int n = P > gx * gy ? P : gx * gy;
+  const int blocks = std::min((n + STATUS_THREADS - 1) / STATUS_THREADS, 1024);
+  static_status_kernel<<<blocks, STATUS_THREADS, 0, st>>>(P, gx * gy, capacity, R_dev, im.ranges, g.tiles_touched, status);
+  g_launches++;
+  return check_launch("static_status", s.debug != 0, st);
 }
 
 int launch_retouch(const gsr_settings& s, int P, const GeometryWS& g, int32_t* radii, const TileOwner& own,

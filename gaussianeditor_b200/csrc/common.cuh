@@ -185,6 +185,10 @@ int launch_retouch(const gsr_settings& s, int P, const GeometryWS& g, int32_t* r
 int run_binning(const gsr_settings& s, const gsr_cloud& c, int R, bool speculative, const GeometryWS& g,
                 const BinningWS& b, const ImageWS& im, const int32_t* radii, cudaStream_t st,
                 const TileOwner& own = TileOwner());
+// Static-capacity forward, after run_binning(.., capacity, speculative = true, ..): status[0..1] = {R, R > capacity}
+// from the device count; on overflow every tile range and every per-Gaussian tile count is zeroed (an empty frame).
+int launch_static_status(const gsr_settings& s, int P, uint32_t capacity, const GeometryWS& g, const ImageWS& im,
+                         int32_t* status, cudaStream_t st);
 // tile_binning.cu: ranges from the tile-count difference array, emission fused into the first of two own radix passes
 constexpr int SORT_TILE = 4096;  // instances per CTA of a radix pass
 bool tile_binning_supported(int gx, int gy);

@@ -16,6 +16,11 @@ simple_knn and the reference tree are absent): same property names (`get_xyz`, `
 (sigmoid / exp / normalize, scene/gaussian_model.py:47-58,221-258), so `gaussian_renderer.render()` consumes it exactly
 as it consumes the real model.  The rasterizer implementation is injected, so the same loop runs on this repository's
 kernels and on the reference's CUDA build (oracle/ref_torch.py) for the A/B render-time fraction.
+
+`run_edit_loop(..., cuda_graph=True)` captures the whole step (both forwards, loss, backward, densification stats and
+``Adam(capturable=True)``) once per Gaussian count with ``torch.cuda.graph`` and replays it, on the rasterizer's
+static-capacity forward; ``static_capacity=True`` runs the same step eagerly. Both never synchronise between
+densification points.
 """
 from __future__ import annotations
 
@@ -32,7 +37,8 @@ from .rasterizer import GaussianRasterizationSettings
 
 
 class EditScene:
-    def __init__(self, cloud: synth.Cloud, device):
+    def __init__(self, cloud: synth.Cloud, device, capturable: bool = False):
+        self.capturable = capturable   # Adam(capturable=True): the optimizer step can be captured in a CUDA graph
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
         eps = 1e-6
         self._xyz = t(cloud.means3D).requires_grad_(True)
@@ -56,7 +62,11 @@ class EditScene:
                 ("opacity", self._opacity, 0.1), ("scaling", self._scaling, 1e-2), ("rotation", self._rotation, 2e-3)]
 
     def _make_optimizer(self):
-        self.optimizer = torch.optim.Adam([{"params": [p], "lr": lr, "name": n} for n, p, lr in self._params()], eps=1e-15)
+        groups = [{"params": [p], "lr": lr, "name": n} for n, p, lr in self._params()]
+        if self.capturable:
+            self.optimizer = torch.optim.Adam(groups, eps=1e-15, capturable=True)
+        else:
+            self.optimizer = torch.optim.Adam(groups, eps=1e-15)
 
     # -- the reference model's read API ---------------------------------------------------------------------
     @property
@@ -73,6 +83,13 @@ class EditScene:
     def add_densification_stats(self, viewspace_grad, update_filter):   # scene/gaussian_model.py:811-815
         self.xyz_gradient_accum[update_filter] += torch.norm(viewspace_grad[update_filter, :2], dim=-1, keepdim=True)
         self.denom[update_filter] += 1
+
+    def add_densification_stats_dense(self, viewspace_grad, update_filter):
+        """add_densification_stats without boolean indexing (no host synchronisation, so it can be captured): the same
+        values, since the rows outside the filter add exactly 0."""
+        norm = torch.norm(viewspace_grad[:, :2], dim=-1, keepdim=True)
+        self.xyz_gradient_accum.add_(torch.where(update_filter[:, None], norm, 0.0))
+        self.denom.add_(update_filter[:, None].float())
 
     def densify_and_prune(self, max_densify_percent=0.01, min_opacity=0.005):
         """Clone the `max_densify_percent` Gaussians with the largest mean view-space gradient, prune those below
@@ -105,15 +122,22 @@ def make_view(cam: synth.Camera, device):
 
 
 def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densification_interval=100, seed=0,
-                  log=None, fused_activations=False):
+                  log=None, fused_activations=False, cuda_graph=False, static_capacity=False, deterministic=None):
     """Returns a dict with total / render wall times (CUDA-event timed) and the per-step Gaussian counts.
-    ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only)."""
+    ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only).
+    ``cuda_graph=True`` captures one step per Gaussian count and replays it (see the module docstring);
+    ``static_capacity=True`` runs that same step eagerly. Both size the rasterizer's static capacity as
+    1.25 x the largest num_rendered over an eager pass of all views + 4096, recomputed after every densification, use
+    Adam(capturable=True), and raise RuntimeError at the next densification point (or the end) if any forward
+    exceeded the capacity. ``deterministic`` is passed to ``render`` when given."""
     from . import gaussian_renderer as GR
+    fixed = bool(cuda_graph or static_capacity)
     cloud, cams = synth.make_config("c5", P=P)
-    scene = EditScene(cloud, device)
+    scene = EditScene(cloud, device, capturable=fixed)
     views = [make_view(c, device) for c in cams]
     pipe = SimpleNamespace(convert_SHs_python=False, compute_cov3D_python=False, debug=False)
     bg = torch.zeros(3, device=device)
+    opt = {} if deterministic is None else {"deterministic": bool(deterministic)}
     # the rasterizer class is injected by swapping the name render() resolves
     old = GR.GaussianRasterizer
     GR.GaussianRasterizer = rasterizer_cls
@@ -125,6 +149,8 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
             for v in views:
                 img = GR.render(v, scene, pipe, bg)["render"]
                 targets.append((img + 0.05 * torch.randn(img.shape, generator=g, device=device)).clamp(0, 1))
+        if fixed:
+            loop = _FixedCapacityStep(GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph)
         render_ms = 0.0
         counts, losses, radii_trace = [], [], []
         rng = np.random.default_rng(seed)
@@ -134,37 +160,133 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
         pend = []
         for step in range(1, steps + 1):
             k = int(rng.integers(len(views)))
-            e0, e1, e2, e3 = ev(), ev(), ev(), ev()
-            e0.record()
-            pkg = GR.render(views[k], scene, pipe, bg, fused_activations=fused_activations)       # forward #1
-            sem = GR.render(views[k], scene, pipe, bg,
-                            override_color=scene.mask[..., None].float().repeat(1, 3))["render"]  # forward #2
-            e1.record()
-            semantic = torch.norm(sem, dim=0) > 0.8                                               # thresholded: no grad
-            loss = 10.0 * (pkg["render"] - targets[k]).abs().mean() + 0.0 * semantic.float().mean()
-            scene.optimizer.zero_grad(set_to_none=True)
-            e2.record()
-            loss.backward()                                                                       # rasterizer backward
-            e3.record()
-            pend.append((e0, e1, e2, e3))
-            with torch.no_grad():
-                vis = pkg["visibility_filter"]
-                scene.max_radii2D[vis] = torch.max(scene.max_radii2D[vis], pkg["radii"][vis].float())
-                scene.add_densification_stats(pkg["viewspace_points"].grad, vis)
-            scene.optimizer.step()
+            if fixed:
+                loss = loop.step(k)
+            else:
+                e0, e1, e2, e3 = ev(), ev(), ev(), ev()
+                e0.record()
+                pkg = GR.render(views[k], scene, pipe, bg, fused_activations=fused_activations)       # forward #1
+                sem = GR.render(views[k], scene, pipe, bg,
+                                override_color=scene.mask[..., None].float().repeat(1, 3))["render"]  # forward #2
+                e1.record()
+                semantic = torch.norm(sem, dim=0) > 0.8                                               # thresholded: no grad
+                loss = 10.0 * (pkg["render"] - targets[k]).abs().mean() + 0.0 * semantic.float().mean()
+                scene.optimizer.zero_grad(set_to_none=True)
+                e2.record()
+                loss.backward()                                                                       # rasterizer backward
+                e3.record()
+                pend.append((e0, e1, e2, e3))
+                with torch.no_grad():
+                    vis = pkg["visibility_filter"]
+                    scene.max_radii2D[vis] = torch.max(scene.max_radii2D[vis], pkg["radii"][vis].float())
+                    scene.add_densification_stats(pkg["viewspace_points"].grad, vis)
+                scene.optimizer.step()
             losses.append(loss.detach())
             if step % densification_interval == 0 and step < steps:
+                if fixed:
+                    loop.check_capacity()
                 radii_trace.append(scene.max_radii2D.clone())   # what the reference's prune test reads (:790-795)
                 scene.densify_and_prune()
+                if fixed:
+                    loop.reset()
             counts.append(scene._xyz.shape[0])
         t_all1.record()
         torch.cuda.synchronize()
+        if fixed:
+            loop.check_capacity()
         for e0, e1, e2, e3 in pend:   # backward time includes the few autograd elementwise kernels around it
             render_ms += e0.elapsed_time(e1) + e2.elapsed_time(e3)
         total_ms = t_all0.elapsed_time(t_all1)
     finally:
         GR.GaussianRasterizer = old
-    return dict(steps=steps, total_ms=total_ms, render_ms=render_ms, render_fraction=render_ms / total_ms,
-                ms_per_step=total_ms / steps, P_first=counts[0], P_last=counts[-1], final_loss=float(loss.detach()),
-                counts=counts, losses=torch.stack(losses).cpu().tolist(), max_radii2D=scene.max_radii2D.cpu(),
-                max_radii2D_at_densify=[r.cpu() for r in radii_trace])
+    out = dict(steps=steps, total_ms=total_ms, render_ms=render_ms, render_fraction=render_ms / total_ms,
+               ms_per_step=total_ms / steps, P_first=counts[0], P_last=counts[-1], final_loss=float(loss.detach()),
+               counts=counts, losses=torch.stack(losses).cpu().tolist(), max_radii2D=scene.max_radii2D.cpu(),
+               max_radii2D_at_densify=[r.cpu() for r in radii_trace])
+    if fixed:   # the step is not split by events: no render time
+        out.update(render_ms=None, render_fraction=None, capacities=loop.capacities)
+    return out
+
+
+class _FixedCapacityStep:
+    """One edit-loop step on the rasterizer's static-capacity forward, run eagerly or as a replayed CUDA graph.
+
+    The capacity is sized once per Gaussian count (`reset`). With `cuda_graph`, the first step after a reset runs eagerly
+    on a side stream (it creates Adam's state and warms every lazy initialisation), the second is captured, and every
+    step copies its camera and target into the captured input tensors and replays. Overflows are accumulated on the
+    device and read only by `check_capacity`."""
+
+    def __init__(self, GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph):
+        self.GR, self.scene, self.views, self.targets, self.pipe, self.bg = GR, scene, views, targets, pipe, bg
+        self.fused, self.opt, self.cuda_graph = fused_activations, opt, cuda_graph
+        dev = bg.device
+        self.overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+        v0 = views[0]
+        self.view = SimpleNamespace(**vars(v0))   # the captured camera: same intrinsics, pose tensors copied per step
+        self.view.world_view_transform = v0.world_view_transform.clone()
+        self.view.full_proj_transform = v0.full_proj_transform.clone()
+        self.view.camera_center = v0.camera_center.clone()
+        self.target = targets[0].clone()
+        self.capacities = []
+        self.reset()
+
+    def reset(self):
+        """New Gaussian count: size the capacity from an eager pass over all views, drop the captured graph."""
+        from .rasterizer import _RasterizeGaussians
+        r_max = 0
+        with torch.no_grad():
+            for v in self.views:
+                self.GR.render(v, self.scene, self.pipe, self.bg)
+                r_max = max(r_max, int(_RasterizeGaussians.last_state.num_rendered))
+        self.capacity = int(r_max * 1.25) + 4096
+        self.capacities.append(self.capacity)
+        self.graph = self.captured = None
+        self.warm = False
+
+    def _body(self, view, target):
+        GR, scene = self.GR, self.scene
+        pkg = GR.render(view, scene, self.pipe, self.bg, fused_activations=self.fused, static_capacity=self.capacity,
+                        **self.opt)                                                                   # forward #1
+        sem_pkg = GR.render(view, scene, self.pipe, self.bg, override_color=scene.mask[..., None].float().repeat(1, 3),
+                            static_capacity=self.capacity, **self.opt)                                 # forward #2
+        semantic = torch.norm(sem_pkg["render"], dim=0) > 0.8
+        loss = 10.0 * (pkg["render"] - target).abs().mean() + 0.0 * semantic.float().mean()
+        scene.optimizer.zero_grad(set_to_none=True)
+        loss.backward()
+        with torch.no_grad():
+            vis = pkg["visibility_filter"]
+            scene.max_radii2D.copy_(torch.where(vis, torch.maximum(scene.max_radii2D, pkg["radii"].float()),
+                                                scene.max_radii2D))
+            scene.add_densification_stats_dense(pkg["viewspace_points"].grad, vis)
+            torch.maximum(self.overflow, pkg["status"][1:], out=self.overflow)
+            torch.maximum(self.overflow, sem_pkg["status"][1:], out=self.overflow)
+        scene.optimizer.step()
+        return loss.detach()
+
+    def step(self, k):
+        if not self.cuda_graph:
+            return self._body(self.views[k], self.targets[k])
+        if not self.warm:   # eager first step of this Gaussian count, on a side stream as torch.cuda.graph wants
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                loss = self._body(self.views[k], self.targets[k])
+            torch.cuda.current_stream().wait_stream(side)
+            self.warm = True
+            return loss
+        v = self.views[k]
+        self.view.world_view_transform.copy_(v.world_view_transform)
+        self.view.full_proj_transform.copy_(v.full_proj_transform)
+        self.view.camera_center.copy_(v.camera_center)
+        self.target.copy_(self.targets[k])
+        if self.graph is None:
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph):
+                self.captured = self._body(self.view, self.target)
+        self.graph.replay()
+        return self.captured.clone()
+
+    def check_capacity(self):
+        """Synchronises: raises RuntimeError if any forward since the start exceeded its static capacity."""
+        if int(self.overflow.item()):
+            raise RuntimeError(f"a forward exceeded the static capacity {self.capacity}: its frame was rendered empty")

@@ -63,7 +63,7 @@ def _python_sh_colors(pc, camera_center) -> torch.Tensor:
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           fused_activations: bool = False, depth_grad: bool = False, deterministic=None):
+           fused_activations: bool = False, depth_grad: bool = False, deterministic=None, static_capacity=None):
     """Render the scene; background tensor must be on the GPU. Returns the reference's dictionary:
     render [3,H,W], viewspace_points [P,3] (grad sink for densification), visibility_filter, radii, depth_3dgs.
 
@@ -79,7 +79,12 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     ``deterministic`` (opt-in, not in the reference): ``True`` / ``False`` selects the rasterizer's bit-reproducible /
     default backward; ``None`` (default) leaves the choice to the rasterizer, which follows
-    ``torch.are_deterministic_algorithms_enabled()``."""
+    ``torch.are_deterministic_algorithms_enabled()``.
+
+    ``static_capacity`` (opt-in, not in the reference; an int): the rasterizer's fixed-capacity forward
+    (``GaussianRasterizer(static_capacity=...)``), which never waits for the GPU, so the step can be captured in a CUDA
+    graph. The result dictionary then also holds ``status``, the rasterizer's device int32[2]
+    ``{num_rendered, num_rendered > static_capacity}``; a frame over the capacity is rendered empty."""
     xyz = pc.get_xyz
     # gradient sink for the 2-D means: densification reads its .grad (gaussian_renderer/__init__.py:60-69)
     screenspace_points = torch.zeros_like(xyz, requires_grad=True) + 0
@@ -92,6 +97,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     opt = {"depth_grad": True} if depth_grad else {}
     if deterministic is not None:
         opt["deterministic"] = bool(deterministic)
+    if static_capacity is not None:
+        opt["static_capacity"] = static_capacity
     rasterizer = GaussianRasterizer(
         raster_settings=_settings_for(viewpoint_camera, bg_color, scaling_modifier, pc.active_sh_degree), **opt)
     python_sh = getattr(pipe, "convert_SHs_python", False)
@@ -116,5 +123,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         else:
             kw["shs"] = pc.get_features.float()
         image, radii, depth = rasterizer(**kw)
-    return {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
-            "depth_3dgs": depth}
+    out = {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
+           "depth_3dgs": depth}
+    if static_capacity is not None:
+        out["status"] = rasterizer.status
+    return out

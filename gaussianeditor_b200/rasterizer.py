@@ -7,7 +7,8 @@ Same public names, argument meaning, return values and error messages as
 
 Differences a caller can observe (all documented in DESIGN.md):
   * kernels run on PyTorch's CURRENT stream (the reference always used the legacy default stream);
-  * the only host synchronisation per forward is one stream sync to read ``num_rendered``;
+  * the only host synchronisation per forward is one stream sync to read ``num_rendered``, and none at all with
+    ``static_capacity`` (the forward then only enqueues work, so a whole training step can be captured in a CUDA graph);
   * gradient tensors are written completely by the kernels (no separate zero-fill passes);
   * ``debug=True`` synchronises after every launch and raises on the first CUDA error, but does not write the
     reference's ``snapshot_*.dump`` files.
@@ -119,9 +120,11 @@ class _ForwardState:
 
 
 def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, *, render=True,
-                  raw_rest=None):
+                  raw_rest=None, static=None):
     """Both forward halves. With ``raw_rest`` (features_rest [P,K,3]) the call is the fused-activation variant:
-    ``sh`` is features_dc [P,1,3] and opacities / scales / rotations are the raw parameters."""
+    ``sh`` is features_dc [P,1,3] and opacities / scales / rotations are the raw parameters.
+    With ``static = (capacity, status)`` both halves run in one gsr_forward_static call sized for ``capacity``: no
+    pinned word, no host wait; num_rendered and the overflow flag land in the device tensor ``status`` int32[2]."""
     lib = _lib.load()
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:46-48
@@ -152,6 +155,12 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
         state.radii = torch.empty(P, dtype=torch.int32, device=device)
         gbytes = _geometry_bytes(lib, P) if P > 0 else 0
         state.geom = torch.empty(gbytes, **u8)
+        if static is not None:
+            cap, status = static
+            color, depth = _forward_static(lib, s, c, P, W, H, cap, status, gbytes, state, st, device,
+                                           raw_rest if raw else None)
+            inputs = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+            return color, depth, state, inputs + ((raw_rest,) if raw else ())
         pinned = _pinned_i32(device)
         pinned[0] = -1
         if raw:
@@ -208,9 +217,38 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
     return color, depth, state, inputs
 
 
+def _forward_static(lib, s, c, P, W, H, cap, status, gbytes, state, st, device, raw_rest):
+    """Second half of _forward_impl on the static-capacity path (gsr_forward_static / gsr_forward_static_raw).
+    Returns (colour, depth); the state keeps no reference to them (the autograd node holds the state)."""
+    u8 = dict(dtype=torch.uint8, device=device)
+    bbytes = lib.gsr_binning_bytes(P, cap, W, H)
+    if bbytes == 0:
+        _lib.check(-2, "gsr_binning_bytes")
+    state.binning = torch.empty(bbytes, **u8)
+    ibytes = lib.gsr_image_bytes(W, H)
+    state.img = torch.empty(ibytes, **u8)
+    color = torch.empty(3, H, W, dtype=torch.float32, device=device)
+    depth = torch.empty(1, H, W, dtype=torch.float32, device=device)
+    state.num_rendered, state.cap = None, cap   # R is on the device only (status[0])
+    args = (cap, _ptr(state.geom), gbytes, _ptr(state.binning), bbytes, _ptr(state.img), ibytes, _ptr(state.radii),
+            _ptr(color), _ptr(depth), C.c_void_p(status.data_ptr()), st)
+    if raw_rest is not None:
+        rc = _lib.RawCloud(P, c.means3D, c.opacities, c.shs, _ptr(raw_rest), c.scales, c.rotations)
+        _lib.check(lib.gsr_forward_static_raw(C.byref(s), C.byref(rc), *args), "gsr_forward_static_raw")
+    else:
+        _lib.check(lib.gsr_forward_static(C.byref(s), C.byref(c), *args), "gsr_forward_static")
+    return color, depth
+
+
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, return_alpha=False, camera_grad=False, depth_grad=False, deterministic=False):
+                        raster_settings, return_alpha=False, camera_grad=False, depth_grad=False, deterministic=False,
+                        static=None):
     rs = raster_settings
+    if static is not None:   # (capacity, status): gsr_forward_static; always the long argument form
+        cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if camera_grad else (None, None, None)
+        return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                         cov3Ds_precomp, rs, return_alpha, *cam, bool(depth_grad), bool(deterministic),
+                                         static)
     if depth_grad or deterministic:
         # depth_grad: the depth output's gradient is used (gsr_backward_depth); without it, it is dropped as in the
         # reference. deterministic: bit-reproducible backward (gsr_backward_deterministic).
@@ -238,9 +276,10 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, return_alpha=False, viewmatrix=None, projmatrix=None, campos=None, depth_grad=False,
-                deterministic=None):
+                deterministic=None, static=None):
         color, depth, state, inputs = _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations,
-                                                    cov3Ds_precomp, raster_settings)
+                                                    cov3Ds_precomp, raster_settings, static=static)
+        ctx.static_form = static is not None
         ctx.raster_settings = raster_settings
         ctx.camera_grad = viewmatrix is not None
         ctx.depth_grad = bool(depth_grad)
@@ -357,6 +396,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads = grads + cam_grads
         if ctx.long_form:   # depth_grad, deterministic
             grads = grads + ((None, None, None) if not ctx.camera_grad else ()) + (None, None)
+        if ctx.static_form:
+            grads = grads + (None,)
         return grads
 
 
@@ -366,10 +407,12 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
-                raster_settings, depth_grad=False, deterministic=None):
+                raster_settings, depth_grad=False, deterministic=None, static=None):
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         color, depth, state, inputs = _forward_impl(means3D, features_dc, empty, opacity_logits, log_scales,
-                                                    raw_rotations, empty, raster_settings, raw_rest=features_rest)
+                                                    raw_rotations, empty, raster_settings, raw_rest=features_rest,
+                                                    static=static)
+        ctx.static_form = static is not None
         ctx.raster_settings = raster_settings
         ctx.state = state
         ctx.depth_grad = bool(depth_grad)
@@ -427,6 +470,8 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                                                     _ptr(binning), binning.numel(), _ptr(img), img.numel(), _ptr(radii),
                                                     _ptr(grad_out_color), _ptr(scratch), sbytes, C.byref(gr), st),
                                "gsr_backward_raw")
+        if ctx.static_form:   # depth_grad, deterministic, static
+            return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None, None
         if ctx.long_form:   # depth_grad, deterministic
             return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None
         if ctx.depth_grad:
@@ -454,7 +499,7 @@ def mark_visible(rs, positions):
 
 class GaussianRasterizer(nn.Module):
     def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False,
-                 deterministic=None):
+                 deterministic=None, static_capacity=None):
         """``return_alpha=True`` (opt-in, not in the reference) appends a fourth output to ``forward``: the alpha image
         ``1 - final_T`` [1,H,W] (the reference keeps final_T as ``accum_alpha`` but never returns it); it is
         differentiable like the colour.
@@ -469,13 +514,50 @@ class GaussianRasterizer(nn.Module):
         same bits; ``False`` keeps the faster default. ``None`` (default) follows
         ``torch.are_deterministic_algorithms_enabled()`` at the time of the call, so ``torch.use_deterministic_algorithms
         (True)`` (Lightning's ``trainer.deterministic=true``) selects it without other changes. Forward outputs are the
-        same in both modes."""
+        same in both modes.
+        ``static_capacity`` (opt-in, for ``forward`` and ``forward_raw``; an int > 0): the forward is sized for at most
+        that many (Gaussian, tile) instances and never reads the count on the host: it only enqueues work, without a
+        host synchronisation or a pinned allocation, so the call (and its backward) can be captured with
+        ``torch.cuda.graph`` and the host can run ahead of the GPU. Each call writes ``self.status``, a device int32[2]
+        tensor ``{num_rendered, num_rendered > static_capacity}``. When the capacity is too small the frame is EMPTY:
+        colour = background, depth = 0, alpha = 0 and all gradients zero. Nothing checks this implicitly: call
+        ``check_capacity()`` (it synchronises) where a synchronisation is acceptable. Outputs and radii are the same as
+        without the option while the capacity suffices; ``apply_weights`` keeps its exact, host-sized path. Not
+        combinable with ``raster_settings.debug`` (which synchronises after every launch)."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_alpha = bool(return_alpha)
         self.camera_grad = bool(camera_grad)
         self.depth_grad = bool(depth_grad)
         self.deterministic = None if deterministic is None else bool(deterministic)
+        if static_capacity is not None:
+            if isinstance(static_capacity, bool) or int(static_capacity) != static_capacity or not (
+                    0 < int(static_capacity) < 2 ** 31):
+                raise ValueError(f"static_capacity must be an int in [1, 2^31), got {static_capacity!r}")
+            static_capacity = int(static_capacity)
+        self.static_capacity = static_capacity
+        self.status = None   # device int32[2] {num_rendered, overflow} of the last static-capacity call
+
+    def _static(self, device):
+        """(capacity, status) for a static-capacity call, or None. Raises before any launch on a debug setting."""
+        if self.static_capacity is None:
+            return None
+        if self.raster_settings.debug:
+            raise ValueError("static_capacity cannot be combined with debug=True: debug synchronises after every launch")
+        if self.status is None or self.status.device != device:
+            self.status = torch.zeros(2, dtype=torch.int32, device=device)
+        return self.static_capacity, self.status
+
+    def check_capacity(self):
+        """Synchronise with the last static-capacity call and raise RuntimeError if its instance count exceeded
+        ``static_capacity`` (that frame was rendered empty). Returns num_rendered otherwise."""
+        if self.static_capacity is None or self.status is None:
+            raise RuntimeError("check_capacity() needs a static_capacity rasterizer that has run a forward")
+        R, over = (int(v) for v in self.status.cpu())
+        if over:
+            raise RuntimeError(f"num_rendered R={R} exceeds static_capacity={self.static_capacity}: the frame was "
+                               f"rendered empty; raise the capacity to at least {R}")
+        return R
 
     def _deterministic(self) -> bool:
         if self.deterministic is None:
@@ -487,6 +569,10 @@ class GaussianRasterizer(nn.Module):
         parameters (``_xyz, _opacity, _features_dc, _features_rest, _scaling, _rotation``); sigmoid / exp / normalize
         and the SH concatenation happen inside the preprocess kernels. Same return tuple as ``forward``."""
         det = self._deterministic()
+        static = self._static(means3D.device)
+        if static is not None:
+            return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
+                                                raw_rotations, self.raster_settings, self.depth_grad, det, static)
         if self.depth_grad or det:
             return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
                                                 raw_rotations, self.raster_settings, self.depth_grad, det)
@@ -508,6 +594,7 @@ class GaussianRasterizer(nn.Module):
         ):
             raise Exception("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!")
 
+        static = self._static(means3D.device)
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         if shs is None:
             shs = empty
@@ -522,7 +609,7 @@ class GaussianRasterizer(nn.Module):
 
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                    cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad, self.depth_grad,
-                                   self._deterministic())
+                                   self._deterministic(), static)
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):

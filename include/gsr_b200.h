@@ -132,6 +132,22 @@ GSR_API int gsr_forward_render_speculative(const gsr_settings* s, const gsr_clou
                        size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
                        const int32_t* radii, float* out_color, float* out_depth, void* stream);
 
+/* ---- forward, both halves, for a fixed capacity: no host copy, no host wait ---------------------------------------
+ * gsr_forward_preprocess + gsr_forward_render_speculative in one call, without the copy of num_rendered to the host:
+ * the call only enqueues work on `stream`, so it can be captured in a CUDA graph and the host can run ahead of the
+ * GPU. The workspaces are sized for `capacity` (gsr_geometry_bytes(P), gsr_binning_bytes(P, capacity, W, H),
+ * gsr_image_bytes(W, H)). A kernel on the stream writes status[0] = num_rendered and status[1] = (num_rendered >
+ * capacity) into the caller's DEVICE buffer `status` (int32[2]).
+ * When num_rendered > capacity the frame is empty, on every binning path: out_color = background, out_depth = 0, the
+ * alpha image (gsr_alpha_image) = 0, and every backward called with `capacity` as its num_rendered returns zero
+ * gradients. The caller reads `status` whenever it chooses to synchronise, and re-sizes.
+ * P == 0 writes {0, 0} and zero images. Every argument (capacity > 0, status, outputs, workspace sizes) is checked
+ * before the first launch. The backward entry points take `capacity` as their num_rendered argument.
+ * gsr_forward_static_raw is the fused-activation form (gsr_raw_cloud, as gsr_forward_preprocess_raw). */
+GSR_API int gsr_forward_static(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
+                       size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                       int32_t* radii, float* out_color, float* out_depth, int32_t* status, void* stream);
+
 /* ---- backward ------------------------------------------------------------------------------------------
  * dL_dout_color [3,H,W]; the three workspaces and `radii` are the ones the forward produced. */
 GSR_API int gsr_backward(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered, const void* geometry,
@@ -294,6 +310,10 @@ typedef struct gsr_raw_grads {
 } gsr_raw_grads;
 GSR_API int gsr_forward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* c, void* geometry,
                                size_t geometry_bytes, int32_t* radii, int32_t* num_rendered_host, void* stream);
+/* gsr_forward_static on the raw parameters (see gsr_forward_static) */
+GSR_API int gsr_forward_static_raw(const gsr_settings* s, const gsr_raw_cloud* c, int32_t capacity, void* geometry,
+                           size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                           int32_t* radii, float* out_color, float* out_depth, int32_t* status, void* stream);
 GSR_API int gsr_backward_raw(const gsr_settings* s, const gsr_raw_cloud* c, int32_t num_rendered, const void* geometry,
                      size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                      size_t image_bytes, const int32_t* radii, const float* dL_dout_color, void* scratch,

@@ -149,5 +149,20 @@ for st, a in zip(steps, accs):
     SS.sparse_return(st, a)
 for st in steps:
     SS.apply_weights_gather(st, torch.zeros(st.n, 3, device=dev), torch.zeros(st.n, 1, dtype=torch.int32, device=dev))
+
+# static-capacity forward (gsr_forward_static) on both binning paths: capacity R (fits) and R/2 (overflow: empty frame,
+# zero gradients), default and deterministic backward, plain and raw inputs
+R_exact = run_ours(cloud, cam, (0.1, 0.2, 0.3))["R"]
+for bvar in (1, 0):
+    _lib.set_option("binning_variant", bvar)
+    for cap, det in ((R_exact, False), (R_exact // 2, False), (R_exact // 2, True)):
+        sr = GaussianRasterizer(rs, deterministic=det, static_capacity=cap, depth_grad=True)
+        ctg = cloud_tensors(cloud, dev, requires_grad=True)
+        col, _, dep = sr(means3D=ctg["means3D"], means2D=torch.zeros_like(ctg["means3D"]), opacities=ctg["opacities"],
+                         shs=ctg["shs"], scales=ctg["scales"], rotations=ctg["rotations"])
+        ((col * torch.from_numpy(dL).to(dev)).sum() + dep.sum()).backward()
+        col, _, dep = sr.forward_raw(*raw)
+        (col * torch.from_numpy(dL).to(dev)).sum().backward()
+_lib.set_option("binning_variant", 1)
 torch.cuda.synchronize()
 print("SANITIZE_CASE_DONE")
