@@ -39,6 +39,8 @@ SYMBOLS = [
     "gsr_shard_alpha_image", "gsr_shard_backward_render_alpha", "gsr_shard_backward_preprocess_camera",
     "gsr_sparse_backward_preprocess_camera", "gsr_frame_broadcast_planes", "gsr_peer_row_put",
     "gsr_forward_static", "gsr_forward_static_raw",
+    "gsr_shard_order_static", "gsr_sparse_order_static", "gsr_shard_render_static", "gsr_shard_static_gate",
+    "gsr_peer_barrier_device",
 ]
 
 
@@ -279,6 +281,16 @@ def load():
     lib.gsr_frame_broadcast_planes.argtypes = [TO, i32, i32, i32, vp, C.POINTER(vp), vp]
     lib.gsr_peer_row_put.restype = C.c_int
     lib.gsr_peer_row_put.argtypes = [i32, i32, vp, i32, C.POINTER(vp), vp]
+    lib.gsr_shard_order_static.restype = C.c_int
+    lib.gsr_shard_order_static.argtypes = [S, TO, i32, vp, sz, vp, vp]
+    lib.gsr_sparse_order_static.restype = C.c_int
+    lib.gsr_sparse_order_static.argtypes = [S, SP, vp, sz, vp, vp, vp]
+    lib.gsr_shard_render_static.restype = C.c_int
+    lib.gsr_shard_render_static.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, i32, i32, vp]
+    lib.gsr_shard_static_gate.restype = C.c_int
+    lib.gsr_shard_static_gate.argtypes = [S, i32, vp, sz, vp, sz, vp, i32, vp, vp, vp, i32, vp, vp]
+    lib.gsr_peer_barrier_device.restype = C.c_int
+    lib.gsr_peer_barrier_device.argtypes = [i32, i32, C.POINTER(vp), i32, vp, vp]
     if lib.gsr_abi_version() != 2:
         raise RuntimeError("libgsr_b200.so ABI version mismatch")
     _lib = lib

@@ -739,14 +739,15 @@ int gsr_shard_preprocess_p2p_raw(const gsr_settings* s, const gsr_raw_cloud* sha
                                    geometry_bytes, radii_total, stream);
 }
 
-int gsr_shard_order(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, void* geometry,
-                    size_t geometry_bytes, int32_t* radii_total, int32_t* num_rendered_host, void* stream) {
+// gsr_shard_order and, with num_rendered_host == nullptr, gsr_shard_order_static (R stays on the device)
+static int shard_order_impl(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, void* geometry,
+                            size_t geometry_bytes, int32_t* radii_total, int32_t* num_rendered_host, void* stream) {
   int rc = check_settings(s);
   if (rc) return rc;
   TileOwner own;
   rc = check_owner(owner, own);
   if (rc) return rc;
-  if (P_total <= 0 || !geometry || !radii_total || !num_rendered_host) { set_error("shard_order: bad arguments"); return GSR_ERR_INVALID; }
+  if (P_total <= 0 || !geometry || !radii_total) { set_error("shard_order: bad arguments"); return GSR_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   GeometryWS g;
   if (!carve_geometry(geometry, P_total, g)) return GSR_ERR_CUDA;
@@ -759,10 +760,84 @@ int gsr_shard_order(const gsr_settings* s, const gsr_tile_owner* owner, int32_t 
   const bool v2 = tile_binning_supported((s->image_width + TILE - 1) / TILE, (s->image_height + TILE - 1) / TILE);
   if (v2) {
     if ((rc = launch_tile_count(g, (s->image_width + TILE - 1) / TILE, (s->image_height + TILE - 1) / TILE, own, st))) return rc;
-    cudaError_t e = cudaMemcpyAsync(num_rendered_host, g.R_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) return check_cuda(e, "num_rendered readback");
+    if (num_rendered_host) {
+      cudaError_t e = cudaMemcpyAsync(num_rendered_host, g.R_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
+      if (e != cudaSuccess) return check_cuda(e, "num_rendered readback");
+    }
   }
   return run_depth_order_and_scan(c, g, v2 ? nullptr : num_rendered_host, st, s->debug != 0);
+}
+
+int gsr_shard_order(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, void* geometry,
+                    size_t geometry_bytes, int32_t* radii_total, int32_t* num_rendered_host, void* stream) {
+  if (!num_rendered_host) { set_error("shard_order: bad arguments"); return GSR_ERR_INVALID; }
+  return shard_order_impl(s, owner, P_total, geometry, geometry_bytes, radii_total, num_rendered_host, stream);
+}
+
+int gsr_shard_order_static(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, void* geometry,
+                           size_t geometry_bytes, int32_t* radii_total, void* stream) {
+  return shard_order_impl(s, owner, P_total, geometry, geometry_bytes, radii_total, nullptr, stream);
+}
+
+// The binning and blending of the owned tiles for a fixed capacity: the speculative binning reads R on the device, and
+// launch_shard_static_status reports it and empties the owned tiles on an R or segment overflow. With the sparse
+// exchange (counts_matrix != null) a truncated segment stays memory-safe: sparse_push_kernel drops the records past
+// seg_cap, and retouch_sparse_kernel, sparse_return_kernel and sparse_gather_kernel clamp every segment to seg_cap.
+int gsr_shard_render_static(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t capacity,
+                            void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                            size_t image_bytes, const int32_t* radii_total, float* out_color, float* out_depth,
+                            int32_t* status, const int32_t* counts_matrix, int32_t world, int32_t seg_cap,
+                            void* stream) {
+  int rc = check_settings(s);
+  if (rc) return rc;
+  TileOwner own;
+  rc = check_owner(owner, own);
+  if (rc) return rc;
+  if (capacity <= 0) { set_error("static capacity must be positive"); return GSR_ERR_INVALID; }
+  if (!status) { set_error("status is null"); return GSR_ERR_INVALID; }
+  if (P_total <= 0 || !out_color || !out_depth || !radii_total) { set_error("shard_render_static: bad arguments"); return GSR_ERR_INVALID; }
+  if (counts_matrix) {
+    if (world < 1 || world > GSR_MAX_PEERS || seg_cap < 1 || (int64_t)world * seg_cap != P_total) {
+      set_error("shard_render_static: need 1 <= world <= %d and world*seg_cap == P_total (%d x %d vs %d)", GSR_MAX_PEERS,
+                world, seg_cap, P_total);
+      return GSR_ERR_INVALID;
+    }
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  gsr_cloud c{};
+  c.P = P_total;
+  GeometryWS g; BinningWS b; ImageWS im;
+  rc = carve_all(s, &c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, g, b, im);
+  if (rc) return rc;
+  rc = run_binning(*s, c, capacity, true, g, b, im, radii_total, st, own);
+  if (rc) return rc;
+  rc = launch_shard_static_status(*s, P_total, (uint32_t)capacity, g, im, counts_matrix, counts_matrix ? world : 0,
+                                  counts_matrix ? seg_cap : 0, status, st);
+  if (rc) return rc;
+  StageScope t(ST_RENDER_FWD, st);
+  return launch_render_fwd(*s, g, b, im, out_color, out_depth, st, own);
+}
+
+int gsr_shard_static_gate(const gsr_settings* s, int32_t P_total, void* geometry, size_t geometry_bytes, void* image,
+                          size_t image_bytes, const int32_t* flags, int32_t num_flags, const float* flag_sum,
+                          const int32_t* error_word, float* frame, int32_t planes, int32_t* status, void* stream) {
+  int rc = check_settings(s);
+  if (rc) return rc;
+  if (!status || !frame || !geometry || !image || P_total <= 0) { set_error("shard_static_gate: bad arguments"); return GSR_ERR_INVALID; }
+  if ((flags == nullptr) == (flag_sum == nullptr) || (flags && (num_flags < 1 || num_flags > GSR_MAX_PEERS))) {
+    set_error("shard_static_gate: need exactly one of flags [1..%d] and flag_sum", GSR_MAX_PEERS);
+    return GSR_ERR_INVALID;
+  }
+  if (planes < 4 || planes > GSR_FRAME_MAX_PLANES) { set_error("shard_static_gate: planes = %d outside 4..%d", planes, GSR_FRAME_MAX_PLANES); return GSR_ERR_INVALID; }
+  ImageWS im;
+  carve_image(image, s->image_width, s->image_height, im);
+  if (im.total > image_bytes) { set_error("image workspace too small: %zu < %zu", image_bytes, im.total); return GSR_ERR_WORKSPACE; }
+  GeometryWS g;
+  if (!carve_geometry(geometry, P_total, g)) return GSR_ERR_CUDA;
+  if (g.total > geometry_bytes) { set_error("geometry workspace too small: %zu < %zu", geometry_bytes, g.total); return GSR_ERR_WORKSPACE; }
+  return launch_shard_static_gate(*s, P_total, g, im, flags, flags ? num_flags : 0, flag_sum,
+                                  reinterpret_cast<const uint32_t*>(error_word), frame, planes, status,
+                                  (cudaStream_t)stream);
 }
 
 int gsr_shard_render(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R, void* geometry,

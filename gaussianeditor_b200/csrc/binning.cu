@@ -223,6 +223,68 @@ static_status_kernel(int P, int ntile, uint32_t cap, const uint32_t* __restrict_
   }
 }
 
+// Static-capacity sharded forward: static_status_kernel for one rank's owned tiles, plus (sparse exchange,
+// counts_matrix != null) the segment check: a segment of more than seg_cap records was truncated by the push, so this
+// rank's candidate lists are incomplete. The matrix is the same on every rank after the barrier that carried its rows,
+// so every rank finds a segment overflow alike; an R overflow is local and is made global by the gate below.
+// status = {R, overflow, largest segment (0 without a matrix), 0}; word 3 is the gate's.
+__global__ void __launch_bounds__(STATUS_THREADS)
+shard_static_status_kernel(int P, int ntile, uint32_t cap, const uint32_t* __restrict__ R_dev,
+                           const int32_t* __restrict__ counts_matrix, int world, int seg_cap, uint2* __restrict__ ranges,
+                           uint32_t* __restrict__ tiles_touched, int32_t* __restrict__ status) {
+  const uint32_t R = __ldg(R_dev);
+  int max_count = 0;
+  if (counts_matrix)
+    for (int k = 0; k < world * GSR_MAX_PEERS; k++) max_count = max(max_count, counts_matrix[k]);
+  const bool overflow = R > cap || max_count > seg_cap;
+  const int i0 = blockIdx.x * STATUS_THREADS + threadIdx.x;
+  if (i0 == 0) {
+    status[0] = (int32_t)R;
+    status[1] = overflow ? 1 : 0;
+    status[2] = max_count;
+    status[3] = 0;
+  }
+  if (!overflow) return;
+  for (int i = i0; i < max(P, ntile); i += gridDim.x * STATUS_THREADS) {
+    if (i < ntile) ranges[i] = make_uint2(0u, 0u);
+    if (i < P) tiles_touched[i] = 0u;
+  }
+}
+
+// The overflow consensus of the static sharded forward, after the frame exchange: `flags` [nflags] (the ranks' overflow
+// words, delivered through the frame barrier) or `flag_sum` (the exact float sum of the ranks' 0/1 flags that rode the
+// frame all-reduce). If any rank overflowed, every rank gets the same empty frame -- colour = background, depth and
+// alpha 0 -- and its owned tiles are emptied, so every backward writes zeros: zero ranges and tile counts, and zero
+// tile_last, where the blending backward starts its walk (the forward has already run on the full lists here).
+// status[1] = the global flag, status[3] = the barrier error word (0 without one).
+__global__ void __launch_bounds__(STATUS_THREADS)
+shard_static_gate_kernel(int P, int ntile, int npix, int planes, const int32_t* __restrict__ flags, int nflags,
+                         const float* __restrict__ flag_sum, const uint32_t* __restrict__ error_word,
+                         const float* __restrict__ bg, uint2* __restrict__ ranges, uint32_t* __restrict__ tile_last,
+                         uint32_t* __restrict__ tiles_touched, float* __restrict__ frame, int32_t* __restrict__ status) {
+  bool any = flag_sum != nullptr && *flag_sum != 0.f;
+  for (int r = 0; r < nflags; r++) any |= flags[r] != 0;
+  const int i0 = blockIdx.x * STATUS_THREADS + threadIdx.x;
+  if (i0 == 0) {
+    status[1] = any ? 1 : 0;
+    status[3] = error_word ? (int32_t)*error_word : 0;
+  }
+  if (!any) return;
+  const long long nframe = (long long)npix * planes;
+  const long long n = max((long long)max(P, ntile), nframe);
+  for (long long i = i0; i < n; i += (long long)gridDim.x * STATUS_THREADS) {
+    if (i < ntile) {
+      ranges[i] = make_uint2(0u, 0u);
+      tile_last[i] = 0u;
+    }
+    if (i < P) tiles_touched[i] = 0u;
+    if (i < nframe) {
+      const int plane = (int)(i / npix);
+      frame[i] = plane < 3 ? __ldg(bg + plane) : 0.f;
+    }
+  }
+}
+
 // CUB's temp-size queries depend only on the item count but cost several runtime calls each; every C-ABI entry point
 // re-derives the workspace layout, so they are memoised (single-threaded callers per the ABI; a mutex keeps it safe).
 struct SizeCache {
@@ -439,6 +501,32 @@ int launch_static_status(const gsr_settings& s, int P, uint32_t capacity, const 
   static_status_kernel<<<blocks, STATUS_THREADS, 0, st>>>(P, gx * gy, capacity, R_dev, im.ranges, g.tiles_touched, status);
   g_launches++;
   return check_launch("static_status", s.debug != 0, st);
+}
+
+int launch_shard_static_status(const gsr_settings& s, int P, uint32_t capacity, const GeometryWS& g, const ImageWS& im,
+                               const int32_t* counts_matrix, int world, int seg_cap, int32_t* status, cudaStream_t st) {
+  const int gx = (s.image_width + TILE - 1) / TILE, gy = (s.image_height + TILE - 1) / TILE;
+  const uint32_t* R_dev = tile_binning_supported(gx, gy) ? g.R_dev : g.offsets + (P - 1);  // as launch_static_status
+  const int n = P > gx * gy ? P : gx * gy;
+  const int blocks = std::min((n + STATUS_THREADS - 1) / STATUS_THREADS, 1024);
+  shard_static_status_kernel<<<blocks, STATUS_THREADS, 0, st>>>(P, gx * gy, capacity, R_dev, counts_matrix, world,
+                                                                seg_cap, im.ranges, g.tiles_touched, status);
+  g_launches++;
+  return check_launch("shard_static_status", s.debug != 0, st);
+}
+
+int launch_shard_static_gate(const gsr_settings& s, int P, const GeometryWS& g, const ImageWS& im, const int32_t* flags,
+                             int nflags, const float* flag_sum, const uint32_t* error_word, float* frame, int planes,
+                             int32_t* status, cudaStream_t st) {
+  const int gx = (s.image_width + TILE - 1) / TILE, gy = (s.image_height + TILE - 1) / TILE;
+  const long long npix = (long long)s.image_width * s.image_height;
+  const long long n = std::max<long long>(std::max(P, gx * gy), npix * planes);
+  const int blocks = (int)std::min<long long>((n + STATUS_THREADS - 1) / STATUS_THREADS, 1024);
+  shard_static_gate_kernel<<<blocks, STATUS_THREADS, 0, st>>>(P, gx * gy, (int)npix, planes, flags, nflags, flag_sum,
+                                                              error_word, s.bg, im.ranges, im.tile_last, g.tiles_touched, frame,
+                                                              status);
+  g_launches++;
+  return check_launch("shard_static_gate", s.debug != 0, st);
 }
 
 int launch_retouch(const gsr_settings& s, int P, const GeometryWS& g, int32_t* radii, const TileOwner& own,

@@ -189,6 +189,16 @@ int run_binning(const gsr_settings& s, const gsr_cloud& c, int R, bool speculati
 // from the device count; on overflow every tile range and every per-Gaussian tile count is zeroed (an empty frame).
 int launch_static_status(const gsr_settings& s, int P, uint32_t capacity, const GeometryWS& g, const ImageWS& im,
                          int32_t* status, cudaStream_t st);
+// Static-capacity sharded forward: status[0..3] = {R, overflow, largest segment, 0}, where overflow also counts a segment
+// of counts_matrix [world, GSR_MAX_PEERS] (sparse exchange; null in the dense one) above seg_cap; the owned tiles are
+// emptied on overflow as above.
+int launch_shard_static_status(const gsr_settings& s, int P, uint32_t capacity, const GeometryWS& g, const ImageWS& im,
+                               const int32_t* counts_matrix, int world, int seg_cap, int32_t* status, cudaStream_t st);
+// After the frame exchange: if flags[0..nflags) or *flag_sum has a non-zero entry, frame [planes,H,W] = background /
+// zeros and the owned tiles are emptied; status[1] = that global flag, status[3] = *error_word (or 0).
+int launch_shard_static_gate(const gsr_settings& s, int P, const GeometryWS& g, const ImageWS& im, const int32_t* flags,
+                             int nflags, const float* flag_sum, const uint32_t* error_word, float* frame, int planes,
+                             int32_t* status, cudaStream_t st);
 // tile_binning.cu: ranges from the tile-count difference array, emission fused into the first of two own radix passes
 constexpr int SORT_TILE = 4096;  // instances per CTA of a radix pass
 bool tile_binning_supported(int gx, int gy);

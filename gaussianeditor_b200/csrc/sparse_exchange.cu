@@ -432,14 +432,22 @@ __global__ void peer_row_put_kernel(const RowPutArgs a) {
 // ---- cross-rank barrier over peer memory ---------------------------------------------------------------------------
 // 512 bytes at the start of every rank's peer-visible block. flags[r] is written by rank r only (the number of the last
 // barrier it has reached); matrix row s is written by rank s only (n[s -> d], the segment sizes of the sparse exchange).
+// The device-epoch barrier (gsr_peer_barrier_device) adds two fields behind the matrix: `epoch`, the number of the last
+// device barrier this rank ran on the block (written by this rank's own barrier kernel only), and status[r], the
+// overflow word rank r sent with its last barrier.
 struct PeerCtrl {
   uint32_t flags[GSR_MAX_PEERS];
   uint32_t error;
   uint32_t pad[7];
   int32_t matrix[GSR_MAX_PEERS][GSR_MAX_PEERS];
+  uint32_t epoch;
+  uint32_t pad2[7];
+  int32_t status[GSR_MAX_PEERS];
 };
 static_assert(sizeof(PeerCtrl) <= GSR_PEER_CTRL_BYTES && offsetof(PeerCtrl, matrix) == GSR_PEER_CTRL_MATRIX_OFFSET &&
-                  offsetof(PeerCtrl, error) == GSR_PEER_CTRL_ERROR_OFFSET, "ctrl layout");
+                  offsetof(PeerCtrl, error) == GSR_PEER_CTRL_ERROR_OFFSET &&
+                  offsetof(PeerCtrl, epoch) == GSR_PEER_CTRL_EPOCH_OFFSET &&
+                  offsetof(PeerCtrl, status) == GSR_PEER_CTRL_STATUS_OFFSET, "ctrl layout");
 
 struct BarrierArgs {
   PeerCtrl* ctrl[GSR_MAX_PEERS];
@@ -467,6 +475,40 @@ __global__ void peer_barrier_kernel(const BarrierArgs a) {
       if (clock64() - t0 > a.timeout_clocks) { *(volatile uint32_t*)&a.ctrl[a.me]->error = 1u; break; }
     }
   }
+  __threadfence_system();
+}
+
+struct BarrierDeviceArgs {
+  PeerCtrl* ctrl[GSR_MAX_PEERS];
+  const int32_t* status_word;  // or null
+  int world, me, with_row;
+  long long timeout_clocks;
+};
+// peer_barrier_kernel with the epoch taken from the own block's counter instead of a kernel argument, so that a replayed
+// CUDA graph advances it: every lane reads the counter before lane 0 stores counter + 1 at the end, and the next barrier
+// on this block (a later kernel of the same stream) sees the new value. With `status_word` its value is stored into
+// status[me] of every block, own included, in front of the fence and the flag, as the matrix row is.
+__global__ void peer_barrier_device_kernel(const BarrierDeviceArgs a) {
+  const int r = threadIdx.x;
+  const uint32_t epoch = *(volatile uint32_t*)&a.ctrl[a.me]->epoch + 1u;
+  __syncwarp();
+  if (r < a.world) {
+    if (a.with_row && r != a.me) {
+#pragma unroll
+      for (int d = 0; d < GSR_MAX_PEERS; d++)
+        *(volatile int32_t*)&a.ctrl[r]->matrix[a.me][d] = *(volatile int32_t*)&a.ctrl[a.me]->matrix[a.me][d];
+    }
+    if (a.status_word) *(volatile int32_t*)&a.ctrl[r]->status[a.me] = *(volatile const int32_t*)a.status_word;
+    __threadfence_system();
+    *(volatile uint32_t*)&a.ctrl[r]->flags[a.me] = epoch;
+    volatile uint32_t* f = &a.ctrl[a.me]->flags[r];
+    const long long t0 = clock64();
+    while ((int32_t)(*f - epoch) < 0) {
+      if (clock64() - t0 > a.timeout_clocks) { *(volatile uint32_t*)&a.ctrl[a.me]->error = 1u; break; }
+    }
+  }
+  __syncwarp();
+  if (r == 0) *(volatile uint32_t*)&a.ctrl[a.me]->epoch = epoch;
   __threadfence_system();
 }
 
@@ -559,11 +601,13 @@ int gsr_sparse_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard,
                                 counts_row, stream);
 }
 
-int gsr_sparse_order(const gsr_settings* s, const gsr_sparse_plan* plan, void* cand_ws, size_t cand_bytes,
-                     const int32_t* counts_matrix, int32_t* radii_cand, int32_t* host_out, void* stream) {
+// gsr_sparse_order and, with host_out == nullptr, gsr_sparse_order_static (no host words: the static forward's status
+// kernel reads the matrix and R on the device)
+static int sparse_order_impl(const gsr_settings* s, const gsr_sparse_plan* plan, void* cand_ws, size_t cand_bytes,
+                             const int32_t* counts_matrix, int32_t* radii_cand, int32_t* host_out, void* stream) {
   int rc = check_plan(plan);
   if (rc) return rc;
-  if (!s || !cand_ws || !counts_matrix || !radii_cand || !host_out) { set_error("sparse_order: null argument"); return GSR_ERR_INVALID; }
+  if (!s || !cand_ws || !counts_matrix || !radii_cand) { set_error("sparse_order: null argument"); return GSR_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   SparseCand sc;
   if (!carve_sparse_cand(cand_ws, plan->world, plan->seg_cap, sc)) return GSR_ERR_CUDA;
@@ -576,22 +620,38 @@ int gsr_sparse_order(const gsr_settings* s, const gsr_sparse_plan* plan, void* c
   retouch_sparse_kernel<<<(M + 255) / 256, 256, 0, st>>>(plan->world, plan->seg_cap, plan->rank, counts_matrix, sc.g.records,
                                                          gx, gy, radii_cand, sc.g.tiles_touched, sc.g.ident, sc.g.depth_keys,
                                                          v2 ? sc.g.tile_diff : nullptr, tile_diff_copies(gx, gy));
-  // host_out[1] (largest segment anywhere) is copied out BEFORE host_out[0] (num_rendered): a host that polls word 0
-  // finds word 1 already in place. The device word is overwritten by the sort afterwards: read first.
-  int32_t* dev_word = reinterpret_cast<int32_t*>(sc.g.depth_keys_sorted);
-  sparse_max_count_kernel<<<1, 32, 0, st>>>(plan->world, counts_matrix, dev_word);
-  g_launches += 2;
-  cudaError_t e = cudaMemcpyAsync(host_out + 1, dev_word, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
-  if (e != cudaSuccess) return check_cuda(e, "max-count readback");
+  g_launches++;
+  if (host_out) {
+    // host_out[1] (largest segment anywhere) is copied out BEFORE host_out[0] (num_rendered): a host that polls word 0
+    // finds word 1 already in place. The device word is overwritten by the sort afterwards: read first.
+    int32_t* dev_word = reinterpret_cast<int32_t*>(sc.g.depth_keys_sorted);
+    sparse_max_count_kernel<<<1, 32, 0, st>>>(plan->world, counts_matrix, dev_word);
+    g_launches++;
+    cudaError_t e = cudaMemcpyAsync(host_out + 1, dev_word, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
+    if (e != cudaSuccess) return check_cuda(e, "max-count readback");
+  }
   if (v2) {
     TileOwner own; own.stride = plan->world; own.phase = plan->rank;
     if ((rc = launch_tile_count(sc.g, gx, gy, own, st))) return rc;
-    e = cudaMemcpyAsync(host_out, sc.g.R_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) return check_cuda(e, "num_rendered readback");
+    if (host_out) {
+      cudaError_t e = cudaMemcpyAsync(host_out, sc.g.R_dev, sizeof(int32_t), cudaMemcpyDeviceToHost, st);
+      if (e != cudaSuccess) return check_cuda(e, "num_rendered readback");
+    }
   }
   gsr_cloud c{};
   c.P = M;
   return run_depth_order_and_scan(c, sc.g, v2 ? nullptr : host_out, st, s->debug != 0);
+}
+
+int gsr_sparse_order(const gsr_settings* s, const gsr_sparse_plan* plan, void* cand_ws, size_t cand_bytes,
+                     const int32_t* counts_matrix, int32_t* radii_cand, int32_t* host_out, void* stream) {
+  if (!host_out) { set_error("sparse_order: null argument"); return GSR_ERR_INVALID; }
+  return sparse_order_impl(s, plan, cand_ws, cand_bytes, counts_matrix, radii_cand, host_out, stream);
+}
+
+int gsr_sparse_order_static(const gsr_settings* s, const gsr_sparse_plan* plan, void* cand_ws, size_t cand_bytes,
+                            const int32_t* counts_matrix, int32_t* radii_cand, void* stream) {
+  return sparse_order_impl(s, plan, cand_ws, cand_bytes, counts_matrix, radii_cand, nullptr, stream);
 }
 
 int gsr_sparse_return(const gsr_sparse_plan* plan, const void* acc_cand, const int32_t* counts_matrix,
@@ -758,6 +818,21 @@ int gsr_peer_barrier(int32_t world, int32_t rank, void* const* peer_ctrl, uint32
   peer_barrier_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
   g_launches++;
   return check_launch("peer_barrier", false, (cudaStream_t)stream);
+}
+
+int gsr_peer_barrier_device(int32_t world, int32_t rank, void* const* peer_ctrl, int32_t with_matrix_row,
+                            const int32_t* status_word, void* stream) {
+  if (world < 1 || world > GSR_MAX_PEERS || rank < 0 || rank >= world || !peer_ctrl) { set_error("peer_barrier_device: bad arguments"); return GSR_ERR_INVALID; }
+  BarrierDeviceArgs a;
+  for (int r = 0; r < GSR_MAX_PEERS; r++) a.ctrl[r] = r < world ? (PeerCtrl*)peer_ctrl[r] : nullptr;
+  for (int r = 0; r < world; r++)
+    if (!a.ctrl[r]) { set_error("peer_barrier_device: peer block %d is null", r); return GSR_ERR_INVALID; }
+  a.status_word = status_word;
+  a.world = world; a.me = rank; a.with_row = with_matrix_row;
+  a.timeout_clocks = 4000000000LL;  // ~2 s at 2 GHz, as gsr_peer_barrier
+  peer_barrier_device_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(a);
+  g_launches++;
+  return check_launch("peer_barrier_device", false, (cudaStream_t)stream);
 }
 
 int gsr_frame_broadcast_planes(const gsr_tile_owner* owner, int32_t W, int32_t H, int32_t planes, const float* frame,

@@ -444,6 +444,100 @@ def shard_alpha(buf: ShardBuffers, alpha: torch.Tensor):
                                              st), "gsr_shard_alpha_image")
 
 
+# ---- fixed-capacity (static) forward: no host copy, no host wait ---------------------------------------------------
+STATUS_WORDS = 4   # status = {R of this rank, overflow (any rank), largest segment (sparse), barrier error (sparse)}
+
+
+class StaticScratch:
+    """A StepWorkspace or SparseRank seen through its ``get`` with every scratch name prefixed ``static_``: the
+    fixed-capacity step keeps buffers of its own, so that an ``apply_weights`` (host-sized, grow-only scratch) can never
+    re-allocate a buffer a captured CUDA graph still points to. Every other attribute is the wrapped object's."""
+
+    def __init__(self, inner):
+        self.inner = inner
+
+    def get(self, name: str, numel: int, dtype, grow: float = 1.0) -> torch.Tensor:
+        return self.inner.get("static_" + name, numel, dtype, grow)
+
+    def __getattr__(self, name):
+        return getattr(self.inner, name)
+
+
+def shard_order_static(buf: ShardBuffers, capacity: int):
+    """shard_order without the readback (gsr_shard_order_static): R stays on the device, and ``buf.R = capacity`` sizes
+    the binning and every backward behind it."""
+    lib = _lib.load()
+    device = buf.geom.device
+    with torch.cuda.device(device):
+        st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(lib.gsr_shard_order_static(C.byref(buf.s), C.byref(buf.own), buf.plan.P_pad, _ptr(buf.geom),
+                                              buf.geom.numel(), _ptr(buf.radii), st), "gsr_shard_order_static")
+    buf.R = int(capacity)
+
+
+def render_static(s, own, P: int, capacity: int, geom: torch.Tensor, radii: torch.Tensor, color: torch.Tensor,
+                  depth: torch.Tensor, status: torch.Tensor, get, counts: Optional[torch.Tensor] = None, world: int = 0,
+                  seg_cap: int = 0):
+    """gsr_shard_render_static of a P-record workspace `geom` for `capacity` instances; returns (binning, img) from
+    `get(name, numel, dtype, grow)`. `counts` (the sparse count matrix, with `world` and `seg_cap`) adds the segment
+    check to ``status``."""
+    lib = _lib.load()
+    device = geom.device
+    W, H = int(s.image_width), int(s.image_height)
+    with torch.cuda.device(device):
+        bbytes = lib.gsr_binning_bytes(P, capacity, W, H)
+        binning = get("binning", bbytes, torch.uint8, 1.0)
+        ibytes = lib.gsr_image_bytes(W, H)
+        img = get("img", ibytes, torch.uint8, 1.0)
+        st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(lib.gsr_shard_render_static(C.byref(s), C.byref(own), P, capacity, _ptr(geom), geom.numel(),
+                                               _ptr(binning), bbytes, _ptr(img), ibytes, _ptr(radii), _ptr(color),
+                                               _ptr(depth), _ptr(status), _ptr(counts), world, seg_cap, st),
+                   "gsr_shard_render_static")
+    return binning, img
+
+
+def shard_render_static(buf: ShardBuffers, color: torch.Tensor, depth: torch.Tensor, status: torch.Tensor):
+    """shard_render for the capacity of shard_order_static: ``status`` (device int32[4]) gets {R, R > capacity, 0, 0}
+    and an overflowing rank's owned tiles are rendered empty."""
+    device = buf.geom.device
+    buf.binning, buf.img = render_static(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.radii, color, depth,
+                                         status, lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow))
+
+
+def static_gate(s, P: int, geom: torch.Tensor, img: torch.Tensor, frame: torch.Tensor, status: torch.Tensor,
+                flags: Optional[torch.Tensor] = None, flag_sum: Optional[torch.Tensor] = None,
+                error_word: Optional[torch.Tensor] = None):
+    """gsr_shard_static_gate: if any rank overflowed (`flags` int32 [world] or the all-reduced float `flag_sum` [1]),
+    `frame` [planes,H,W] becomes the empty frame and this rank's tiles are emptied, so every backward returns zeros.
+    status[1] = the global flag, status[3] = the barrier error word."""
+    lib = _lib.load()
+    device = geom.device
+    with torch.cuda.device(device):
+        st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(lib.gsr_shard_static_gate(C.byref(s), P, _ptr(geom), geom.numel(), _ptr(img), img.numel(),
+                                             _ptr(flags), 0 if flags is None else int(flags.numel()), _ptr(flag_sum),
+                                             _ptr(error_word), _ptr(frame), int(frame.size(0)), _ptr(status), st),
+                   "gsr_shard_static_gate")
+
+
+def static_status_error(status, capacity: int, segment_capacity: Optional[int], rank: int) -> Optional[str]:
+    """The message ``check_capacity`` raises for the host copy `status` [4] of a static sharded forward, or None."""
+    R, over, max_count, err = (int(v) for v in status)
+    if err:
+        return (f"rank {rank}: a peer barrier of the sparse exchange timed out (a peer rank died, hung or runs a "
+                "different step sequence); the exchanged data of this step are not valid")
+    if not over:
+        return None
+    if R > capacity:
+        why = f"this rank's instance count R={R} exceeds static_capacity={capacity}"
+    elif segment_capacity is not None and max_count > segment_capacity:
+        why = f"a sparse segment of {max_count} records exceeds segment_capacity={segment_capacity}"
+    else:
+        why = f"another rank's instance count exceeds static_capacity={capacity} (this rank's R={R})"
+    return f"rank {rank}: {why}: the frame was rendered empty on every rank; re-size and rebuild the module"
+
+
 def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: torch.Tensor, img: torch.Tensor,
                           grad_out_color: torch.Tensor, acc: torch.Tensor, deterministic: bool, get,
                           grad_depth: Optional[torch.Tensor] = None, grad_alpha: Optional[torch.Tensor] = None):
@@ -737,6 +831,74 @@ class _ShardedRasterize(torch.autograd.Function):
         return (*grads, None, None, None, None, None, None, d_rest, None, *cam_grads)
 
 
+class _ShardedRasterizeStatic(torch.autograd.Function):
+    """_ShardedRasterize for a fixed capacity (two more inputs, `capacity` and the device `status` int32[4]): no host
+    copy and no host wait. The frame all-reduce carries one more float, this rank's overflow flag, and the gate empties
+    the frame on every rank when any flag is set. The backward is _ShardedRasterize's, with R = capacity."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, plan,
+                exchange, pool, deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False,
+                viewmatrix=None, projmatrix=None, campos=None, capacity=1, status=None):
+        ws = pool.take(means3D.device)
+        buf = shard_preprocess(plan, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                               ws=ws, raw_rest=raw_rest)
+        weakref.finalize(buf, pool.give, ws)
+        buf.ws = StaticScratch(ws)                     # scratch of its own, never grown by apply_weights
+        if buf.peer is not None:
+            exchange.barrier(means3D.device)
+        else:
+            exchange.all_gather_inplace(exchange_view(buf))
+        shard_order_static(buf, capacity)
+        planes, npix = (5 if return_alpha else 4), buf.H * buf.W
+        flat = torch.zeros(planes * npix + 1, dtype=torch.float32, device=means3D.device)
+        frame = flat[:planes * npix].view(planes, buf.H, buf.W)
+        shard_render_static(buf, frame[:3], frame[3:4], status)
+        if return_alpha:
+            shard_alpha(buf, frame[4:])
+        flat[-1:].copy_(status[1:2])                   # this rank's 0/1 flag; the all-reduce sums it exactly
+        exchange.all_reduce_sum(flat)
+        static_gate(buf.s, buf.plan.P_pad, buf.geom, buf.img, frame, status, flag_sum=flat[-1:])
+        ctx.buf, ctx.exchange, ctx.deterministic, ctx.depth_grad = buf, exchange, deterministic, bool(depth_grad)
+        ctx.return_alpha, ctx.camera_grad, ctx.rs = bool(return_alpha), viewmatrix is not None, rs
+        if ctx.depth_grad or ctx.return_alpha:
+            ctx.set_materialize_grads(False)
+        radii = shard_slice(buf.radii, plan).clone()
+        ctx.mark_non_differentiable(radii)
+        if return_alpha:
+            return frame[:3], radii, frame[3:4], frame[4:]
+        return frame[:3], radii, frame[3:4]
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
+        return (*_ShardedRasterize.backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha), None, None)
+
+
+def check_static_options(static_capacity, segment_capacity, mode: Optional[str], raster_settings):
+    """The argument checks of ShardedGaussianRasterizer's fixed-capacity forward, made before any collective or device
+    access. Returns (static_capacity, segment_capacity) as ints or None."""
+    def as_count(v, name):   # GaussianRasterizer(static_capacity=...)'s check
+        try:
+            ok = not isinstance(v, bool) and int(v) == v and 0 < int(v) < 2 ** 31
+        except (TypeError, ValueError):
+            ok = False
+        if not ok:
+            raise ValueError(f"{name} must be an int in [1, 2^31), got {v!r}")
+        return int(v)
+    if static_capacity is None:
+        if segment_capacity is not None:
+            raise ValueError("segment_capacity needs static_capacity")
+        return None, None
+    static_capacity = as_count(static_capacity, "static_capacity")
+    if segment_capacity is not None:
+        segment_capacity = as_count(segment_capacity, "segment_capacity")
+        if mode == "dense":
+            raise ValueError("segment_capacity applies to mode='sparse' only")
+    if raster_settings.debug:
+        raise ValueError("static_capacity cannot be combined with debug=True: debug synchronises after every launch")
+    return static_capacity, segment_capacity
+
+
 def p2p_available(exchange: "Exchange") -> bool:
     """Peer mappings need every rank of the group on ONE node with peer access between all device pairs. Checked
     collectively (every rank gets the same answer), so that all ranks take the same code path."""
@@ -808,20 +970,38 @@ class ShardedGaussianRasterizer(nn.Module):
     their ``.grad`` on every rank is the gradient of the whole cloud (the ranks' partials added in ascending rank
     order), the same bits on every rank. Both combine with both modes, ``deterministic`` and ``depth_grad``; neither is
     available on ``forward_raw``.
+    ``static_capacity`` (opt-in, an int in [1, 2^31)): ``GaussianRasterizer(static_capacity=N)`` for a sharded cloud. N
+    is the instance capacity of this rank's owned tiles; ``forward`` and ``forward_raw`` (forward and backward) then never
+    wait for the device and never touch host memory, so a sharded training step can be captured with
+    ``torch.cuda.graph``. ``segment_capacity`` (sparse mode only; default: the allocation, which can never overflow) is
+    the fixed capacity of every sparse segment, the records one rank sends to another. ``self.status`` is a device
+    int32[4] ``{R of this rank, overflow, largest segment (sparse), barrier error (sparse)}``; overflow is 1 on EVERY rank
+    when any rank's R exceeded N or any segment exceeded ``segment_capacity``, and that frame is then EMPTY on every rank
+    (background colour, depth and alpha 0, every gradient exactly zero). Nothing checks it implicitly:
+    ``check_capacity()`` synchronises and raises. Otherwise frames, radii and alpha are the default path's bits and
+    gradients agree with it (bit for bit with ``deterministic=True``). ``apply_weights`` keeps its exact, host-sized path.
+    Not combinable with ``raster_settings.debug``.
     """
 
     def __init__(self, raster_settings: GaussianRasterizationSettings, P_total: int, group=None,
                  p2p: Optional[bool] = None, mode: Optional[str] = None, max_in_flight: int = 3,
                  deterministic: Optional[bool] = None, depth_grad: bool = False, return_alpha: bool = False,
-                 camera_grad: bool = False):
+                 camera_grad: bool = False, static_capacity=None, segment_capacity=None):
         super().__init__()
         self.raster_settings = raster_settings
         self.deterministic = bool(deterministic)
         self.depth_grad = bool(depth_grad)
         self.return_alpha = bool(return_alpha)
         self.camera_grad = bool(camera_grad)
+        # checked before any collective: a bad option raises on its rank instead of leaving the peers waiting
+        self.static_capacity, self.segment_capacity = check_static_options(static_capacity, segment_capacity, mode,
+                                                                           raster_settings)
+        self.status = None   # device int32[4] of the last static forward
         self.exchange = Exchange(group)
         self.plan = ShardPlan(int(P_total), self.exchange.world, self.exchange.rank)
+        if self.segment_capacity is not None and self.segment_capacity > max(self.plan.slice_len, 1):
+            raise ValueError(f"segment_capacity must be in [1, {max(self.plan.slice_len, 1)}] (the allocation), got "
+                             f"{self.segment_capacity}")
         can_p2p = p2p_available(self.exchange) if (p2p is None or p2p or mode == "sparse") else False
         if p2p and not can_p2p:
             raise RuntimeError("p2p=True needs all ranks on one node with peer access between every device pair")
@@ -831,6 +1011,8 @@ class ShardedGaussianRasterizer(nn.Module):
             raise ValueError("mode must be 'sparse' or 'dense'")
         if mode == "sparse" and not can_p2p:
             raise RuntimeError("mode='sparse' needs peer mappings (all ranks on one node with peer access)")
+        if mode == "dense" and self.segment_capacity is not None:   # (mode=None resolved to dense: same on every rank)
+            raise ValueError("segment_capacity applies to mode='sparse' only")
         self.mode = mode
         self.pool = self.sparse_pool = None
         if mode == "sparse":
@@ -838,7 +1020,8 @@ class ShardedGaussianRasterizer(nn.Module):
             dev = torch.device("cuda", torch.cuda.current_device())
             self.sparse_pool = SS.SparsePool(self.plan, dev, int(raster_settings.image_width),
                                              int(raster_settings.image_height), self.exchange, depth=max_in_flight,
-                                             alpha=self.return_alpha, camera=self.camera_grad)
+                                             alpha=self.return_alpha, camera=self.camera_grad,
+                                             device_epoch=self.static_capacity is not None)
         else:
             # fused preprocess + all-gather through peer-mapped workspaces (faster than the NCCL all-gather)
             self.pool = WorkspacePool(self.exchange, _geometry_bytes(_lib.load(), self.plan.P_pad),
@@ -887,6 +1070,9 @@ class ShardedGaussianRasterizer(nn.Module):
         depth_grad = getattr(self, "depth_grad", False)
         return_alpha = getattr(self, "return_alpha", False)
         cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if getattr(self, "camera_grad", False) else (None, None, None)
+        if getattr(self, "static_capacity", None) is not None:
+            return self._apply_static(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp,
+                                      raw_rest, depth_grad, return_alpha, cam)
         if self.mode == "sparse":
             from . import sparse_sharded as SS
             rk0 = self.sparse_pool.all[0]
@@ -898,6 +1084,43 @@ class ShardedGaussianRasterizer(nn.Module):
         return _ShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                        cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic,
                                        depth_grad, raw_rest, return_alpha, *cam)
+
+    def _apply_static(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest,
+                      depth_grad, return_alpha, cam):
+        rs = self.raster_settings
+        if rs.debug:
+            raise ValueError("static_capacity cannot be combined with debug=True: debug synchronises after every launch")
+        if self.status is None or self.status.device != means3D.device:
+            self.status = torch.zeros(STATUS_WORDS, dtype=torch.int32, device=means3D.device)
+        if self.mode == "sparse":
+            from . import sparse_sharded as SS
+            rk0 = self.sparse_pool.all[0]
+            if int(rs.image_width) != rk0.W or int(rs.image_height) != rk0.H:
+                raise RuntimeError("sparse mode: the image size is fixed at construction (peer-mapped frames)")
+            seg_cap = self.segment_capacity if self.segment_capacity is not None else rk0.cap_alloc
+            return SS._SparseShardedRasterizeStatic.apply(
+                means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, rs, self.sparse_pool,
+                self.exchange, self.deterministic, depth_grad, raw_rest, return_alpha, *cam, self.static_capacity,
+                seg_cap, self.status)
+        return _ShardedRasterizeStatic.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                             cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic,
+                                             depth_grad, raw_rest, return_alpha, *cam, self.static_capacity,
+                                             self.status)
+
+    def check_capacity(self) -> int:
+        """Synchronise with the last static forward and raise RuntimeError if it overflowed anywhere (that frame was
+        rendered empty on every rank) or a peer barrier timed out. The answer is the same on every rank; the message
+        names what overflowed. Returns this rank's instance count R otherwise. Never called implicitly."""
+        if self.static_capacity is None or self.status is None:
+            raise RuntimeError("check_capacity() needs a static_capacity rasterizer that has run a forward")
+        seg = None
+        if self.mode == "sparse":
+            seg = self.segment_capacity if self.segment_capacity is not None else self.sparse_pool.all[0].cap_alloc
+        status = self.status.cpu()
+        msg = static_status_error(status, self.static_capacity, seg, self.plan.rank)
+        if msg is not None:
+            raise RuntimeError(msg)
+        return int(status[0])
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):

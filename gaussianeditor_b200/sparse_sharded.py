@@ -37,6 +37,7 @@ from .sharded import (ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, _shard_clo
 
 MAXP = 8  # GSR_MAX_PEERS
 CTRL_BYTES, CTRL_MATRIX_OFFSET, CTRL_ERROR_OFFSET = 512, 64, 32   # GSR_PEER_CTRL_{BYTES,MATRIX_OFFSET,ERROR_OFFSET}
+CTRL_EPOCH_OFFSET, CTRL_STATUS_OFFSET = 320, 352   # GSR_PEER_CTRL_{EPOCH,STATUS}_OFFSET (device-epoch barrier)
 AW_CNT_SLOT = 11   # GSR_SPARSE_AW_CNT_SLOT: float of an apply_weights candidate row that carries the int32 count bits
 ROW_FLOATS = 64    # GSR_PEER_ROW_FLOATS: floats per slot of gsr_peer_row_put
 CAM_SLOT_BYTES = 4 * MAXP * ROW_FLOATS   # the camera-gradient slots of a block (only with camera_grad)
@@ -87,7 +88,11 @@ class SparseRank:
             self.block[:CTRL_BYTES].zero_()
             self.matrix = self.block[CTRL_MATRIX_OFFSET:CTRL_MATRIX_OFFSET + 4 * MAXP * MAXP].view(torch.int32).view(MAXP, MAXP)[:plan.world]
             self.err_word = self.block[CTRL_ERROR_OFFSET:CTRL_ERROR_OFFSET + 4].view(torch.int32)
+            # device-epoch barrier: this rank's barrier counter and the overflow words the ranks sent with their barriers
+            self.epoch_word = self.block[CTRL_EPOCH_OFFSET:CTRL_EPOCH_OFFSET + 4].view(torch.int32)
+            self.status_array = self.block[CTRL_STATUS_OFFSET:CTRL_STATUS_OFFSET + 4 * MAXP].view(torch.int32)[:plan.world]
         self.epoch = 0
+        self.device_epoch = False   # True: every barrier on this block is gsr_peer_barrier_device (static forward)
         if exchange is not None:
             torch.cuda.synchronize(device)
             exchange.barrier(device)      # every rank's control words are zero before anybody raises a flag
@@ -140,7 +145,7 @@ class SparseRank:
 
     def close(self):
         self.scratch.clear()
-        self.matrix = self.err_word = None
+        self.matrix = self.err_word = self.epoch_word = self.status_array = None
         if self.peer is not None:
             self.block = None
             self.peer.close()
@@ -282,11 +287,21 @@ def camera_put(rk: SparseRank, row: torch.Tensor):
                    "gsr_peer_row_put")
 
 
-def peer_barrier(rk: SparseRank, with_row: bool = False):
+def peer_barrier(rk: SparseRank, with_row: bool = False, status_word: Optional[torch.Tensor] = None):
     """Cross-rank barrier on the compute stream through the control words of the peer-mapped blocks (gsr_peer_barrier):
     work queued behind it starts once every rank has reached the same point; with `with_row` this rank's row of the
-    count matrix is first copied into every peer's matrix (the all-gather of the segment sizes)."""
+    count matrix is first copied into every peer's matrix (the all-gather of the segment sizes). On a block of a static
+    module (``rk.device_epoch``) it is gsr_peer_barrier_device, which can be replayed in a CUDA graph; `status_word`
+    (device int32 [1]) then lands in slot `rank` of every rank's ``status_array``."""
     lib = _lib.load()
+    if rk.device_epoch:
+        with torch.cuda.device(rk.device):
+            stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
+            _lib.check(lib.gsr_peer_barrier_device(rk.plan.world, rk.plan.rank, rk.ctrl_ptr_array, 1 if with_row else 0,
+                                                   _ptr(status_word), stream), "gsr_peer_barrier_device")
+        return
+    if status_word is not None:
+        raise RuntimeError("a status word travels with device-epoch barriers only")
     rk.epoch += 1
     with torch.cuda.device(rk.device):
         stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
@@ -348,6 +363,47 @@ def sparse_backward_preprocess(st: SparseStep, depth: bool = False, camera: Opti
     return preprocess_grads(lib, n, st.M, st.inputs, rk.device, call)
 
 
+def sparse_order_static(st: SparseStep, capacity: int):
+    """sparse_order without the host words (gsr_sparse_order_static): R and the largest segment stay on the device (the
+    status kernel of sparse_render_static reads them), and ``st.R = capacity`` sizes the binning and the backward."""
+    lib = _lib.load()
+    rk = st.rk
+    with torch.cuda.device(rk.device):
+        M = rk.plan.world * st.cap
+        st.radii_cand = rk.get("radii_cand", M, torch.int32)
+        stream = C.c_void_p(torch.cuda.current_stream(rk.device).cuda_stream)
+        cand_bytes = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
+        _lib.check(lib.gsr_sparse_order_static(C.byref(st.s), C.byref(st.cplan), _ptr(rk.cand), cand_bytes,
+                                               _ptr(rk.matrix), _ptr(st.radii_cand), stream), "gsr_sparse_order_static")
+    st.R = int(capacity)
+    st.max_count = None
+
+
+def sparse_render_static(st: SparseStep, color: torch.Tensor, depth: torch.Tensor, status: torch.Tensor):
+    """sparse_render for the capacity of sparse_order_static (gsr_shard_render_static with the count matrix): status
+    gets {R, R > capacity or a segment > seg_cap, largest segment, 0} and the owned tiles are emptied on overflow."""
+    from .sharded import render_static
+    lib = _lib.load()
+    rk = st.rk
+    M = rk.plan.world * st.cap
+    gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
+    st.binning, st.img = render_static(st.s, rk.plan.owner(), M, st.R, rk.cand[:gb], st.radii_cand, color, depth,
+                                       status, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow), rk.matrix,
+                                       rk.plan.world, st.cap)
+
+
+def sparse_static_gate(st: SparseStep, frame: torch.Tensor, status: torch.Tensor):
+    """The overflow gate of the static forward on `frame` (a copy of the peer-visible frame), after the frame barrier
+    that carried every rank's overflow word into ``status_array``. Queued before this rank's next barrier on the block:
+    no peer can overwrite the status array before the gate has read it."""
+    from .sharded import static_gate
+    lib = _lib.load()
+    rk = st.rk
+    gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
+    static_gate(st.s, rk.plan.world * st.cap, rk.cand[:gb], st.img, frame, status, flags=rk.status_array,
+                error_word=rk.err_word)
+
+
 def next_capacity(max_count: int, cap_alloc: int) -> int:
     """Segment capacity for the next step from the largest segment seen (identical on every rank: the count matrix is
     all-reduced): 10 % headroom (every slot of headroom is a hole the depth sort still carries), 4096-slot granularity,
@@ -366,11 +422,12 @@ class SparsePool:
     with workspace k on the peers. Also holds the adaptive segment capacity shared by all ranks."""
 
     def __init__(self, plan: ShardPlan, device, W, H, exchange: Exchange, depth: int = 2, alpha: bool = False,
-                 camera: bool = False):
+                 camera: bool = False, device_epoch: bool = False):
         self.all = []
         for k in range(depth):
             rk = SparseRank(plan, device, W, H, exchange=exchange, alpha=alpha, camera=camera)
             rk.index = k
+            rk.device_epoch = bool(device_epoch)   # a static module: device-epoch barriers only, apply_weights included
             self.all.append(rk)
         self.free = list(self.all)
         self.cap = self.all[0].cap_alloc     # first step: worst case; adapts after the first count matrix
@@ -555,3 +612,54 @@ class _SparseShardedRasterize(torch.autograd.Function):
         _mark("gather+preprocess backward")
         ctx.st = None   # the workspace goes back to the pool now, not when the output tensors die
         return (*grads, None, None, None, None, None, d_rest, None, *cam_grads)
+
+
+class _SparseShardedRasterizeStatic(torch.autograd.Function):
+    """_SparseShardedRasterize for a fixed instance capacity and segment capacity (three more inputs: `capacity`,
+    `seg_cap` and the device `status` int32[4]): no redo loop, no pinned words, no host wait, device-epoch barriers (the
+    pool must be built with device_epoch=True). The frame barrier carries this rank's overflow word to every rank and the
+    gate empties the output frame everywhere when any rank overflowed. The backward is _SparseShardedRasterize's with
+    R = capacity, on scratch buffers of its own (sharded.StaticScratch)."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange,
+                deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False, viewmatrix=None,
+                projmatrix=None, campos=None, capacity=1, seg_cap=1, status=None):
+        from .sharded import StaticScratch
+        rk0 = pool.all[0]
+        if (return_alpha and rk0.planes != 5) or (viewmatrix is not None and not rk0.camera) or not rk0.device_epoch:
+            raise RuntimeError("the static sparse forward needs a SparsePool built with device_epoch=True (and alpha=True / "
+                               "camera=True for return_alpha / camera gradients)")
+        rk = pool.take()
+        try:
+            st = sparse_preprocess(rk, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                                   seg_cap, raw_rest)
+            st.rk = StaticScratch(rk)                       # scratch of its own, never grown by apply_weights
+            peer_barrier(rk, with_row=True)                # counts + barrier: every push has landed
+            sparse_order_static(st, capacity)
+        except BaseException:
+            pool.give(rk)
+            raise
+        weakref.finalize(st, pool.give, rk)
+        frame = rk.frame                                    # one writer per pixel: no zero-fill (see the default path)
+        sparse_render_static(st, frame[:3], frame[3:4], status)
+        if return_alpha:
+            sparse_alpha(st, frame[4:5])
+        frame_broadcast(rk)
+        peer_barrier(rk, status_word=status[1:2])           # this rank's overflow word -> every rank's status array
+        out = frame.clone()
+        sparse_static_gate(st, out, status)
+        ctx.st, ctx.exchange, ctx.deterministic, ctx.depth_grad = st, exchange, deterministic, bool(depth_grad)
+        ctx.return_alpha, ctx.camera_grad, ctx.rs = bool(return_alpha), viewmatrix is not None, rs
+        if ctx.depth_grad or ctx.return_alpha:
+            ctx.set_materialize_grads(False)
+        radii = rk.radii_local[:rk.plan.count].clone()
+        ctx.mark_non_differentiable(radii)
+        if return_alpha:
+            return out[:3], radii, out[3:4], out[4:5]
+        return out[:3], radii, out[3:4]
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
+        return (*_SparseShardedRasterize.backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha), None, None,
+                None)

@@ -595,6 +595,18 @@ GSR_API int gsr_sparse_apply_weights_gather(const gsr_sparse_plan* plan, const v
 #define GSR_PEER_CTRL_MATRIX_OFFSET 64
 GSR_API int gsr_peer_barrier(int32_t world, int32_t rank, void* const* peer_ctrl /* [world] host */, uint32_t epoch,
                      int32_t with_matrix_row, void* stream);
+/* gsr_peer_barrier with a DEVICE epoch, for a step that is captured in a CUDA graph and replayed (where a host-side
+ * epoch argument would be frozen). The epoch is the uint32 counter at byte GSR_PEER_CTRL_EPOCH_OFFSET of the OWN block:
+ * the kernel reads it, runs the barrier with counter + 1 and stores counter + 1, so every barrier (and every replay of
+ * one) advances it by one; only this rank writes it. status_word (device int32, may be NULL) is stored into slot `rank`
+ * of the [GSR_MAX_PEERS] int32 status array at byte GSR_PEER_CTRL_STATUS_OFFSET of EVERY block, own included, before the
+ * flag is raised (as the matrix row); it must be read before this rank's next barrier on the block. Timeout and sticky
+ * error word as gsr_peer_barrier. A block must only ever see one kind of barrier: host epochs (gsr_peer_barrier) or
+ * device epochs (this call). */
+#define GSR_PEER_CTRL_EPOCH_OFFSET 320
+#define GSR_PEER_CTRL_STATUS_OFFSET 352
+GSR_API int gsr_peer_barrier_device(int32_t world, int32_t rank, void* const* peer_ctrl /* [world] host */,
+                                    int32_t with_matrix_row, const int32_t* status_word /* may be NULL */, void* stream);
 /* Copies the tile rows this rank owns of its [4,H,W] frame (colour + depth) into the frames of all other ranks
  * (128-bit peer stores): with one writer per pixel this replaces the all-reduce of the frames. A cross-rank barrier
  * must follow before the frames are read. */
@@ -624,6 +636,49 @@ GSR_API int gsr_sparse_backward_preprocess_camera(const gsr_settings* s, const g
                                                   const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
                                                   void* acc_slice, size_t acc_bytes, const gsr_grads* grads,
                                                   int32_t depth, const gsr_camera_grads* camera, void* stream);
+
+/* ---- Gaussian-sharded path for a fixed capacity: no host copy, no host wait -------------------------------------
+ * The sharded counterpart of gsr_forward_static: every call only enqueues work, so a sharded step can be captured in
+ * a CUDA graph. One rank's forward:
+ *   dense : gsr_shard_preprocess(_p2p) -> ALL-GATHER (or barrier) -> gsr_shard_order_static
+ *           -> gsr_shard_render_static(capacity, status) -> gsr_shard_alpha_image (optional)
+ *           -> ALL-REDUCE(sum) of [planes*H*W + 1] floats whose last float is this rank's status[1] (an exact sum of 0/1)
+ *           -> gsr_shard_static_gate(flag_sum = that last float)
+ *   sparse: gsr_sparse_preprocess(seg_cap) -> gsr_peer_barrier_device(with_matrix_row) -> gsr_sparse_order_static
+ *           -> gsr_shard_render_static(P_total = world*seg_cap, capacity, status, counts_matrix, world, seg_cap)
+ *           -> gsr_frame_broadcast(_planes) -> gsr_peer_barrier_device(status_word = status + 1)
+ *           -> gsr_shard_static_gate(flags = the control block's status array [world], error_word) on a copy of the frame
+ *   gsr_shard_order_static / gsr_sparse_order_static: gsr_shard_order / gsr_sparse_order without the host words.
+ *   gsr_shard_render_static: gsr_shard_render with the binning sized for `capacity` instances (gsr_binning_bytes(P_total,
+ *       capacity, W, H)); R is read on the device. status (device int32[4]) = {R of this rank, overflow, largest segment
+ *       (0 without a matrix), 0}: overflow is R > capacity or, with counts_matrix ([world, GSR_MAX_PEERS], the complete
+ *       matrix after the barrier), a segment above seg_cap (world*seg_cap must equal P_total). On overflow the owned
+ *       tiles are emptied. Records past seg_cap were dropped by the push and every sparse kernel clamps a segment to
+ *       seg_cap, so a truncated step stays memory-safe.
+ *   gsr_shard_static_gate: if any of flags[0..num_flags) is non-zero, or *flag_sum != 0 (exactly one of the two is
+ *       given), frame [planes,H,W] (planes 4 or 5) = background colour, depth 0, alpha 0, and this rank's tile ranges,
+ *       per-tile backward start points and tile counts are zeroed, so every backward returns exact zeros (the
+ *       deterministic reduction then reads nothing).
+ *       status[1] = that global flag, the same on every rank; status[3] = *error_word (the control block's sticky
+ *       barrier error word; NULL: 0). In the sparse exchange it must be queued before this rank's next barrier on the
+ *       block: no peer can overwrite the status array before then.
+ * The backward entry points take `capacity` as their num_rendered argument (binning, deterministic and accumulator
+ * scratch sized by it), as with gsr_forward_static. Every argument is checked before the first launch. */
+GSR_API int gsr_shard_order_static(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, void* geometry,
+                                   size_t geometry_bytes, int32_t* radii_total, void* stream);
+GSR_API int gsr_sparse_order_static(const gsr_settings* s, const gsr_sparse_plan* plan, void* cand_ws, size_t cand_bytes,
+                                    const int32_t* counts_matrix, int32_t* radii_cand, void* stream);
+GSR_API int gsr_shard_render_static(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t capacity,
+                                    void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes,
+                                    void* image, size_t image_bytes, const int32_t* radii_total, float* out_color,
+                                    float* out_depth, int32_t* status /* [4] device */,
+                                    const int32_t* counts_matrix /* may be NULL */, int32_t world, int32_t seg_cap,
+                                    void* stream);
+GSR_API int gsr_shard_static_gate(const gsr_settings* s, int32_t P_total, void* geometry, size_t geometry_bytes,
+                                  void* image, size_t image_bytes, const int32_t* flags /* [num_flags] or NULL */,
+                                  int32_t num_flags, const float* flag_sum /* or NULL */,
+                                  const int32_t* error_word /* may be NULL */, float* frame, int32_t planes,
+                                  int32_t* status /* [4] device */, void* stream);
 
 /* ---- tuning / instrumentation ---------------------------------------------------------------------------
  * gsr_set_option("render_variant", v) etc.; unknown names return GSR_ERR_INVALID.

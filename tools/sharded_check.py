@@ -226,6 +226,113 @@ def check_alpha_camera(a, cloud, cam, bg, dL, dev, world):
         (" alpha_camera=ok" if ok else " alpha_camera=FAILED")
 
 
+def check_static(a, cloud, cams, bg, dL, dev, world):
+    """--static: ShardedGaussianRasterizer(static_capacity=N) with deterministic, alpha and depth (and, in a second run,
+    camera) gradients. Per camera, the eager static step must equal the default step bit for bit (frames, radii,
+    gradients, camera gradients) with status[1] == 0; a forward + backward captured in a CUDA graph and replayed for the
+    cameras must equal the eager static calls bit for bit, status included; and in sparse mode the control blocks'
+    epoch counters must advance by (device barriers per step) x (replays)."""
+    from gaussianeditor_b200.rasterizer import _RasterizeGaussians
+    P = cloud.means3D.shape[0]
+    t = cloud_tensors(cloud, dev)
+    views = cams[:3]
+    g = np.random.default_rng(11)
+    H, W = views[0].image_height, views[0].image_width
+    dD = torch.from_numpy(g.random((1, H, W), dtype=np.float32) * 0.1).to(dev)
+    dA = torch.from_numpy(g.random((1, H, W), dtype=np.float32) - 0.5).to(dev)
+    cam_keys = ("viewmatrix", "projmatrix", "campos")
+    R_max = 0
+    for v in views:   # N = 1.25 x the largest R + 4096 (the single-GPU R bounds every rank's)
+        GaussianRasterizer(settings_from(v, bg, cloud.sh_degree, dev))(
+            means3D=t["means3D"], means2D=torch.zeros_like(t["means3D"]), opacities=t["opacities"], shs=t["shs"],
+            scales=t["scales"], rotations=t["rotations"])
+        R_max = max(R_max, int(_RasterizeGaussians.last_state.num_rendered))
+    N = int(1.25 * R_max) + 4096
+    ok, msg = True, ""
+    for camera in (False, True):
+        opts = dict(deterministic=True, return_alpha=True, depth_grad=True, camera_grad=camera)
+        p2p = True if a.mode == "sparse" else a.p2p
+        base = settings_from(views[0], bg, cloud.sh_degree, dev)
+        srs = base._replace(**{k: getattr(base, k).clone().requires_grad_(camera) for k in cam_keys})
+        default = S.ShardedGaussianRasterizer(base, P, p2p=p2p, mode=a.mode, **opts)
+        static = S.ShardedGaussianRasterizer(srs, P, p2p=p2p, mode=a.mode, static_capacity=N, **opts)
+        plan = static.plan
+        leaves = {k: S.shard_slice(v, plan).clone().requires_grad_(True) for k, v in t.items()}
+        m2 = torch.zeros_like(leaves["means3D"], requires_grad=True)
+
+        def step(r):
+            out = r(means3D=leaves["means3D"], means2D=m2, opacities=leaves["opacities"], shs=leaves["shs"],
+                    scales=leaves["scales"], rotations=leaves["rotations"])
+            ((out[0] * dL).sum() + (out[2] * dD).sum() + (out[3] * dA).sum()).backward()
+            return out
+
+        def clear():
+            for v in list(leaves.values()) + [m2] + ([getattr(srs, k) for k in cam_keys] if camera else []):
+                v.grad = None
+
+        def result(out, rs):
+            grads = [v.grad.clone() for v in list(leaves.values()) + [m2]]
+            cgrads = [getattr(rs, k).grad.clone() for k in cam_keys] if camera else []
+            return [o.detach().clone() for o in out], grads, cgrads
+
+        def set_view(v):
+            rs = settings_from(v, bg, cloud.sh_degree, dev)
+            with torch.no_grad():
+                for k in cam_keys:
+                    getattr(srs, k).copy_(getattr(rs, k))
+            return rs
+
+        def same(x, y):
+            return all(torch.equal(p, q) for p, q in zip(x[0] + x[1] + x[2], y[0] + y[1] + y[2]))
+
+        eager, stat = [], []
+        for v in views:
+            rs = settings_from(v, bg, cloud.sh_degree, dev)
+            if camera:
+                rs = rs._replace(**{k: getattr(rs, k).clone().requires_grad_(True) for k in cam_keys})
+            default.raster_settings = rs
+            clear()
+            ref = result(step(default), rs)
+            set_view(v)
+            clear()
+            got = result(step(static), srs)
+            stat.append((got, static.status.clone()))
+            ok = ok and same(ref, got) and int(static.status[1]) == 0 and static.check_capacity() >= 0
+            eager.append(ref)
+        # capture one forward + backward after an eager warm-up on a side stream, then replay it for every view
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(2):
+                clear()
+                step(static)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        clear()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = step(static)
+        epochs = lambda: sum(int(rk.epoch_word[0]) for rk in static.sparse_pool.all) if a.mode == "sparse" else 0
+        e0 = epochs()
+        for v, (want, want_status) in zip(views, stat):
+            set_view(v)
+            graph.replay()
+            torch.cuda.synchronize()
+            got = ([o.detach() for o in out], [v.grad for v in list(leaves.values()) + [m2]],
+                   [getattr(srs, k).grad for k in cam_keys] if camera else [])
+            ok = ok and same(want, got) and torch.equal(static.status, want_status)
+        per_step = (3 + (1 if camera else 0)) if a.mode == "sparse" else 0   # row, frame, return (+ camera) barriers
+        ok = ok and epochs() - e0 == per_step * len(views)
+        msg += f" static(camera={camera}) N={N} epochs+={epochs() - e0}"
+        del out, graph
+        import gc
+        gc.collect()
+        torch.cuda.synchronize()
+        default.close()
+        static.close()
+    return ok, msg + (" static=ok" if ok else " static=FAILED")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--config", default="c3")
@@ -247,11 +354,23 @@ def main():
                     help="also check camera_grad=True: camera gradients of the whole cloud, the same bits on every rank")
     ap.add_argument("--no-fill", action="store_true",
                     help="with --deterministic: torch.utils.deterministic.fill_uninitialized_memory = False")
+    ap.add_argument("--static", action="store_true",
+                    help="check only static_capacity: eager static == default, captured + replayed == eager")
     a = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     dev = torch.device("cuda", local)
     S.init_distributed("nccl", dev)
     cloud, cams = synth.make_config(a.config, P=a.P)
+    if a.static:
+        st_ok, st_msg = check_static(a, cloud, cams, (0.2, 0.5, 0.1), torch.from_numpy(np.random.default_rng(3).random(
+            (3, cams[0].image_height, cams[0].image_width), dtype=np.float32)).to(dev), dev, world)
+        flag = torch.tensor([1 if st_ok else 0], device=dev)
+        dist.all_reduce(flag, op=dist.ReduceOp.MIN)
+        if rank == 0:
+            print(f"world={world} mode={a.mode} p2p={a.p2p}{st_msg}")
+            print("SHARDED_CHECK_OK" if int(flag) == 1 else "SHARDED_CHECK_FAILED")
+        dist.destroy_process_group()
+        sys.exit(0 if int(flag) == 1 else 1)
     cam = cams[0]
     bg = (0.2, 0.5, 0.1)
     H, W = cam.image_height, cam.image_width
