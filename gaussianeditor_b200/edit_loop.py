@@ -208,6 +208,169 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
     return out
 
 
+_SCENE_ATTR = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
+               "scaling": "_scaling", "rotation": "_rotation"}   # EditScene's param-group names -> attributes
+
+
+def sharded_scene(cloud: synth.Cloud, device, plan) -> EditScene:
+    """The EditScene of the whole `cloud` (mask included) cut to `plan`'s rows, with zero statistics and a fresh Adam."""
+    from .sharded import shard_slice
+    scene = EditScene(cloud, device)
+    with torch.no_grad():
+        for attr in _SCENE_ATTR.values():
+            setattr(scene, attr, shard_slice(getattr(scene, attr).detach(), plan).clone().requires_grad_(True))
+        scene.mask = shard_slice(scene.mask, plan).clone()
+        n = plan.count
+        scene.max_radii2D = torch.zeros(n, device=device)
+        scene.xyz_gradient_accum = torch.zeros(n, 1, device=device)
+        scene.denom = torch.zeros(n, 1, device=device)
+    scene._make_optimizer()
+    return scene
+
+
+def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0, mode=None, deterministic=False,
+                          group=None, max_densify_percent=0.01, min_opacity=0.005):
+    """The config-5 step of ``run_edit_loop`` on a Gaussian-sharded cloud, one process per GPU (collective: every rank
+    of `group` calls it with the same arguments; the process group must exist, NCCL).
+
+    Every rank builds the same synthetic cloud and "20 % nearest the origin" mask and keeps its ``shard_slice``. Each
+    step renders the same view on every rank through ``ShardedGaussianRasterizer`` (SH colours with gradient, then
+    ``colors_precomp = mask``), takes the L1 loss on the full frame, back-propagates, updates ``max_radii2D`` and the
+    densification statistics from the local radii and ``viewspace_points.grad``, and runs Adam on the local rows.
+    Every `densification_interval` steps (not after the last): ``global_top_k`` of ``xyz_gradient_accum / denom`` picks
+    the clone set, each rank prunes low opacity (keeping the selected rows) and appends its clones with
+    ``optim_surgery`` (clones start with zero moments, kept rows keep theirs: the reference's behaviour), ``rebalance``
+    with K = 2 moves rows, Adam state and the mask to their new owners, the statistics restart at zero and the
+    rasterizer is re-created for the new size. `mode` and `deterministic` go to the rasterizer.
+
+    Returns ``run_edit_loop``'s dict (counts are global) plus ``densify`` (per densification: ms of selection, surgery,
+    rebalance and re-creation, bytes moved across ranks), ``params`` (this rank's final rows), ``plan`` and ``mode``."""
+    from .gaussian_renderer import _settings_for
+    from .sharded import Exchange, ShardPlan, ShardedGaussianRasterizer
+    device = torch.device("cuda", torch.cuda.current_device())
+    ex = Exchange(group)
+    cloud, cams = synth.make_config("c5", P=P)
+    plan = ShardPlan(cloud.means3D.shape[0], ex.world, ex.rank)
+    scene = sharded_scene(cloud, device, plan)
+    views = [make_view(c, device) for c in cams]
+    bg = torch.zeros(3, device=device)
+    settings = lambda v: _settings_for(v, bg, 1.0, scene.active_sh_degree)
+    make = lambda p: ShardedGaussianRasterizer(settings(views[0]), p.P_total, group=group, mode=mode,
+                                               deterministic=bool(deterministic))
+    rast = make(plan)
+    mode = rast.mode
+
+    def forward(view, colors=None):
+        rast.raster_settings = settings(view)
+        means2D = torch.zeros_like(scene._xyz, requires_grad=True) + 0   # viewspace_points, as render() makes it
+        if means2D.requires_grad:   # not under no_grad (the targets)
+            means2D.retain_grad()
+        kw = dict(shs=scene.get_features) if colors is None else dict(colors_precomp=colors)
+        color, radii, _ = rast(means3D=scene.get_xyz, means2D=means2D, opacities=scene.get_opacity,
+                               scales=scene.get_scaling, rotations=scene.get_rotation, **kw)
+        return color, radii, means2D
+
+    ev = lambda: torch.cuda.Event(enable_timing=True)
+    try:
+        with torch.no_grad():   # cached originals -> edited targets (guidance stub: + seeded noise), as run_edit_loop
+            g = torch.Generator(device=device).manual_seed(seed)
+            targets = []
+            for v in views:
+                img = forward(v)[0]
+                targets.append((img + 0.05 * torch.randn(img.shape, generator=g, device=device)).clamp(0, 1))
+        counts, losses, radii_trace, pend, densify = [], [], [], [], []
+        rng = np.random.default_rng(seed)
+        torch.cuda.synchronize()
+        t_all0, t_all1 = ev(), ev()
+        t_all0.record()
+        for step in range(1, steps + 1):
+            k = int(rng.integers(len(views)))
+            e0, e1, e2, e3 = ev(), ev(), ev(), ev()
+            e0.record()
+            color, radii, means2D = forward(views[k])                                          # forward #1
+            sem, _, _ = forward(views[k], scene.mask[..., None].float().repeat(1, 3))          # forward #2
+            e1.record()
+            semantic = torch.norm(sem, dim=0) > 0.8
+            loss = 10.0 * (color - targets[k]).abs().mean() + 0.0 * semantic.float().mean()
+            scene.optimizer.zero_grad(set_to_none=True)
+            e2.record()
+            loss.backward()
+            e3.record()
+            pend.append((e0, e1, e2, e3))
+            loss = loss.detach()   # the graph (and the workspaces its forwards hold) dies here, not at the next step
+            del color, sem
+            with torch.no_grad():
+                vis = radii > 0
+                scene.max_radii2D[vis] = torch.max(scene.max_radii2D[vis], radii[vis].float())
+                scene.add_densification_stats(means2D.grad, vis)
+            scene.optimizer.step()
+            losses.append(loss.detach())
+            if step % densification_interval == 0 and step < steps:
+                radii_trace.append(scene.max_radii2D.clone())
+                plan, phase = sharded_densify(scene, ex, plan, rast, max_densify_percent, min_opacity)
+                rast = make(plan)
+                torch.cuda.synchronize()
+                phase["recreate"] = (time.perf_counter() - phase.pop("_t")) * 1e3
+                densify.append(phase)
+            counts.append(plan.P_total)
+        t_all1.record()
+        torch.cuda.synchronize()
+        render_ms = sum(e0.elapsed_time(e1) + e2.elapsed_time(e3) for e0, e1, e2, e3 in pend)
+        total_ms = t_all0.elapsed_time(t_all1)
+    finally:
+        rast.close()
+    return dict(steps=steps, total_ms=total_ms, render_ms=render_ms, render_fraction=render_ms / total_ms,
+                ms_per_step=total_ms / steps, P_first=counts[0], P_last=counts[-1], final_loss=float(loss.detach()),
+                counts=counts, losses=torch.stack(losses).cpu().tolist(), max_radii2D=scene.max_radii2D.cpu(),
+                max_radii2D_at_densify=[r.cpu() for r in radii_trace], densify=densify, plan=plan, mode=mode,
+                world=ex.world, params={n: getattr(scene, a).detach() for n, a in _SCENE_ATTR.items()},
+                mask=scene.mask, optimizer=scene.optimizer)
+
+
+def sharded_densify(scene, ex, plan, rast=None, max_densify_percent=0.01, min_opacity=0.005):
+    """One densification of run_sharded_edit_loop (collective) on this rank's rows of `scene`: global top-k, local prune
+    and clone, rebalance (K = 2, the mask carried along), statistics reset; closes `rast`. Returns (new plan, phase
+    times in ms and bytes moved); the caller re-creates the rasterizer and times that from ``phase["_t"]``."""
+    from . import optim_surgery
+    from . import shard_rebalance as SR
+    phase = {}
+    torch.cuda.synchronize()
+    marks = [time.perf_counter()]
+
+    def lap(name):
+        torch.cuda.synchronize()
+        marks.append(time.perf_counter())
+        phase[name] = (marks[-1] - marks[-2]) * 1e3
+
+    with torch.no_grad():
+        grads = (scene.xyz_gradient_accum / scene.denom).squeeze(1)     # NaN where denom == 0: counts as 0
+        k = max(1, int(plan.P_total * max_densify_percent))
+        sel = SR.global_top_k(ex, plan, grads, k)
+        lap("select")
+        keep = (torch.sigmoid(scene._opacity).squeeze(1) >= min_opacity) | sel
+        kept = optim_surgery.prune_optimizer(scene.optimizer, keep)
+        clone = sel[keep]
+        optim_surgery.cat_tensors_to_optimizer(scene.optimizer, {n: p.detach()[clone] for n, p in kept.items()})
+        mask = torch.cat((scene.mask[keep], scene.mask[sel]))
+        counts = [int(keep.sum()), int(sel.sum())]
+        lap("surgery")
+        stats = {}
+        new_plan, (scene.mask,) = SR.rebalance(ex, plan, counts, scene.optimizer, extras=(mask,), stats=stats)
+        for group in scene.optimizer.param_groups:
+            setattr(scene, _SCENE_ATTR[group["name"]], group["params"][0])
+        n = new_plan.count
+        dev = scene._xyz.device
+        scene.max_radii2D = torch.zeros(n, device=dev)
+        scene.xyz_gradient_accum = torch.zeros(n, 1, device=dev)
+        scene.denom = torch.zeros(n, 1, device=dev)
+        lap("rebalance")
+    phase.update(bytes_moved=stats["bytes_moved"], rows_moved=stats["rows_moved"], P_new=new_plan.P_total)
+    if rast is not None:
+        rast.close()
+    phase["_t"] = marks[-1]
+    return new_plan, phase
+
+
 class _FixedCapacityStep:
     """One edit-loop step on the rasterizer's static-capacity forward, run eagerly or as a replayed CUDA graph.
 

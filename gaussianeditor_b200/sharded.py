@@ -133,6 +133,22 @@ class Exchange:
     def all_reduce_sum(self, t: torch.Tensor):
         self.dist.all_reduce(t, op=self.dist.ReduceOp.SUM, group=self.group)
 
+    def all_to_all_single(self, out: torch.Tensor, inp: torch.Tensor, out_splits, in_splits):
+        """Uneven all-to-all along dim 0: rank r receives `out_splits[q]` rows from every rank q, in rank order, and
+        sends `in_splits[d]` rows of `inp` to rank d (the row moves of shard_rebalance.rebalance)."""
+        if self.world == 1:
+            out.copy_(inp)
+            return
+        self.dist.all_to_all_single(out, inp, output_split_sizes=list(out_splits), input_split_sizes=list(in_splits),
+                                    group=self.group)
+
+    def broadcast(self, t: torch.Tensor, src: int = 0):
+        """`t` of group rank `src` on every rank."""
+        if self.world == 1:
+            return
+        g = src if self.group is None else self.dist.get_global_rank(self.group, src)
+        self.dist.broadcast(t, g, group=self.group)
+
     def reduce_scatter_sum(self, total: torch.Tensor, out: torch.Tensor):
         """out[n, ...] = sum over ranks of total[rank*n:(rank+1)*n]."""
         if self.backend == "nccl":
@@ -1028,11 +1044,15 @@ class ShardedGaussianRasterizer(nn.Module):
                                       bool(can_p2p if p2p is None else p2p))
 
     def close(self):
-        """Release the peer-mapped workspaces (collective: every rank must call it)."""
+        """Release the peer-mapped and step workspaces (collective: every rank must call it). A densified cloud gets a
+        new module: ``close()`` and construct ``ShardedGaussianRasterizer(rs, P_new, ...)``, as often as needed in one
+        process group. Calling ``close()`` again does nothing; a closed module cannot render."""
         if self.pool is not None:
             self.pool.close()
         if self.sparse_pool is not None:
             self.sparse_pool.close()
+        self.pool = self.sparse_pool = None
+        self.closed = True
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
@@ -1066,6 +1086,8 @@ class ShardedGaussianRasterizer(nn.Module):
                            features_rest)
 
     def _apply(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest):
+        if getattr(self, "closed", False):
+            raise RuntimeError("this ShardedGaussianRasterizer was closed: construct a new one")
         rs = self.raster_settings
         depth_grad = getattr(self, "depth_grad", False)
         return_alpha = getattr(self, "return_alpha", False)
@@ -1129,6 +1151,8 @@ class ShardedGaussianRasterizer(nn.Module):
         rows and are updated in place (accumulated over calls); ``image_weights`` [CH,H,W] is the full mask, the same on
         every rank. ``cnt`` equals the single-GPU result bit for bit, ``weights`` up to the order of the float sums
         (bit for bit from call to call with ``deterministic=True``)."""
+        if getattr(self, "closed", False):
+            raise RuntimeError("this ShardedGaussianRasterizer was closed: construct a new one")
         if not getattr(self, "deterministic", False):
             _check_deterministic_flag()
         rs = self.raster_settings
