@@ -41,6 +41,7 @@ SYMBOLS = [
     "gsr_forward_static", "gsr_forward_static_raw",
     "gsr_shard_order_static", "gsr_sparse_order_static", "gsr_shard_render_static", "gsr_shard_static_gate",
     "gsr_peer_barrier_device",
+    "gsr_grad_mask_scratch_bytes", "gsr_backward_masked", "gsr_backward_raw_masked",
 ]
 
 
@@ -291,6 +292,13 @@ def load():
     lib.gsr_shard_static_gate.argtypes = [S, i32, vp, sz, vp, sz, vp, i32, vp, vp, vp, i32, vp, vp]
     lib.gsr_peer_barrier_device.restype = C.c_int
     lib.gsr_peer_barrier_device.argtypes = [i32, i32, C.POINTER(vp), i32, vp, vp]
+    lib.gsr_grad_mask_scratch_bytes.restype = sz; lib.gsr_grad_mask_scratch_bytes.argtypes = [i32, i32]
+    lib.gsr_backward_masked.restype = C.c_int
+    lib.gsr_backward_masked.argtypes = [S, Cl, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp, sz, C.POINTER(Grads), CG,
+                                        vp, sz, vp, vp, sz, vp]
+    lib.gsr_backward_raw_masked.restype = C.c_int
+    lib.gsr_backward_raw_masked.argtypes = [S, RC, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, sz, RG, CG, vp, sz, vp,
+                                            vp, sz, vp]
     if lib.gsr_abi_version() != 2:
         raise RuntimeError("libgsr_b200.so ABI version mismatch")
     _lib = lib

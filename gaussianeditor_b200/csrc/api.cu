@@ -187,6 +187,23 @@ static int carve_det_checked(const DetScratch& ds, int P, int64_t R, int CH, Det
   return GSR_OK;
 }
 
+// the gradient mask of one masked call (gsr_backward_masked / gsr_backward_raw_masked) and its first[] scratch
+struct MaskScratch {
+  const uint8_t* mask;
+  void* ptr;
+  size_t bytes;
+};
+static int carve_mask_checked(const MaskScratch& ms, const gsr_settings& s, GradMaskWS& gm) {
+  const size_t need = grad_mask_first_bytes(s.image_width, s.image_height);
+  if (!ms.ptr || ms.bytes < need) {
+    set_error("grad_mask scratch too small: %zu < %zu (gsr_grad_mask_scratch_bytes)", ms.bytes, need);
+    return GSR_ERR_WORKSPACE;
+  }
+  gm.mask = ms.mask;
+  gm.first = (uint32_t*)ms.ptr;
+  return GSR_OK;
+}
+
 // First forward half on a carved workspace: preprocess, depth order, tile-count scan, and the copy of num_rendered to
 // the host. With the tile-binning path (tile_binning.cu) the preprocess kernel accumulates the count itself, so the copy
 // is issued right behind it and the host learns R while the GPU is still sorting. num_rendered_host == nullptr (the
@@ -330,7 +347,8 @@ static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, c
                          const void* binning, size_t binning_bytes, const void* image, size_t image_bytes,
                          const int32_t* radii, const float* dL_dout_color, const float* dL_dout_alpha, void* scratch,
                          size_t scratch_bytes, const gsr_grads* gr, void* stream, const gsr_camera_grads* cam = nullptr,
-                         const float* dL_dout_depth = nullptr, const DetScratch* ds = nullptr) {
+                         const float* dL_dout_depth = nullptr, const DetScratch* ds = nullptr,
+                         const MaskScratch* ms = nullptr) {
   int rc = validate_cloud(s, c);
   if (rc) return rc;
   if (!gr || !dL_dout_color) { set_error("grads / dL_dout_color is null"); return GSR_ERR_INVALID; }
@@ -350,6 +368,8 @@ static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, c
   if (!scratch || scratch_bytes < need) { set_error("backward scratch too small: %zu < %zu", scratch_bytes, need); return GSR_ERR_WORKSPACE; }
   DetWS det;
   if (ds && (rc = carve_det_checked(*ds, c->P, R, 0, det))) return rc;
+  GradMaskWS gm;
+  if (ms && (rc = carve_mask_checked(*ms, *s, gm))) return rc;
   {
     StageScope t(ST_RENDER_BWD, st);  // includes zeroing the accumulators (deterministic mode: the reduction)
     if (!ds || R <= 0) {  // the deterministic reduction writes every accumulator itself
@@ -358,7 +378,7 @@ static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, c
     }
     if (R > 0) {
       rc = launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)scratch, st, TileOwner(), dL_dout_alpha, dL_dout_depth,
-                             ds ? &det : nullptr, c->P, R);
+                             ds ? &det : nullptr, c->P, R, ms ? &gm : nullptr);
       if (rc) return rc;
     }
   }
@@ -373,7 +393,8 @@ static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, c
     CameraBackward cb{cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos, (float*)cam->scratch};
     return launch_preprocess_bwd(*s, *c, g, radii, (const float*)scratch, *gr, st, nullptr, &cb, depth);
   }
-  return launch_preprocess_bwd(*s, *c, g, radii, (const float*)scratch, *gr, st, nullptr, nullptr, depth);
+  return launch_preprocess_bwd(*s, *c, g, radii, (const float*)scratch, *gr, st, nullptr, nullptr, depth,
+                               ms ? ms->mask : nullptr);
 }
 
 size_t gsr_camera_scratch_bytes(int32_t P) { return camera_scratch_bytes(P > 0 ? P : 1); }
@@ -523,7 +544,7 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
                              size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                              size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
                              const float* dL_dout_depth, void* scratch, size_t scratch_bytes, const gsr_raw_grads* gr,
-                             void* stream, const DetScratch* ds = nullptr) {
+                             void* stream, const DetScratch* ds = nullptr, const MaskScratch* ms = nullptr) {
   gsr_cloud c;
   int rc = raw_to_cloud(s, r, c);
   if (rc) return rc;
@@ -539,6 +560,8 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
   if (!scratch || scratch_bytes < need) { set_error("backward scratch too small: %zu < %zu", scratch_bytes, need); return GSR_ERR_WORKSPACE; }
   DetWS det;
   if (ds && (rc = carve_det_checked(*ds, c.P, R, 0, det))) return rc;
+  GradMaskWS gm;
+  if (ms && (rc = carve_mask_checked(*ms, *s, gm))) return rc;
   {
     StageScope t(ST_RENDER_BWD, st);
     if (!ds || R <= 0) {  // the deterministic reduction writes every accumulator itself
@@ -547,14 +570,15 @@ static int raw_backward_impl(const gsr_settings* s, const gsr_raw_cloud* r, int3
     }
     if (R > 0) {
       rc = launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)scratch, st, TileOwner(), nullptr, dL_dout_depth,
-                             ds ? &det : nullptr, c.P, R);
+                             ds ? &det : nullptr, c.P, R, ms ? &gm : nullptr);
       if (rc) return rc;
     }
   }
   const gsr_grads full = raw_grads_as_full(*gr);
   RawBackward raw{r->features_rest, gr->dL_dfeatures_rest};
   StageScope t(ST_PRE_BWD, st);
-  return launch_preprocess_bwd(*s, c, g, radii, (const float*)scratch, full, st, &raw, nullptr, dL_dout_depth != nullptr);
+  return launch_preprocess_bwd(*s, c, g, radii, (const float*)scratch, full, st, &raw, nullptr, dL_dout_depth != nullptr,
+                               ms ? ms->mask : nullptr);
 }
 
 int gsr_backward_raw(const gsr_settings* s, const gsr_raw_cloud* r, int32_t R, const void* geometry,
@@ -583,6 +607,48 @@ int gsr_backward_raw_deterministic(const gsr_settings* s, const gsr_raw_cloud* r
   const DetScratch ds{det_scratch, det_scratch_bytes};
   return raw_backward_impl(s, r, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
                            dL_dout_color, dL_dout_depth, scratch, scratch_bytes, gr, stream, &ds);
+}
+
+// ---- masked backward: gradients only for the Gaussians with grad_mask[i] != 0 ----------------------------------
+size_t gsr_grad_mask_scratch_bytes(int32_t W, int32_t H) { return grad_mask_first_bytes(W > 0 ? W : 0, H > 0 ? H : 0); }
+
+static int check_mask_args(const uint8_t* grad_mask, const gsr_camera_grads* cam) {
+  if (cam) {
+    set_error("camera gradients sum over every Gaussian: they cannot be combined with a gradient mask (camera must be null)");
+    return GSR_ERR_INVALID;
+  }
+  if (!grad_mask) { set_error("grad_mask is null"); return GSR_ERR_INVALID; }
+  return GSR_OK;
+}
+
+int gsr_backward_masked(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry,
+                        size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
+                        size_t image_bytes, const int32_t* radii, const float* dL_dout_color, const float* dL_dout_alpha,
+                        const float* dL_dout_depth, void* scratch, size_t scratch_bytes, const gsr_grads* gr,
+                        const gsr_camera_grads* cam, void* det_scratch, size_t det_scratch_bytes,
+                        const uint8_t* grad_mask, void* mask_scratch, size_t mask_scratch_bytes, void* stream) {
+  const int rc = check_mask_args(grad_mask, cam);
+  if (rc) return rc;
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  const MaskScratch ms{grad_mask, mask_scratch, mask_scratch_bytes};
+  return backward_impl(s, c, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                       dL_dout_color, dL_dout_alpha, scratch, scratch_bytes, gr, stream, nullptr, dL_dout_depth,
+                       det_scratch ? &ds : nullptr, &ms);
+}
+
+int gsr_backward_raw_masked(const gsr_settings* s, const gsr_raw_cloud* r, int32_t R, const void* geometry,
+                            size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
+                            size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                            const float* dL_dout_depth, void* scratch, size_t scratch_bytes, const gsr_raw_grads* gr,
+                            const gsr_camera_grads* cam, void* det_scratch, size_t det_scratch_bytes,
+                            const uint8_t* grad_mask, void* mask_scratch, size_t mask_scratch_bytes, void* stream) {
+  const int rc = check_mask_args(grad_mask, cam);
+  if (rc) return rc;
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  const MaskScratch ms{grad_mask, mask_scratch, mask_scratch_bytes};
+  return raw_backward_impl(s, r, R, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                           dL_dout_color, dL_dout_depth, scratch, scratch_bytes, gr, stream, det_scratch ? &ds : nullptr,
+                           &ms);
 }
 
 // ---- Gaussian-sharded multi-GPU path ---------------------------------------------------------------------

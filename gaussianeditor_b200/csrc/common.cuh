@@ -212,10 +212,19 @@ int launch_render_fwd(const gsr_settings& s, const GeometryWS& g, const BinningW
                       float* out_color, float* out_depth, cudaStream_t st, const TileOwner& own = TileOwner());
 // dL_ddepth != nullptr: also the depth image's upstream [H*W]; dL/dz of each splat goes to acc slot 9 (variant 15 only)
 // det != nullptr: deterministic mode: rows + reduction instead of atomics; acc needs no memset (all P rows written)
+// Masked backward (gsr_backward_masked): only Gaussians with grad_mask[i] != 0 take gradients. first[tile] is the
+// 1-based list position of the tile's front-most edited instance (GRAD_MASK_NONE: the tile has none), written by
+// grad_mask_first_kernel ahead of render_bwd; gsr_grad_mask_scratch_bytes(W, H) holds it.
+constexpr uint32_t GRAD_MASK_NONE = 0xffffffffu;
+struct GradMaskWS {
+  const uint8_t* mask;  // [P]
+  uint32_t* first;      // [Ntile]
+};
+size_t grad_mask_first_bytes(int W, int H);  // first[] of a W x H frame (gsr_grad_mask_scratch_bytes)
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own = TileOwner(),
                       const float* dL_dalpha_img = nullptr, const float* dL_ddepth = nullptr,
-                      const DetWS* det = nullptr, int P = 0, int64_t R = 0);
+                      const DetWS* det = nullptr, int P = 0, int64_t R = 0, const GradMaskWS* gm = nullptr);
 // raw != nullptr: RAW variant -- gradients w.r.t. the raw parameters (gr.dL_dsh = d features_dc, raw->dL_dfeatures_rest)
 struct RawBackward {
   const float* features_rest;
@@ -232,7 +241,8 @@ size_t camera_scratch_bytes(int P);
 // depth: acc slot 9 holds dL/dz (launch_render_bwd with dL_ddepth) and enters the mean (and view-matrix) gradient
 int launch_preprocess_bwd(const gsr_settings& s, const gsr_cloud& c, const GeometryWS& g, const int32_t* radii,
                           const float* acc, const gsr_grads& gr, cudaStream_t st, const RawBackward* raw = nullptr,
-                          const CameraBackward* cam = nullptr, bool depth = false);
+                          const CameraBackward* cam = nullptr, bool depth = false, const uint8_t* grad_mask = nullptr);
+// grad_mask != nullptr (never with cam): a Gaussian with grad_mask[i] == 0 takes the culled branch and gets +0 gradients
 // out_alpha[i] = 1 - final_T[i]  (the reference keeps final_T as ImageState::accum_alpha, rasterizer_impl.h:50)
 int launch_alpha_image(const float* final_T, size_t n, float* out_alpha, cudaStream_t st);
 // the same on the tile rows `own` owns only (the sharded forward writes final_T there and nowhere else)

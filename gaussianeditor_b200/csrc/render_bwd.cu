@@ -59,6 +59,12 @@ template <class Base> struct BwdDetArgs : Base {
   float* rows;           // [2R, ACC_STRIDE]
   uint8_t* flags;        // [2R]
 };
+// Arguments of the masked instantiations (MASK, gsr_backward_masked): which Gaussians take gradients, and where each
+// tile's walk may stop (grad_mask_first_kernel).
+template <class Base> struct BwdMaskArgs : Base {
+  const uint8_t* grad_mask;  // [P] nonzero: the Gaussian is edited
+  const uint32_t* first;     // [Ntile] 1-based position of the front-most edited instance, GRAD_MASK_NONE if none
+};
 template <bool DEPTH, bool DET = false>
 using BwdArgsT = std::conditional_t<DET, BwdDetArgs<std::conditional_t<DEPTH, BwdDepthArgs, BwdArgs>>,
                                     std::conditional_t<DEPTH, BwdDepthArgs, BwdArgs>>;
@@ -117,6 +123,22 @@ __device__ __forceinline__ void hit_update(PixState& p, float* g, float dx, floa
   g[6] = fmaf(wdx, dy, g[6]);
   g[7] = fmaf(wdy, dy, g[7]);
   g[8] += w;
+}
+
+// MASK: the pixel-state part of hit_update alone, for a splat of a Gaussian that takes no gradient. The operations are
+// hit_update's own (rcp with its alpha > 0 select, T * rcp, the dot product s, ar + alpha*(s - ar)), so every later
+// edited splat sees the bits it would see in the unmasked walk.
+template <bool DEPTH = false>
+__device__ __forceinline__ void state_update(PixState& p, float alpha, float c0, float c1, float c2, float z = 0.f) {
+  const float oma = 1.f - alpha;
+  float rcp;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rcp) : "f"(oma));
+  rcp = alpha > 0.f ? rcp : 1.0f;
+  p.T = p.T * rcp;
+  float s = fmaf(c2, p.d2, fmaf(c1, p.d1, c0 * p.d0));
+  if constexpr (DEPTH) s = fmaf(z, p.dD, s);
+  const float dL_dalpha = s - p.ar;
+  p.ar = fmaf(alpha, dL_dalpha, p.ar);
 }
 
 // Warp totals of the moments -> the reference's nine gradient contributions (acc layout: 0..2 dcolor, 3..4 dmean2D,
@@ -440,206 +462,25 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
 // DET: variant 15 (or its DEPTH form) in deterministic mode. Mapping, staging, evaluation, skip decisions and the
 // batched sum are unchanged; the staging lane computes the instance's emission slot and keeps it in sid in place of the
 // Gaussian index, and the flush stores the finished row at that slot instead of adding it to acc.
+// MASK: variant 15 (any of its DEPTH / DET forms) for gsr_backward_masked. The staging lane loads grad_mask of the
+// instance's Gaussian and carries it in bit 31 of the staged sub-block mask (q1.w; `act` clears it again). A splat of an
+// unedited Gaussian is evaluated as usual, but its hits only advance the pixel state (state_update): no column, no batch
+// slot, no flush, no row or flag. The walk stops at the tile's front-most edited position (a.first), and a warp or tile
+// without an edited instance in its range returns at once.
 template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false, bool DEPTH = false,
           bool DET = false>
 __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgsT<DEPTH, DET> a, const int ntiles) {
-  static_assert(!BATCHED || (NSB == 4 && SKIP && !MASKSKIP), "the batched reduction is written for variant 15");
-  static_assert(!DEPTH || BATCHED, "the depth channel is written for variant 15");
-  static_assert(!DET || BATCHED, "deterministic mode is written for variant 15");
-  constexpr int NM = batch_moments<DEPTH>();
-  __shared__ float4 s_stage[BW_WARPS][3][32];
-  __shared__ uint32_t s_id[BW_WARPS][32];
-  constexpr int PARTS = 8 / NSB;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int gw = blockIdx.x * BW_WARPS + warp;
-  const int part = gw % PARTS;
-  if (gw / PARTS >= ntiles) return;
-  const int tile = owned_tile(gw / PARTS, a.gx, a.own_stride, a.own_phase);  // ntiles counts the OWNED tiles
-  float4(*stg)[32] = s_stage[warp];
-  uint32_t* sid = s_id[warp];
-  float4* bpart = nullptr;  // BATCHED: part[slot][moment][BATCH_ROW] of this warp
-  if constexpr (BATCHED) {
-    __shared__ float4 s_part[BW_WARPS][BATCH_NB * NM * (BATCH_ROW / 4)];
-    bpart = s_part[warp];
-  }
-  // BATCHED: a 1 followed by the stage index j (< 32) of each filled slot in 5 bits, the latest slot lowest; warp-uniform
-  uint32_t jpack = 1;
-  float* col = reinterpret_cast<float*>(bpart) + lane;  // BATCHED: this lane's column in the next free slot
-
-  const int tx = tile % a.gx, ty = tile / a.gx;
-  const int lx = lane & 7, ly = lane >> 3;
-  const float X0 = (float)(tx * TILE), Y0 = (float)(ty * TILE);
-  const float fx = X0 + (float)lx, fy = Y0 + (float)ly;
-  const uint2 range = a.ranges[tile];
-  if (a.tile_last[tile] == 0) return;
-  const size_t HW = (size_t)a.H * a.W;
-  const float bg0 = a.bg[0], bg1 = a.bg[1], bg2 = a.bg[2];
-  const float ddelx_dx = 0.5f * a.W, ddely_dy = 0.5f * a.H;
-  const LaneRole role = lane_role(lane);
-
-  PixState ps[NSB];
-  uint32_t nc[NSB], sblast[NSB];
-  uint32_t my_last = 0;
-#pragma unroll
-  for (int k = 0; k < NSB; k++) {
-    const int kg = part * NSB + k;
-    const int px = tx * TILE + 8 * (kg & 1) + lx, py = ty * TILE + 4 * (kg >> 1) + ly;
-    PixState p;
-    p.T = 0.f; p.ar = 0.f; p.d0 = p.d1 = p.d2 = 0.f; p.bgT = 0.f;
-    if constexpr (DEPTH) p.dD = 0.f;
-    nc[k] = 0;
-    if (px < a.W && py < a.H) {
-      const size_t pix_id = (size_t)a.W * py + px;
-      const float Tf = a.final_T[pix_id];
-      p.T = Tf;
-      p.d0 = a.dL_dpix[pix_id];
-      p.d1 = a.dL_dpix[HW + pix_id];
-      p.d2 = a.dL_dpix[2 * HW + pix_id];
-      if constexpr (DEPTH) p.dD = a.dL_ddepth[pix_id];
-      p.bgT = Tf * bg_term(a, pix_id, bg0, bg1, bg2, p);
-      nc[k] = a.n_contrib[pix_id];
-    }
-    ps[k] = p;
-    sblast[k] = __reduce_max_sync(0xffffffffu, nc[k]);
-    my_last = max(my_last, sblast[k]);
-  }
-
-  for (int hi = (int)my_last; hi > 0; hi -= 32) {
-    const int pos = hi - lane;
-    uint32_t mask = 0, id = 0, ex = 0;
-    float4 q0, q1, q2;
-    if (pos >= 1) {
-      id = a.point_list[range.x + pos - 1];
-      const float4* r = reinterpret_cast<const float4*>(a.records + id);
-      q0 = __ldg(r);
-      q1 = __ldg(r + 1);
-      q2 = __ldg(r + 2);
-      mask = splat_subblock_mask<NSB>(q0, q1, X0, Y0, part);
-      if constexpr (DET) {  // after the mask: one register less across splat_subblock_mask (no spill at 5 CTAs/SM)
-        if (mask != 0) ex = __ldg(a.excl + id);
-      }
-    }
-    const uint32_t keep = __ballot_sync(0xffffffffu, mask != 0);
-    const int cnt = __popc(keep);
-    if (mask != 0) {
-      const int slot = __popc(keep & ((1u << lane) - 1u));
-      uint32_t es = 0;  // DET: the instance's emission slot, kept in sid (the flush needs no Gaussian index then)
-      if constexpr (DET)
-        es = emission_slot(ex, q0.x, q0.y, __float_as_int(q2.w), a.gx, a.gy, tx, ty, a.own_stride, a.own_phase);
-      q1.w = __uint_as_float(mask);
-      q2.w = __uint_as_float((uint32_t)pos);
-      stg[0][slot] = q0;
-      stg[1][slot] = q1;
-      stg[2][slot] = q2;
-      sid[slot] = DET ? es : id;
-    }
-    __syncwarp();
-    const uint32_t lo = (uint32_t)max(hi - 31, 1);
-    uint32_t act = 0;
-#pragma unroll
-    for (int k = 0; k < NSB; k++)
-      if (sblast[k] >= lo) act |= 1u << k;
-
-    for (int j = 0; j < cnt; j++) {
-      const float4 s1 = stg[1][j];
-      const uint32_t m = __float_as_uint(s1.w) & act;
-      if (m == 0) continue;
-      const float4 s0 = stg[0][j];
-      const float4 s2 = stg[2][j];
-      const uint32_t spos = __float_as_uint(s2.w);
-      float dxv[2], dxA[2], dxB[2], dyv[NSB / 2], t0[NSB / 2];
-#pragma unroll
-      for (int c = 0; c < 2; c++) {
-        dxv[c] = s0.x - (fx + 8.0f * c);
-        dxA[c] = __fmul_rn(dxv[c], s0.z);
-        dxB[c] = __fmul_rn(dxv[c], s0.w);
-      }
-#pragma unroll
-      for (int r = 0; r < NSB / 2; r++) {
-        dyv[r] = s0.y - (fy + 4.0f * (float)(part * (NSB / 2) + r));
-        t0[r] = __fmul_rn(__fmul_rn(dyv[r], s1.x), dyv[r]);
-      }
-      // ---- NSB independent evaluations ----
-      float G[NSB], al[NSB], pw[NSB];
-      bool near = false;
-#pragma unroll
-      for (int k = 0; k < NSB; k++) {
-        if (MASKSKIP && !((m >> k) & 1u)) {  // warp-uniform: the splat's alpha >= 1/255 ellipse misses this sub-block
-          pw[k] = 1.0f; G[k] = 0.f; al[k] = 0.f;
-          continue;
-        }
-        const int c = k & 1, r = k >> 1;
-        const float s = __fmaf_rn(dxv[c], dxA[c], t0[r]);
-        pw[k] = __fmaf_rn(s, -0.5f, -__fmul_rn(dxB[c], dyv[r]));
-        G[k] = ex2_approx(pw[k] * 1.4426950408889634f);
-        al[k] = fminf(0.99f, s1.y * G[k]);
-        near |= fabsf(al[k] - 1.0f / 255.0f) <= (1.0f / 255.0f) * 1e-5f;
-      }
-      if (near) {  // rare: too close to the 1/255 threshold to call with ex2.approx -> the forward's exact arithmetic
-#pragma unroll
-        for (int k = 0; k < NSB; k++) {
-          if (MASKSKIP && !((m >> k) & 1u)) continue;
-          G[k] = expf(pw[k]);
-          al[k] = fminf(0.99f, __fmul_rn(s1.y, G[k]));
-        }
-      }
-      bool anyhit = false;
-      uint32_t hitk = 0;  // SKIP: warp-uniform mask of sub-blocks with at least one hit
-#pragma unroll
-      for (int k = 0; k < NSB; k++) {
-        const bool ok = ((m >> k) & 1u) && !(pw[k] > 0.0f) && spos <= nc[k] && !(al[k] < 1.0f / 255.0f);
-        G[k] = ok ? G[k] : 0.f;
-        al[k] = ok ? al[k] : 0.f;
-        anyhit |= ok;
-        if (SKIP && __any_sync(0xffffffffu, ok)) hitk |= 1u << k;
-      }
-      if (SKIP ? hitk == 0 : !__any_sync(0xffffffffu, anyhit)) continue;
-      float g[NM];
-#pragma unroll
-      for (int i = 0; i < NM; i++) g[i] = 0.f;
-#pragma unroll
-      for (int k = 0; k < NSB; k++) {
-        // (alpha, G) = (0, 0) makes every update below an exact no-op: 1/(1-0) = 1, +0 contributions
-        if (SKIP && !((hitk >> k) & 1u)) continue;
-        if (MASKSKIP && !((m >> k) & 1u)) continue;
-        hit_update<DEPTH>(ps[k], g, dxv[k & 1], dyv[k >> 1], G[k], al[k], s1.y, s2.x, s2.y, s2.z, s1.z);
-      }
-      if constexpr (!BATCHED) {
-        float m8;
-        const float tot = warp_sum9(g, lane, m8);
-        finish_and_add(a.acc + (size_t)sid[j] * ACC_STRIDE, tot, m8, role, s0.z, s0.w, s1.x, s1.y, ddelx_dx, ddely_dy);
-      } else {
-#pragma unroll
-        for (int i = 0; i < NM; i++) col[BATCH_ROW * i] = g[i];
-        col += NM * BATCH_ROW;
-        jpack = (jpack << 5) | (uint32_t)j;
-        if (jpack >= 1u << (5 * BATCH_NB)) {  // all slots filled
-          __syncwarp();
-          if constexpr (DET)
-            flush_moments<DEPTH, true>(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy, a.rows, a.flags,
-                                       part);
-          else
-            flush_moments<DEPTH>(bpart, jpack, BATCH_NB, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
-          __syncwarp();  // the next splat overwrites slot 0
-          jpack = 1;
-          col -= BATCH_NB * NM * BATCH_ROW;
-        }
-      }
-    }
-    if constexpr (BATCHED) {
-      if (jpack > 1) {  // before the stage is refilled
-        __syncwarp();
-        if constexpr (DET)
-          flush_moments<DEPTH, true>(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy,
-                                     a.rows, a.flags, part);
-        else
-          flush_moments<DEPTH>(bpart, jpack, (31 - __clz(jpack)) / 5, stg, sid, a.acc, lane, ddelx_dx, ddely_dy);
-        col = reinterpret_cast<float*>(bpart) + lane;
-        jpack = 1;
-      }
-    }
-    __syncwarp();
-  }
+  constexpr bool MASK = false;
+#include "render_bwd_flat_body.inc"
+}
+// MASK form of variant 15 (gsr_backward_masked), with DEPTH / DET as render_bwd_flat_kernel. A kernel of its own name
+// (not a further template parameter of render_bwd_flat_kernel), so that every existing kernel keeps its symbol.
+template <int MINB, bool DEPTH, bool DET>
+__global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_masked_kernel(const BwdMaskArgs<BwdArgsT<DEPTH, DET>> a,
+                                                                                const int ntiles) {
+  constexpr int NSB = 4;
+  constexpr bool SKIP = true, MASKSKIP = false, BATCHED = true, MASK = true;
+#include "render_bwd_flat_body.inc"
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -710,11 +551,91 @@ __global__ void __launch_bounds__(TILE_PIX) render_bwd_cta_kernel(const BwdArgs 
   }
 }
 
+// ------------------------------------------------------------------------------------------------------
+// Masked backward: where each tile's walk may stop. One warp per tile scans the list front to back in chunks of 32,
+// positions [0, min(tile_last, list length)), loads grad_mask of each instance's Gaussian and takes a ballot:
+// first[tile] = 1-based position of the first edited instance, GRAD_MASK_NONE when there is none. At most 4 + 1 bytes
+// per walked instance, and a tile stops reading at its first edited instance.
+// ------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(BW_WARPS * 32) grad_mask_first_kernel(const uint2* __restrict__ ranges,
+                                                                        const uint32_t* __restrict__ point_list,
+                                                                        const uint32_t* __restrict__ tile_last,
+                                                                        const uint8_t* __restrict__ grad_mask,
+                                                                        uint32_t* __restrict__ first, int ntiles) {
+  const int lane = threadIdx.x & 31;
+  const int tile = blockIdx.x * BW_WARPS + (threadIdx.x >> 5);
+  if (tile >= ntiles) return;
+  const uint2 range = ranges[tile];
+  const uint32_t n = min(tile_last[tile], range.y > range.x ? range.y - range.x : 0u);
+  uint32_t f = GRAD_MASK_NONE;
+  for (uint32_t b = 0; b < n; b += 32) {
+    const uint32_t i = b + lane;
+    const bool e = i < n && __ldg(grad_mask + __ldg(point_list + range.x + i)) != 0;
+    const uint32_t hit = __ballot_sync(0xffffffffu, e);
+    if (hit) {
+      f = b + (uint32_t)__ffs(hit);  // __ffs is 1-based: the 1-based position
+      break;
+    }
+  }
+  if (lane == 0) first[tile] = f;
+}
+
 }  // namespace
+
+size_t grad_mask_first_bytes(int W, int H) {
+  const size_t ntiles = (size_t)((W + TILE - 1) / TILE) * ((H + TILE - 1) / TILE);
+  return align_up((ntiles > 0 ? ntiles : 1) * sizeof(uint32_t));
+}
+
+// The masked walk: first[] of every tile, then one of the four MASK instantiations of variant 15. 4 CTAs/SM for all four
+// except the atomic colour kernel, which keeps the default's 5 (see DESIGN.md section 3 for the register counts).
+static int launch_render_bwd_masked(const BwdArgs& a, int ntiles, const float* dL_ddepth, const DetWS* det,
+                                    const GradMaskWS& gm, bool debug, cudaStream_t st) {
+  grad_mask_first_kernel<<<(ntiles + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(
+      a.ranges, a.point_list, a.tile_last, gm.mask, gm.first, ntiles);
+  g_launches++;
+  int rc = check_launch("grad_mask_first", debug, st);
+  if (rc) return rc;
+  const int blocks = (ntiles * 2 + BW_WARPS - 1) / BW_WARPS;
+  auto fill = [&](auto& ma) {
+    ma.grad_mask = gm.mask;
+    ma.first = gm.first;
+  };
+  if (det != nullptr) {
+    if (dL_ddepth != nullptr) {
+      BwdMaskArgs<BwdDetArgs<BwdDepthArgs>> ma;
+      static_cast<BwdArgs&>(ma) = a;
+      ma.dL_ddepth = dL_ddepth;
+      ma.excl = det->excl; ma.rows = det->rows; ma.flags = det->flags;
+      fill(ma);
+      render_bwd_masked_kernel<4, true, true><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+    } else {
+      BwdMaskArgs<BwdDetArgs<BwdArgs>> ma;
+      static_cast<BwdArgs&>(ma) = a;
+      ma.excl = det->excl; ma.rows = det->rows; ma.flags = det->flags;
+      fill(ma);
+      render_bwd_masked_kernel<4, false, true><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+    }
+  } else if (dL_ddepth != nullptr) {
+    BwdMaskArgs<BwdDepthArgs> ma;
+    static_cast<BwdArgs&>(ma) = a;
+    ma.dL_ddepth = dL_ddepth;
+    fill(ma);
+    render_bwd_masked_kernel<4, true, false><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+  } else {
+    BwdMaskArgs<BwdArgs> ma;
+    static_cast<BwdArgs&>(ma) = a;
+    fill(ma);
+    render_bwd_masked_kernel<5, false, false><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+  }
+  g_launches++;
+  return check_launch("render_bwd (masked)", debug, st);
+}
 
 int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
                       const float* dL_dpix, float* acc, cudaStream_t st, const TileOwner& own,
-                      const float* dL_dalpha_img, const float* dL_ddepth, const DetWS* det, int P, int64_t R) {
+                      const float* dL_dalpha_img, const float* dL_ddepth, const DetWS* det, int P, int64_t R,
+                      const GradMaskWS* gm) {
   BwdArgs a;
   a.dL_dalpha_img = dL_dalpha_img;
   a.own_stride = own.stride; a.own_phase = own.phase;
@@ -724,6 +645,12 @@ int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningW
   a.bg = s.bg; a.final_T = im.final_T; a.n_contrib = im.n_contrib; a.dL_dpix = dL_dpix; a.acc = acc;
   const int ntiles = a.gx * own.owned_rows(a.gy);  // tiles this rank walks (all of them when own = {1,0})
   if (ntiles == 0) return GSR_OK;
+  if (gm != nullptr) {  // masked backward (single-GPU entry points only): variant 15, atomic or deterministic
+    int rc = det ? launch_det_prepare(P, R, 2, g, *det, st) : GSR_OK;
+    if (rc) return rc;
+    if ((rc = launch_render_bwd_masked(a, ntiles, dL_ddepth, det, *gm, s.debug != 0, st))) return rc;
+    return det ? launch_det_reduce_acc(P, dL_ddepth != nullptr, g, *det, acc, st) : GSR_OK;
+  }
   if (det != nullptr) {  // deterministic mode: variant 15 (or its depth form) writes rows, one kernel reduces them
     int rc = launch_det_prepare(P, R, 2, g, *det, st);
     if (rc) return rc;

@@ -55,7 +55,17 @@ class EditScene:
         self.max_radii2D = torch.zeros(P, device=device)
         self.xyz_gradient_accum = torch.zeros(P, 1, device=device)
         self.denom = torch.zeros(P, 1, device=device)
+        self.hooks = None   # apply_grad_mask: the registered gradient hooks
         self._make_optimizer()
+
+    def apply_grad_mask(self):
+        """GaussianEditor's ``apply_grad_mask`` (scene/gaussian_model.py:837-856): a hook on each parameter multiplies its
+        gradient by ``mask``, read when the hook runs. Here on all six parameters, ``_rotation`` included (GaussianEditor
+        leaves it out), so that every gradient of an unedited Gaussian is zero, as under ``render(..., grad_mask=...)``.
+        Densification re-registers the hooks on the new tensors."""
+        def hook(grad):
+            return grad * (self.mask[:, None] if grad.ndim == 2 else self.mask[:, None, None])
+        self.hooks = [getattr(self, a).register_hook(hook) for a in _SCENE_ATTR.values()]
 
     def _params(self):
         return [("xyz", self._xyz, 1.6e-5), ("f_dc", self._features_dc, 2.5e-3), ("f_rest", self._features_rest, 1.25e-4),
@@ -91,11 +101,14 @@ class EditScene:
         self.xyz_gradient_accum.add_(torch.where(update_filter[:, None], norm, 0.0))
         self.denom.add_(update_filter[:, None].float())
 
-    def densify_and_prune(self, max_densify_percent=0.01, min_opacity=0.005):
+    def densify_and_prune(self, max_densify_percent=0.01, min_opacity=0.005, masked=False):
         """Clone the `max_densify_percent` Gaussians with the largest mean view-space gradient, prune those below
-        `min_opacity` (shape of scene/gaussian_model.py:768-809; the split branch is folded into clone)."""
+        `min_opacity` (shape of scene/gaussian_model.py:768-809; the split branch is folded into clone). ``masked``: an
+        edit under a gradient mask, whose unmasked view-space gradients are zeroed first (gaussian_model.py:773)."""
         with torch.no_grad():
             grads = (self.xyz_gradient_accum / self.denom.clamp_min(1)).squeeze(1)
+            if masked:
+                grads.masked_fill_(~self.mask, 0.0)
             P = grads.numel()
             k = max(1, int(P * max_densify_percent))
             sel = torch.topk(grads, k).indices
@@ -111,6 +124,8 @@ class EditScene:
             self.xyz_gradient_accum = torch.zeros(n, 1, device=dev)
             self.denom = torch.zeros(n, 1, device=dev)
             self._make_optimizer()   # the reference re-stitches Adam state; the harness restarts it
+        if self.hooks is not None:
+            self.apply_grad_mask()
 
 
 def make_view(cam: synth.Camera, device):
@@ -122,18 +137,29 @@ def make_view(cam: synth.Camera, device):
 
 
 def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densification_interval=100, seed=0,
-                  log=None, fused_activations=False, cuda_graph=False, static_capacity=False, deterministic=None):
+                  log=None, fused_activations=False, cuda_graph=False, static_capacity=False, deterministic=None,
+                  grad_mask=None):
     """Returns a dict with total / render wall times (CUDA-event timed) and the per-step Gaussian counts.
     ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only).
     ``cuda_graph=True`` captures one step per Gaussian count and replays it (see the module docstring);
     ``static_capacity=True`` runs that same step eagerly. Both size the rasterizer's static capacity as
     1.25 x the largest num_rendered over an eager pass of all views + 4096, recomputed after every densification, use
     Adam(capturable=True), and raise RuntimeError at the next densification point (or the end) if any forward
-    exceeded the capacity. ``deterministic`` is passed to ``render`` when given."""
+    exceeded the capacity. ``deterministic`` is passed to ``render`` when given.
+    ``grad_mask`` trains under the scene's mask ("20 % nearest the origin") as a GaussianEditor edit does: ``"hooks"``
+    registers ``EditScene.apply_grad_mask`` (GaussianEditor's hooks, on all six parameters), ``"kernel"`` passes
+    ``grad_mask=scene.mask`` to the SH render instead; both zero the unmasked view-space gradients before densifying.
+    ``None`` (default): no mask."""
     from . import gaussian_renderer as GR
+    if grad_mask not in (None, "hooks", "kernel"):
+        raise ValueError(f'grad_mask must be None, "hooks" or "kernel", got {grad_mask!r}')
     fixed = bool(cuda_graph or static_capacity)
     cloud, cams = synth.make_config("c5", P=P)
     scene = EditScene(cloud, device, capturable=fixed)
+    if grad_mask == "hooks":
+        scene.apply_grad_mask()
+    # the SH render's mask argument, looked up per step: densification replaces scene.mask
+    mask_kw = (lambda: {"grad_mask": scene.mask}) if grad_mask == "kernel" else (lambda: {})
     views = [make_view(c, device) for c in cams]
     pipe = SimpleNamespace(convert_SHs_python=False, compute_cov3D_python=False, debug=False)
     bg = torch.zeros(3, device=device)
@@ -150,7 +176,7 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                 img = GR.render(v, scene, pipe, bg)["render"]
                 targets.append((img + 0.05 * torch.randn(img.shape, generator=g, device=device)).clamp(0, 1))
         if fixed:
-            loop = _FixedCapacityStep(GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph)
+            loop = _FixedCapacityStep(GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw)
         render_ms = 0.0
         counts, losses, radii_trace = [], [], []
         rng = np.random.default_rng(seed)
@@ -165,7 +191,7 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
             else:
                 e0, e1, e2, e3 = ev(), ev(), ev(), ev()
                 e0.record()
-                pkg = GR.render(views[k], scene, pipe, bg, fused_activations=fused_activations)       # forward #1
+                pkg = GR.render(views[k], scene, pipe, bg, fused_activations=fused_activations, **mask_kw())  # #1
                 sem = GR.render(views[k], scene, pipe, bg,
                                 override_color=scene.mask[..., None].float().repeat(1, 3))["render"]  # forward #2
                 e1.record()
@@ -186,7 +212,7 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                 if fixed:
                     loop.check_capacity()
                 radii_trace.append(scene.max_radii2D.clone())   # what the reference's prune test reads (:790-795)
-                scene.densify_and_prune()
+                scene.densify_and_prune(masked=grad_mask is not None)
                 if fixed:
                     loop.reset()
             counts.append(scene._xyz.shape[0])
@@ -202,7 +228,8 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
     out = dict(steps=steps, total_ms=total_ms, render_ms=render_ms, render_fraction=render_ms / total_ms,
                ms_per_step=total_ms / steps, P_first=counts[0], P_last=counts[-1], final_loss=float(loss.detach()),
                counts=counts, losses=torch.stack(losses).cpu().tolist(), max_radii2D=scene.max_radii2D.cpu(),
-               max_radii2D_at_densify=[r.cpu() for r in radii_trace])
+               max_radii2D_at_densify=[r.cpu() for r in radii_trace],
+               params={n: getattr(scene, a).detach() for n, a in _SCENE_ATTR.items()}, optimizer=scene.optimizer)
     if fixed:   # the step is not split by events: no render time
         out.update(render_ms=None, render_fraction=None, capacities=loop.capacities)
     return out
@@ -379,9 +406,9 @@ class _FixedCapacityStep:
     step copies its camera and target into the captured input tensors and replays. Overflows are accumulated on the
     device and read only by `check_capacity`."""
 
-    def __init__(self, GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph):
+    def __init__(self, GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw=dict):
         self.GR, self.scene, self.views, self.targets, self.pipe, self.bg = GR, scene, views, targets, pipe, bg
-        self.fused, self.opt, self.cuda_graph = fused_activations, opt, cuda_graph
+        self.fused, self.opt, self.cuda_graph, self.mask_kw = fused_activations, opt, cuda_graph, mask_kw
         dev = bg.device
         self.overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         v0 = views[0]
@@ -409,7 +436,7 @@ class _FixedCapacityStep:
     def _body(self, view, target):
         GR, scene = self.GR, self.scene
         pkg = GR.render(view, scene, self.pipe, self.bg, fused_activations=self.fused, static_capacity=self.capacity,
-                        **self.opt)                                                                   # forward #1
+                        **self.opt, **self.mask_kw())                                                 # forward #1
         sem_pkg = GR.render(view, scene, self.pipe, self.bg, override_color=scene.mask[..., None].float().repeat(1, 3),
                             static_capacity=self.capacity, **self.opt)                                 # forward #2
         semantic = torch.norm(sem_pkg["render"], dim=0) > 0.8

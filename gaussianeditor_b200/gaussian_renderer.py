@@ -63,7 +63,8 @@ def _python_sh_colors(pc, camera_center) -> torch.Tensor:
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           fused_activations: bool = False, depth_grad: bool = False, deterministic=None, static_capacity=None):
+           fused_activations: bool = False, depth_grad: bool = False, deterministic=None, static_capacity=None,
+           grad_mask=None):
     """Render the scene; background tensor must be on the GPU. Returns the reference's dictionary:
     render [3,H,W], viewspace_points [P,3] (grad sink for densification), visibility_filter, radii, depth_3dgs.
 
@@ -84,7 +85,12 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     ``static_capacity`` (opt-in, not in the reference; an int): the rasterizer's fixed-capacity forward
     (``GaussianRasterizer(static_capacity=...)``), which never waits for the GPU, so the step can be captured in a CUDA
     graph. The result dictionary then also holds ``status``, the rasterizer's device int32[2]
-    ``{num_rendered, num_rendered > static_capacity}``; a frame over the capacity is rendered empty."""
+    ``{num_rendered, num_rendered > static_capacity}``; a frame over the capacity is rendered empty.
+
+    ``grad_mask`` (opt-in, not in the reference; a bool or uint8 CUDA tensor [P], e.g. ``pc.mask``): only the masked
+    Gaussians take gradients, every gradient row of the others is +0.0, and the rasterizer skips their backward work
+    (``GaussianRasterizer(grad_mask=...)``). It replaces GaussianEditor's ``apply_grad_mask`` hooks; see INTEGRATION.md
+    for the differences."""
     xyz = pc.get_xyz
     # gradient sink for the 2-D means: densification reads its .grad (gaussian_renderer/__init__.py:60-69)
     screenspace_points = torch.zeros_like(xyz, requires_grad=True) + 0
@@ -92,13 +98,15 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         screenspace_points.retain_grad()
     except Exception:
         pass
-    # depth_grad / deterministic are passed only when asked for: by default the rasterizer is constructed exactly as the
+    # depth_grad / deterministic / static_capacity / grad_mask are passed only when asked for: by default the rasterizer is constructed exactly as the
     # reference's render() does, so any class with the reference's constructor (raster_settings only) can stand in for it
     opt = {"depth_grad": True} if depth_grad else {}
     if deterministic is not None:
         opt["deterministic"] = bool(deterministic)
     if static_capacity is not None:
         opt["static_capacity"] = static_capacity
+    if grad_mask is not None:
+        opt["grad_mask"] = grad_mask
     rasterizer = GaussianRasterizer(
         raster_settings=_settings_for(viewpoint_camera, bg_color, scaling_modifier, pc.active_sh_degree), **opt)
     python_sh = getattr(pipe, "convert_SHs_python", False)

@@ -116,7 +116,7 @@ def _make_cloud(P, means3D, opacities, sh, colors_precomp, scales, rotations, co
 
 class _ForwardState:
     """What the forward leaves behind for backward / apply_weights / parity tests."""
-    __slots__ = ("geom", "binning", "img", "radii", "num_rendered", "cap", "P", "M", "W", "H")
+    __slots__ = ("geom", "binning", "img", "radii", "num_rendered", "cap", "P", "M", "W", "H", "mask_first")
 
 
 def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, *, render=True,
@@ -479,6 +479,141 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
         return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None
 
 
+def _masked_scratch(lib, state, ctx, device):
+    """(det_scratch, bytes, mask_scratch, bytes) of a masked backward; the first[] scratch stays on the forward state
+    (``state.mask_first``, int32 [Ntile]) for tests and instrumentation."""
+    u8 = dict(dtype=torch.uint8, device=device)
+    dscratch, dbytes = None, 0
+    if ctx.deterministic:
+        dbytes = lib.gsr_deterministic_scratch_bytes(state.P, state.cap, 0)
+        dscratch = torch.empty(dbytes, **u8)
+    mbytes = lib.gsr_grad_mask_scratch_bytes(state.W, state.H)
+    mscratch = torch.empty(mbytes, **u8)
+    state.mask_first = mscratch
+    return dscratch, dbytes, mscratch, mbytes
+
+
+class _RasterizeGaussiansMasked(torch.autograd.Function):
+    """``GaussianRasterizer(grad_mask=...)`` on ``forward``: the forward of _RasterizeGaussians, and one backward through
+    gsr_backward_masked for every combination of alpha, depth, deterministic mode and static capacity. The mask is kept
+    on the node as given (not saved for backward): the backward reads whatever it holds then."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                raster_settings, return_alpha, depth_grad, deterministic, static, grad_mask):
+        out = _RasterizeGaussians.forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                          cov3Ds_precomp, raster_settings, return_alpha, None, None, None, depth_grad,
+                                          deterministic, static)
+        ctx.grad_mask = grad_mask
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
+        lib = _lib.load()
+        rs, state = ctx.raster_settings, ctx.state
+        (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, radii, geom, binning,
+         img) = ctx.saved_tensors
+        device = means3D.device
+        P, M, W, H = state.P, state.M, state.W, state.H
+        with torch.cuda.device(device):
+            if grad_out_color is None:   # depth_grad: only the depth and/or alpha outputs carry a loss
+                grad_out_color = torch.zeros(3, H, W, dtype=torch.float32, device=device)
+            grad_out_color = _f32c(grad_out_color, device)
+            f32 = dict(dtype=torch.float32, device=device)
+            dL_dmeans3D = torch.empty(P, 3, **f32); dL_dmeans2D = torch.empty(P, 3, **f32)
+            dL_dcolors = torch.empty(P, 3, **f32); dL_dopacity = torch.empty(P, 1, **f32)
+            dL_dcov3D = torch.empty(P, 6, **f32); dL_dsh = torch.empty(P, M, 3, **f32)
+            dL_dscales = torch.empty(P, 3, **f32); dL_drotations = torch.empty(P, 4, **f32)
+            if P > 0:
+                keep = []
+                s = _make_settings(rs, M, device, keep)
+                c = _make_cloud(P, means3D, opacities, sh, colors_precomp, scales, rotations, cov3Ds_precomp)
+                sbytes = lib.gsr_backward_scratch_bytes(P)
+                scratch = torch.empty(sbytes, dtype=torch.uint8, device=device)
+                gr = _lib.Grads(_ptr(dL_dmeans3D), _ptr(dL_dmeans2D), _ptr(dL_dcolors), _ptr(dL_dopacity),
+                                _ptr(dL_dcov3D), _ptr(dL_dsh), _ptr(dL_dscales), _ptr(dL_drotations))
+                st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+                gd = _f32c(grad_depth, device) if ctx.depth_grad and grad_depth is not None else None
+                ga = None if grad_alpha is None else _f32c(grad_alpha, device)
+                dscratch, dbytes, mscratch, mbytes = _masked_scratch(lib, state, ctx, device)
+                _lib.check(lib.gsr_backward_masked(C.byref(s), C.byref(c), state.cap, _ptr(geom), geom.numel(),
+                                                   _ptr(binning), binning.numel(), _ptr(img), img.numel(), _ptr(radii),
+                                                   _ptr(grad_out_color), _ptr(ga), _ptr(gd), _ptr(scratch), sbytes,
+                                                   C.byref(gr), None, _ptr(dscratch), dbytes, _ptr(ctx.grad_mask),
+                                                   _ptr(mscratch), mbytes, st), "gsr_backward_masked")
+                if scales.numel() == 0:  # cov3D_precomp path: the reference leaves these at their zero-fill
+                    dL_dscales.zero_(); dL_drotations.zero_()
+        return (dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D,
+                None, None, None, None, None, None)
+
+
+class _RasterizeGaussiansRawMasked(torch.autograd.Function):
+    """``GaussianRasterizer(grad_mask=...)`` on ``forward_raw``: the forward of _RasterizeGaussiansRaw, the backward
+    through gsr_backward_raw_masked."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
+                raster_settings, depth_grad, deterministic, static, grad_mask):
+        out = _RasterizeGaussiansRaw.forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest,
+                                             log_scales, raw_rotations, raster_settings, depth_grad, deterministic,
+                                             static)
+        ctx.grad_mask = grad_mask
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out_color, grad_radii, grad_depth):
+        lib = _lib.load()
+        rs, state = ctx.raster_settings, ctx.state
+        (means3D, dc, rest, logits, log_scales, raw_rot, radii, geom, binning, img) = ctx.saved_tensors
+        device = means3D.device
+        P, M = state.P, state.M
+        with torch.cuda.device(device):
+            if grad_out_color is None:   # depth_grad: a loss on the depth alone
+                grad_out_color = torch.zeros(3, state.H, state.W, dtype=torch.float32, device=device)
+            grad_out_color = _f32c(grad_out_color, device)
+            f32 = dict(dtype=torch.float32, device=device)
+            d_m3 = torch.empty(P, 3, **f32); d_m2 = torch.empty(P, 3, **f32); d_op = torch.empty(P, 1, **f32)
+            d_dc = torch.empty(P, 1, 3, **f32); d_rest = torch.empty(P, M - 1, 3, **f32)
+            d_sc = torch.empty(P, 3, **f32); d_ro = torch.empty(P, 4, **f32)
+            if P > 0:
+                keep = []
+                s = _make_settings(rs, M, device, keep)
+                rc = _lib.RawCloud(P, _ptr(means3D), _ptr(logits), _ptr(dc), _ptr(rest), _ptr(log_scales), _ptr(raw_rot))
+                gr = _lib.RawGrads(_ptr(d_m3), _ptr(d_m2), _ptr(d_op), _ptr(d_dc), _ptr(d_rest), _ptr(d_sc), _ptr(d_ro))
+                sbytes = lib.gsr_backward_scratch_bytes(P)
+                scratch = torch.empty(sbytes, dtype=torch.uint8, device=device)
+                st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+                gd = _f32c(grad_depth, device) if ctx.depth_grad and grad_depth is not None else None
+                dscratch, dbytes, mscratch, mbytes = _masked_scratch(lib, state, ctx, device)
+                _lib.check(lib.gsr_backward_raw_masked(C.byref(s), C.byref(rc), state.cap, _ptr(geom), geom.numel(),
+                                                       _ptr(binning), binning.numel(), _ptr(img), img.numel(),
+                                                       _ptr(radii), _ptr(grad_out_color), _ptr(gd), _ptr(scratch),
+                                                       sbytes, C.byref(gr), None, _ptr(dscratch), dbytes,
+                                                       _ptr(ctx.grad_mask), _ptr(mscratch), mbytes, st),
+                           "gsr_backward_raw_masked")
+        return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None, None, None
+
+
+def _check_grad_mask(mask, camera_grad, raster_settings):
+    """Constructor checks of ``grad_mask``; returns the mask as uint8 (a bool mask is viewed, not copied)."""
+    if not isinstance(mask, torch.Tensor):
+        raise ValueError(f"grad_mask must be a torch.Tensor, got {type(mask).__name__}")
+    if mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"grad_mask must be a bool or uint8 tensor, got {mask.dtype}")
+    if mask.dim() != 1:
+        raise ValueError(f"grad_mask must be 1-D [P], got shape {tuple(mask.shape)}")
+    if not mask.is_cuda:
+        raise ValueError(f"grad_mask must be on the rasterizer's CUDA device, got {mask.device}")
+    view = getattr(raster_settings, "viewmatrix", None)
+    if isinstance(view, torch.Tensor) and view.is_cuda and view.device != mask.device:
+        raise ValueError(f"grad_mask is on {mask.device}, the camera on {view.device}")
+    if not mask.is_contiguous():
+        raise ValueError("grad_mask must be contiguous")
+    if camera_grad:
+        raise ValueError("grad_mask cannot be combined with camera_grad: the camera gradient sums over every Gaussian")
+    return mask.view(torch.uint8) if mask.dtype == torch.bool else mask
+
+
 def mark_visible(rs, positions):
     """Frustum test of `positions` [P,3] under the camera of `rs` -> bool [P] (GaussianRasterizer.markVisible)."""
     # __init__.py:248-256 / rasterize_points.cu:159-175
@@ -499,7 +634,7 @@ def mark_visible(rs, positions):
 
 class GaussianRasterizer(nn.Module):
     def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False,
-                 deterministic=None, static_capacity=None):
+                 deterministic=None, static_capacity=None, grad_mask=None):
         """``return_alpha=True`` (opt-in, not in the reference) appends a fourth output to ``forward``: the alpha image
         ``1 - final_T`` [1,H,W] (the reference keeps final_T as ``accum_alpha`` but never returns it); it is
         differentiable like the colour.
@@ -523,7 +658,16 @@ class GaussianRasterizer(nn.Module):
         colour = background, depth = 0, alpha = 0 and all gradients zero. Nothing checks this implicitly: call
         ``check_capacity()`` (it synchronises) where a synchronisation is acceptable. Outputs and radii are the same as
         without the option while the capacity suffices; ``apply_weights`` keeps its exact, host-sized path. Not
-        combinable with ``raster_settings.debug`` (which synchronises after every launch)."""
+        combinable with ``raster_settings.debug`` (which synchronises after every launch).
+        ``grad_mask`` (opt-in, for ``forward`` and ``forward_raw``; a bool or uint8 CUDA tensor [P]): only the Gaussians
+        with ``grad_mask[i] != 0`` take gradients. Every gradient row of the others -- means3D, means2D, colours or SH,
+        opacity, scales, rotations, cov3D, or the raw parameters -- is exactly +0.0, and the kernels skip their work
+        (gsr_backward_masked): what GaussianEditor's ``apply_grad_mask`` hooks do after a full backward, but for all
+        parameters, rotations included. The other rows equal the unmasked backward's: bit for bit when deterministic,
+        to the rounding of the float atomics otherwise. The forward is unchanged. Combines with ``return_alpha``,
+        ``depth_grad``, ``deterministic`` and ``static_capacity``; not with ``camera_grad`` (ValueError). The backward
+        reads the tensor given here when it runs: changing it in place between forward and backward is the caller's
+        business, as it is for the hooks."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_alpha = bool(return_alpha)
@@ -537,6 +681,16 @@ class GaussianRasterizer(nn.Module):
             static_capacity = int(static_capacity)
         self.static_capacity = static_capacity
         self.status = None   # device int32[2] {num_rendered, overflow} of the last static-capacity call
+        self.grad_mask = None if grad_mask is None else _check_grad_mask(grad_mask, self.camera_grad, raster_settings)
+
+    def _grad_mask(self, means3D):
+        """The uint8 mask for a forward on `means3D`, checked against its device and P."""
+        m = self.grad_mask
+        if m.device != means3D.device:
+            raise ValueError(f"grad_mask is on {m.device}, means3D on {means3D.device}")
+        if m.numel() != means3D.size(0):
+            raise ValueError(f"grad_mask has {m.numel()} entries for P = {means3D.size(0)} Gaussians")
+        return m
 
     def _static(self, device):
         """(capacity, status) for a static-capacity call, or None. Raises before any launch on a debug setting."""
@@ -570,6 +724,10 @@ class GaussianRasterizer(nn.Module):
         and the SH concatenation happen inside the preprocess kernels. Same return tuple as ``forward``."""
         det = self._deterministic()
         static = self._static(means3D.device)
+        if self.grad_mask is not None:
+            return _RasterizeGaussiansRawMasked.apply(means3D, means2D, opacity_logits, features_dc, features_rest,
+                                                      log_scales, raw_rotations, self.raster_settings, self.depth_grad,
+                                                      det, static, self._grad_mask(means3D))
         if static is not None:
             return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
                                                 raw_rotations, self.raster_settings, self.depth_grad, det, static)
@@ -607,6 +765,10 @@ class GaussianRasterizer(nn.Module):
         if cov3D_precomp is None:
             cov3D_precomp = empty
 
+        if self.grad_mask is not None:
+            return _RasterizeGaussiansMasked.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
+                                                   cov3D_precomp, raster_settings, self.return_alpha, self.depth_grad,
+                                                   self._deterministic(), static, self._grad_mask(means3D))
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                    cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad, self.depth_grad,
                                    self._deterministic(), static)

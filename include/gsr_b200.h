@@ -332,6 +332,35 @@ GSR_API int gsr_backward_raw_deterministic(const gsr_settings* s, const gsr_raw_
                                    void* scratch, size_t scratch_bytes, const gsr_raw_grads* grads, void* det_scratch,
                                    size_t det_scratch_bytes, void* stream);
 
+/* ---- masked backward (opt-in; gradients only for the Gaussians under edit) -----------------------------------
+ * grad_mask [P] (one byte per Gaussian, device memory): every per-Gaussian gradient of a Gaussian with grad_mask[i] == 0
+ * is written as +0.0 (means3D, means2D, colours or SH, opacity, cov3D, scales, rotations; on the raw entry point every
+ * raw-parameter gradient). The rows with grad_mask[i] != 0 are those of the unmasked backward: bit for bit with
+ * det_scratch (deterministic mode), to the rounding of the float atomics without it. The blending backward skips the
+ * work of unedited Gaussians: their splats only advance the pixel state, each tile's walk stops at its front-most
+ * edited instance, and tiles without one are not walked. The preprocess backward treats them as culled.
+ * gsr_backward_masked takes the arguments of gsr_backward_deterministic, plus grad_mask and mask_scratch (at least
+ * gsr_grad_mask_scratch_bytes(W, H) bytes of device memory, contents irrelevant); det_scratch may be NULL (the default,
+ * atomic kernels), dL_dout_alpha and dL_dout_depth may be NULL, camera must be NULL (the camera gradient sums over every
+ * Gaussian). gsr_backward_raw_masked is the same for gsr_backward_raw_deterministic (fused activations). A NULL
+ * grad_mask or a non-NULL camera returns GSR_ERR_INVALID. The forward is unchanged. */
+GSR_API size_t gsr_grad_mask_scratch_bytes(int32_t image_width, int32_t image_height);
+GSR_API int gsr_backward_masked(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered, const void* geometry,
+                        size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
+                        size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                        const float* dL_dout_alpha /* may be NULL */, const float* dL_dout_depth /* may be NULL */,
+                        void* scratch, size_t scratch_bytes, const gsr_grads* grads,
+                        const gsr_camera_grads* camera /* must be NULL */, void* det_scratch /* may be NULL */,
+                        size_t det_scratch_bytes, const uint8_t* grad_mask, void* mask_scratch,
+                        size_t mask_scratch_bytes, void* stream);
+GSR_API int gsr_backward_raw_masked(const gsr_settings* s, const gsr_raw_cloud* c, int32_t num_rendered,
+                            const void* geometry, size_t geometry_bytes, const void* binning, size_t binning_bytes,
+                            const void* image, size_t image_bytes, const int32_t* radii, const float* dL_dout_color,
+                            const float* dL_dout_depth /* may be NULL */, void* scratch, size_t scratch_bytes,
+                            const gsr_raw_grads* grads, const gsr_camera_grads* camera /* must be NULL */,
+                            void* det_scratch /* may be NULL */, size_t det_scratch_bytes, const uint8_t* grad_mask,
+                            void* mask_scratch, size_t mask_scratch_bytes, void* stream);
+
 /* ---- Gaussian-sharded multi-GPU path (BASELINE config 4; SURVEY.md 8(e)) ----------------------------------
  * The reference has no multi-GPU rasterizer; these entry points split the single-GPU pipeline at the two places
  * where the Gaussian-index decomposition (preprocess, fused preprocess backward) meets the tile decomposition
