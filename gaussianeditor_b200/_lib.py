@@ -42,6 +42,10 @@ SYMBOLS = [
     "gsr_shard_order_static", "gsr_sparse_order_static", "gsr_shard_render_static", "gsr_shard_static_gate",
     "gsr_peer_barrier_device",
     "gsr_grad_mask_scratch_bytes", "gsr_backward_masked", "gsr_backward_raw_masked",
+    "gsr_shard_preprocess_masked", "gsr_shard_preprocess_raw_masked", "gsr_shard_preprocess_p2p_masked",
+    "gsr_shard_preprocess_p2p_raw_masked", "gsr_sparse_preprocess_masked", "gsr_sparse_preprocess_raw_masked",
+    "gsr_shard_backward_render_masked", "gsr_shard_backward_preprocess_masked", "gsr_shard_backward_preprocess_raw_masked",
+    "gsr_sparse_backward_preprocess_masked", "gsr_sparse_backward_preprocess_raw_masked",
 ]
 
 
@@ -299,6 +303,32 @@ def load():
     lib.gsr_backward_raw_masked.restype = C.c_int
     lib.gsr_backward_raw_masked.argtypes = [S, RC, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, sz, RG, CG, vp, sz, vp,
                                             vp, sz, vp]
+    u8 = vp  # grad_mask: device bytes
+    lib.gsr_shard_preprocess_masked.restype = C.c_int
+    lib.gsr_shard_preprocess_masked.argtypes = [S, Cl, i32, i32, i32, vp, sz, vp, u8, vp]
+    lib.gsr_shard_preprocess_raw_masked.restype = C.c_int
+    lib.gsr_shard_preprocess_raw_masked.argtypes = [S, RC, i32, i32, i32, vp, sz, vp, u8, vp]
+    lib.gsr_shard_preprocess_p2p_masked.restype = C.c_int
+    lib.gsr_shard_preprocess_p2p_masked.argtypes = [S, Cl, i32, i32, i32, C.POINTER(vp), i32, i32, sz, vp, u8, vp]
+    lib.gsr_shard_preprocess_p2p_raw_masked.restype = C.c_int
+    lib.gsr_shard_preprocess_p2p_raw_masked.argtypes = [S, RC, i32, i32, i32, C.POINTER(vp), i32, i32, sz, vp, u8, vp]
+    lib.gsr_sparse_preprocess_masked.restype = C.c_int
+    lib.gsr_sparse_preprocess_masked.argtypes = [S, Cl, SP, vp, sz, vp, C.POINTER(vp), sz, vp, u8, vp]
+    lib.gsr_sparse_preprocess_raw_masked.restype = C.c_int
+    lib.gsr_sparse_preprocess_raw_masked.argtypes = [S, RC, SP, vp, sz, vp, C.POINTER(vp), sz, vp, u8, vp]
+    lib.gsr_shard_backward_render_masked.restype = C.c_int
+    lib.gsr_shard_backward_render_masked.argtypes = [S, TO, i32, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, sz, vp, sz,
+                                                     vp, sz, vp]
+    lib.gsr_shard_backward_preprocess_masked.restype = C.c_int
+    lib.gsr_shard_backward_preprocess_masked.argtypes = [S, Cl, i32, i32, vp, sz, vp, vp, C.POINTER(Grads), i32, CG, u8,
+                                                         vp]
+    lib.gsr_shard_backward_preprocess_raw_masked.restype = C.c_int
+    lib.gsr_shard_backward_preprocess_raw_masked.argtypes = [S, RC, i32, i32, vp, sz, vp, vp, RG, i32, u8, vp]
+    lib.gsr_sparse_backward_preprocess_masked.restype = C.c_int
+    lib.gsr_sparse_backward_preprocess_masked.argtypes = [S, Cl, SP, vp, sz, vp, vp, sz, vp, sz, C.POINTER(Grads), i32,
+                                                          CG, u8, vp]
+    lib.gsr_sparse_backward_preprocess_raw_masked.restype = C.c_int
+    lib.gsr_sparse_backward_preprocess_raw_masked.argtypes = [S, RC, SP, vp, sz, vp, vp, sz, vp, sz, RG, i32, u8, vp]
     if lib.gsr_abi_version() != 2:
         raise RuntimeError("libgsr_b200.so ABI version mismatch")
     _lib = lib

@@ -135,6 +135,15 @@ int check_shard_camera(const gsr_camera_grads* cam, int P) {
   return GSR_OK;
 }
 
+int check_mask_args(const uint8_t* grad_mask, const gsr_camera_grads* cam) {
+  if (cam) {
+    set_error("camera gradients sum over every Gaussian: they cannot be combined with a gradient mask (camera must be null)");
+    return GSR_ERR_INVALID;
+  }
+  if (!grad_mask) { set_error("grad_mask is null"); return GSR_ERR_INVALID; }
+  return GSR_OK;
+}
+
 int zero_shard_camera(const gsr_camera_grads* cam, cudaStream_t st) {
   cudaError_t e = cudaMemsetAsync(cam->dL_dviewmatrix, 0, 16 * sizeof(float), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(cam->dL_dprojmatrix, 0, 16 * sizeof(float), st);
@@ -612,15 +621,6 @@ int gsr_backward_raw_deterministic(const gsr_settings* s, const gsr_raw_cloud* r
 // ---- masked backward: gradients only for the Gaussians with grad_mask[i] != 0 ----------------------------------
 size_t gsr_grad_mask_scratch_bytes(int32_t W, int32_t H) { return grad_mask_first_bytes(W > 0 ? W : 0, H > 0 ? H : 0); }
 
-static int check_mask_args(const uint8_t* grad_mask, const gsr_camera_grads* cam) {
-  if (cam) {
-    set_error("camera gradients sum over every Gaussian: they cannot be combined with a gradient mask (camera must be null)");
-    return GSR_ERR_INVALID;
-  }
-  if (!grad_mask) { set_error("grad_mask is null"); return GSR_ERR_INVALID; }
-  return GSR_OK;
-}
-
 int gsr_backward_masked(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry,
                         size_t geometry_bytes, const void* binning, size_t binning_bytes, const void* image,
                         size_t image_bytes, const int32_t* radii, const float* dL_dout_color, const float* dL_dout_alpha,
@@ -680,10 +680,12 @@ int gsr_view_exchange(void* geometry, int32_t P_total, gsr_exchange_view* out) {
   return GSR_OK;
 }
 
-// gsr_shard_preprocess and, with `raw`, gsr_shard_preprocess_raw (`shard` unused)
+// gsr_shard_preprocess and, with `raw`, gsr_shard_preprocess_raw (`shard` unused); with `grad_mask` their masked
+// twins, whose records carry the edit word
 static int shard_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
                                  int32_t P_total, int32_t index_base, int32_t slice_len, void* geometry,
-                                 size_t geometry_bytes, int32_t* radii_total, void* stream) {
+                                 size_t geometry_bytes, int32_t* radii_total, void* stream,
+                                 const uint8_t* grad_mask = nullptr) {
   gsr_cloud c;
   int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
@@ -699,7 +701,7 @@ static int shard_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, 
   StageScope t(ST_PRE_FWD, st);
   if (c.P > 0) {
     rc = launch_preprocess_fwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, st, nullptr, 0,
-                               raw != nullptr, raw ? raw->features_rest : nullptr);
+                               raw != nullptr, raw ? raw->features_rest : nullptr, false, grad_mask);
     if (rc) return rc;
   }
   const int pad = slice_len - c.P;  // slots of the slice behind the shard: culled (radius 0 in the record)
@@ -721,6 +723,24 @@ int gsr_shard_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard, 
                              void* stream) {
   return shard_preprocess_impl(s, nullptr, shard, P_total, index_base, slice_len, geometry, geometry_bytes, radii_total,
                                stream);
+}
+
+int gsr_shard_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
+                                int32_t slice_len, void* geometry, size_t geometry_bytes, int32_t* radii_total,
+                                const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return shard_preprocess_impl(s, shard, nullptr, P_total, index_base, slice_len, geometry, geometry_bytes, radii_total,
+                               stream, grad_mask);
+}
+
+int gsr_shard_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                    int32_t index_base, int32_t slice_len, void* geometry, size_t geometry_bytes,
+                                    int32_t* radii_total, const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return shard_preprocess_impl(s, nullptr, shard, P_total, index_base, slice_len, geometry, geometry_bytes, radii_total,
+                               stream, grad_mask);
 }
 
 int gsr_peer_alloc(size_t bytes, void** ptr_out, void* handle_out) {
@@ -750,11 +770,12 @@ int gsr_peer_open(const void* handle, void** ptr_out) {
 int gsr_peer_close(void* ptr) { return ptr ? check_cuda(cudaIpcCloseMemHandle(ptr), "cudaIpcCloseMemHandle") : GSR_OK; }
 int gsr_peer_free(void* ptr) { return ptr ? check_cuda(cudaFree(ptr), "peer_free") : GSR_OK; }
 
-// gsr_shard_preprocess_p2p and, with `raw`, gsr_shard_preprocess_p2p_raw (`shard` unused)
+// gsr_shard_preprocess_p2p and, with `raw`, gsr_shard_preprocess_p2p_raw (`shard` unused); with `grad_mask` their
+// masked twins
 static int shard_preprocess_p2p_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
                                      int32_t P_total, int32_t index_base, int32_t slice_len, void* const* peer_geometry,
                                      int32_t world, int32_t rank, size_t geometry_bytes, int32_t* radii_total,
-                                     void* stream) {
+                                     void* stream, const uint8_t* grad_mask = nullptr) {
   gsr_cloud c;
   int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
@@ -780,7 +801,7 @@ static int shard_preprocess_p2p_impl(const gsr_settings* s, const gsr_cloud* sha
   StageScope t(ST_PRE_FWD, st);
   if (c.P > 0) {
     rc = launch_preprocess_fwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, st, dst, world,
-                               raw != nullptr, raw ? raw->features_rest : nullptr);
+                               raw != nullptr, raw ? raw->features_rest : nullptr, false, grad_mask);
     if (rc) return rc;
   }
   const int pad = slice_len - c.P;
@@ -803,6 +824,26 @@ int gsr_shard_preprocess_p2p_raw(const gsr_settings* s, const gsr_raw_cloud* sha
                                  size_t geometry_bytes, int32_t* radii_total, void* stream) {
   return shard_preprocess_p2p_impl(s, nullptr, shard, P_total, index_base, slice_len, peer_geometry, world, rank,
                                    geometry_bytes, radii_total, stream);
+}
+
+int gsr_shard_preprocess_p2p_masked(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
+                                    int32_t slice_len, void* const* peer_geometry, int32_t world, int32_t rank,
+                                    size_t geometry_bytes, int32_t* radii_total, const uint8_t* grad_mask,
+                                    void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return shard_preprocess_p2p_impl(s, shard, nullptr, P_total, index_base, slice_len, peer_geometry, world, rank,
+                                   geometry_bytes, radii_total, stream, grad_mask);
+}
+
+int gsr_shard_preprocess_p2p_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                        int32_t index_base, int32_t slice_len, void* const* peer_geometry,
+                                        int32_t world, int32_t rank, size_t geometry_bytes, int32_t* radii_total,
+                                        const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return shard_preprocess_p2p_impl(s, nullptr, shard, P_total, index_base, slice_len, peer_geometry, world, rank,
+                                   geometry_bytes, radii_total, stream, grad_mask);
 }
 
 // gsr_shard_order and, with num_rendered_host == nullptr, gsr_shard_order_static (R stays on the device)
@@ -932,7 +973,7 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
                                       size_t binning_bytes, const void* image, size_t image_bytes,
                                       const float* dL_dout_color, void* acc_total, size_t acc_bytes, void* stream,
                                       const DetScratch* ds, const float* dL_dout_depth = nullptr,
-                                      const float* dL_dout_alpha = nullptr) {
+                                      const float* dL_dout_alpha = nullptr, const MaskScratch* ms = nullptr) {
   int rc = check_settings(s);
   if (rc) return rc;
   TileOwner own;
@@ -943,6 +984,8 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
   if (!acc_total || acc_bytes < need) { set_error("accumulators too small: %zu < %zu", acc_bytes, need); return GSR_ERR_WORKSPACE; }
   DetWS det;
   if (ds && (rc = carve_det_checked(*ds, P_total, R, 0, det))) return rc;
+  GradMaskWS gm;
+  if (ms && (rc = carve_mask_checked(*ms, *s, gm))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   gsr_cloud c{};
   c.P = P_total;
@@ -957,7 +1000,23 @@ static int shard_backward_render_impl(const gsr_settings* s, const gsr_tile_owne
   }
   if (R == 0) return GSR_OK;
   return launch_render_bwd(*s, g, b, im, dL_dout_color, (float*)acc_total, st, own, dL_dout_alpha, dL_dout_depth,
-                           ds ? &det : nullptr, P_total, R);
+                           ds ? &det : nullptr, P_total, R, ms ? &gm : nullptr);
+}
+
+// The masked blend backward of a tile owner: the edit bits are the records' edit words, written by the masked preprocess
+// twins on the ranks that own the Gaussians, so one entry point serves the dense and the sparse workspaces alike.
+int gsr_shard_backward_render_masked(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
+                                     const void* geometry, size_t geometry_bytes, const void* binning,
+                                     size_t binning_bytes, const void* image, size_t image_bytes,
+                                     const float* dL_dout_color, const float* dL_dout_alpha,
+                                     const float* dL_dout_depth, void* acc_total, size_t acc_bytes, void* det_scratch,
+                                     size_t det_scratch_bytes, void* mask_scratch, size_t mask_scratch_bytes,
+                                     void* stream) {
+  const DetScratch ds{det_scratch, det_scratch_bytes};
+  const MaskScratch ms{nullptr, mask_scratch, mask_scratch_bytes};
+  return shard_backward_render_impl(s, owner, P_total, R, geometry, geometry_bytes, binning, binning_bytes, image,
+                                    image_bytes, dL_dout_color, acc_total, acc_bytes, stream,
+                                    det_scratch ? &ds : nullptr, dL_dout_depth, dL_dout_alpha, &ms);
 }
 
 int gsr_shard_backward_render_alpha(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total, int32_t R,
@@ -1084,7 +1143,7 @@ static int shard_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud
                                           int32_t P_total, int32_t index_base, const void* geometry,
                                           size_t geometry_bytes, const int32_t* radii_total, const void* acc_slice,
                                           const gsr_grads* gr, const gsr_raw_grads* rgr, bool depth, void* stream,
-                                          const gsr_camera_grads* cam = nullptr) {
+                                          const gsr_camera_grads* cam = nullptr, const uint8_t* grad_mask = nullptr) {
   gsr_cloud c;
   int rc = shard_cloud(s, shard, raw, c);
   if (rc) return rc;
@@ -1111,7 +1170,7 @@ static int shard_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud
   if (raw) {
     const RawBackward rb{raw->features_rest, rgr->dL_dfeatures_rest};
     return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, (const float*)acc_slice,
-                                 raw_grads_as_full(*rgr), st, &rb, nullptr, depth);
+                                 raw_grads_as_full(*rgr), st, &rb, nullptr, depth, grad_mask);
   }
   if (cam) {
     const CameraBackward cb{cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos, (float*)cam->scratch};
@@ -1119,7 +1178,7 @@ static int shard_backward_preprocess_impl(const gsr_settings* s, const gsr_cloud
                                  (const float*)acc_slice, *gr, st, nullptr, &cb, depth);
   }
   return launch_preprocess_bwd(*s, c, slice_geometry(g, index_base), radii_total + index_base, (const float*)acc_slice,
-                               *gr, st, nullptr, nullptr, depth);
+                               *gr, st, nullptr, nullptr, depth, grad_mask);
 }
 
 int gsr_shard_backward_preprocess_camera(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
@@ -1152,6 +1211,29 @@ int gsr_shard_backward_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud
                                       int32_t depth, void* stream) {
   return shard_backward_preprocess_impl(s, nullptr, shard, P_total, index_base, geometry, geometry_bytes, radii_total,
                                         acc_slice, nullptr, gr, depth != 0, stream);
+}
+
+// masked twins: the shard's slice geometry is indexed locally, so grad_mask holds the shard's own rows [shard.P]
+int gsr_shard_backward_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                         int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                         const int32_t* radii_total, const void* acc_slice, const gsr_grads* gr,
+                                         int32_t depth, const gsr_camera_grads* camera, const uint8_t* grad_mask,
+                                         void* stream) {
+  const int rc = check_mask_args(grad_mask, camera);
+  if (rc) return rc;
+  return shard_backward_preprocess_impl(s, shard, nullptr, P_total, index_base, geometry, geometry_bytes, radii_total,
+                                        acc_slice, gr, nullptr, depth != 0, stream, nullptr, grad_mask);
+}
+
+int gsr_shard_backward_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                             int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                             const int32_t* radii_total, const void* acc_slice,
+                                             const gsr_raw_grads* gr, int32_t depth, const uint8_t* grad_mask,
+                                             void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return shard_backward_preprocess_impl(s, nullptr, shard, P_total, index_base, geometry, geometry_bytes, radii_total,
+                                        acc_slice, nullptr, gr, depth != 0, stream, nullptr, grad_mask);
 }
 
 int gsr_view_geometry(const void* geometry, int32_t P, gsr_geometry_view* out) {

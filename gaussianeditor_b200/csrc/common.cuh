@@ -21,8 +21,11 @@ constexpr int TILE_PIX = TILE * TILE;
 // Per-Gaussian "splat record": everything the two render kernels need about a projected Gaussian, packed
 // into 48 contiguous, 16-byte-aligned bytes so that one tile-list gather is three 128-bit loads
 // (the reference gathers from five separate arrays: means2D, conic_opacity, rgb, depths, point ids).
-//   q0 = { x, y, conic.a, conic.b }      q1 = { conic.c, opacity, view-depth, <unused> }
+//   q0 = { x, y, conic.a, conic.b }      q1 = { conic.c, opacity, view-depth, edit word }
 //   q2 = { r, g, b, radius (int bits; 0 = culled, the only field a culled record defines) }
+// The edit word is 0 except from the masked preprocess forms (gsr_shard_preprocess_masked and its twins), which write
+// GRAD_MASK_EDIT for an edited Gaussian; only the masked backward of a tile owner reads it. Every other kernel ignores
+// q1.w (the render and tracing kernels overwrite it in their staged copies).
 struct __align__(16) SplatRecord {
   float4 q0, q1, q2;
 };
@@ -166,6 +169,8 @@ int shard_cloud(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_clo
 int check_shard_camera(const gsr_camera_grads* cam, int P);
 // writes this rank's zero partial (a shard without Gaussians: no preprocess backward runs)
 int zero_shard_camera(const gsr_camera_grads* cam, cudaStream_t st);
+// the arguments every masked entry point checks first: a mask, and no camera gradients (they sum over every Gaussian)
+int check_mask_args(const uint8_t* grad_mask, const gsr_camera_grads* cam);
 
 // ---- stage entry points (host side; each file owns its kernels) ------------------------------------------
 // peer_records/npeers: fused all-gather of the sharded path (every rank's view of this shard's record slice), else 0
@@ -173,7 +178,9 @@ int zero_shard_camera(const gsr_camera_grads* cam, cudaStream_t st);
 // c.shs is features_dc [P,1,3] and features_rest [P,M-1,3] holds the other coefficients (may be null when M == 1).
 int launch_preprocess_fwd(const gsr_settings& s, const gsr_cloud& c, const GeometryWS& g, int32_t* radii,
                           cudaStream_t st, SplatRecord* const* peer_records = nullptr, int npeers = 0, bool raw = false,
-                          const float* features_rest = nullptr, bool count_tiles = false);
+                          const float* features_rest = nullptr, bool count_tiles = false,
+                          const uint8_t* grad_mask = nullptr);
+// grad_mask != nullptr: the masked forms, which write GRAD_MASK_EDIT into q1.w of an edited Gaussian's record
 // depth_sort.cu: depth order + offsets scan without CUB; scratch lives in GeometryWS::cub_temp
 size_t depth_sort_scratch_bytes(int P);
 int run_depth_sort_own(int P, const GeometryWS& g, cudaStream_t st, bool debug);
@@ -216,8 +223,9 @@ int launch_render_fwd(const gsr_settings& s, const GeometryWS& g, const BinningW
 // 1-based list position of the tile's front-most edited instance (GRAD_MASK_NONE: the tile has none), written by
 // grad_mask_first_kernel ahead of render_bwd; gsr_grad_mask_scratch_bytes(W, H) holds it.
 constexpr uint32_t GRAD_MASK_NONE = 0xffffffffu;
+constexpr uint32_t GRAD_MASK_EDIT = 1u;  // the edit word (SplatRecord q1.w) of an edited Gaussian's record
 struct GradMaskWS {
-  const uint8_t* mask;  // [P]
+  const uint8_t* mask;  // [P]; null: the edit bits are the records' edit words (a sharded tile owner's lists)
   uint32_t* first;      // [Ntile]
 };
 size_t grad_mask_first_bytes(int W, int H);  // first[] of a W x H frame (gsr_grad_mask_scratch_bytes)

@@ -62,7 +62,7 @@ template <class Base> struct BwdDetArgs : Base {
 // Arguments of the masked instantiations (MASK, gsr_backward_masked): which Gaussians take gradients, and where each
 // tile's walk may stop (grad_mask_first_kernel).
 template <class Base> struct BwdMaskArgs : Base {
-  const uint8_t* grad_mask;  // [P] nonzero: the Gaussian is edited
+  const uint8_t* grad_mask;  // [P] nonzero: the Gaussian is edited (unused by render_bwd_recmask_kernel)
   const uint32_t* first;     // [Ntile] 1-based position of the front-most edited instance, GRAD_MASK_NONE if none
 };
 template <bool DEPTH, bool DET = false>
@@ -467,10 +467,12 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
 // unedited Gaussian is evaluated as usual, but its hits only advance the pixel state (state_update): no column, no batch
 // slot, no flush, no row or flag. The walk stops at the tile's front-most edited position (a.first), and a warp or tile
 // without an edited instance in its range returns at once.
+// MASKREC (with MASK): the edit bit is the record's edit word q1.w (preprocess_fwd_masked_kernel) instead of grad_mask[id],
+// taken by the staging lane from the q1 it has already loaded, before q1.w becomes the sub-block mask.
 template <int NSB, int MINB, bool SKIP = false, bool MASKSKIP = false, bool BATCHED = false, bool DEPTH = false,
           bool DET = false>
 __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_flat_kernel(const BwdArgsT<DEPTH, DET> a, const int ntiles) {
-  constexpr bool MASK = false;
+  constexpr bool MASK = false, MASKREC = false;
 #include "render_bwd_flat_body.inc"
 }
 // MASK form of variant 15 (gsr_backward_masked), with DEPTH / DET as render_bwd_flat_kernel. A kernel of its own name
@@ -479,7 +481,17 @@ template <int MINB, bool DEPTH, bool DET>
 __global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_masked_kernel(const BwdMaskArgs<BwdArgsT<DEPTH, DET>> a,
                                                                                 const int ntiles) {
   constexpr int NSB = 4;
-  constexpr bool SKIP = true, MASKSKIP = false, BATCHED = true, MASK = true;
+  constexpr bool SKIP = true, MASKSKIP = false, BATCHED = true, MASK = true, MASKREC = false;
+#include "render_bwd_flat_body.inc"
+}
+// MASKREC form of render_bwd_masked_kernel for a tile owner of the Gaussian-sharded path (gsr_shard_backward_render_masked):
+// a list entry is a global index (dense) or a candidate slot (sparse), so no per-rank mask can be indexed by it; the
+// record carries the bit instead. a.grad_mask is unused.
+template <int MINB, bool DEPTH, bool DET>
+__global__ void __launch_bounds__(BW_WARPS * 32, MINB) render_bwd_recmask_kernel(const BwdMaskArgs<BwdArgsT<DEPTH, DET>> a,
+                                                                                 const int ntiles) {
+  constexpr int NSB = 4;
+  constexpr bool SKIP = true, MASKSKIP = false, BATCHED = true, MASK = true, MASKREC = true;
 #include "render_bwd_flat_body.inc"
 }
 
@@ -580,6 +592,34 @@ __global__ void __launch_bounds__(BW_WARPS * 32) grad_mask_first_kernel(const ui
   if (lane == 0) first[tile] = f;
 }
 
+// grad_mask_first_kernel for a tile owner of the Gaussian-sharded path: warp n walks the n-th OWNED tile (owned_tile, as
+// the masked walk reads first[]), and an instance is edited when its record's edit word q1.w is nonzero. The entries of
+// the tiles this rank does not own are neither read nor written.
+__global__ void __launch_bounds__(BW_WARPS * 32) grad_mask_first_owner_kernel(const uint2* __restrict__ ranges,
+                                                                              const uint32_t* __restrict__ point_list,
+                                                                              const uint32_t* __restrict__ tile_last,
+                                                                              const SplatRecord* __restrict__ records,
+                                                                              uint32_t* __restrict__ first, int ntiles,
+                                                                              int gx, int own_stride, int own_phase) {
+  const int lane = threadIdx.x & 31;
+  const int n_own = blockIdx.x * BW_WARPS + (threadIdx.x >> 5);
+  if (n_own >= ntiles) return;
+  const int tile = owned_tile(n_own, gx, own_stride, own_phase);
+  const uint2 range = ranges[tile];
+  const uint32_t n = min(tile_last[tile], range.y > range.x ? range.y - range.x : 0u);
+  uint32_t f = GRAD_MASK_NONE;
+  for (uint32_t b = 0; b < n; b += 32) {
+    const uint32_t i = b + lane;
+    const bool e = i < n && __float_as_uint(__ldg(&records[__ldg(point_list + range.x + i)].q1.w)) != 0;
+    const uint32_t hit = __ballot_sync(0xffffffffu, e);
+    if (hit) {
+      f = b + (uint32_t)__ffs(hit);
+      break;
+    }
+  }
+  if (lane == 0) first[tile] = f;
+}
+
 }  // namespace
 
 size_t grad_mask_first_bytes(int W, int H) {
@@ -587,12 +627,26 @@ size_t grad_mask_first_bytes(int W, int H) {
   return align_up((ntiles > 0 ? ntiles : 1) * sizeof(uint32_t));
 }
 
-// The masked walk: first[] of every tile, then one of the four MASK instantiations of variant 15. 4 CTAs/SM for all four
-// except the atomic colour kernel, which keeps the default's 5 (see DESIGN.md section 3 for the register counts).
+// one MASK instantiation of variant 15: edit bits from grad_mask (single GPU) or from the records (gm.mask == null)
+template <int MINB, bool DEPTH, bool DET>
+static void launch_masked_form(const BwdMaskArgs<BwdArgsT<DEPTH, DET>>& ma, int blocks, int ntiles, cudaStream_t st) {
+  if (ma.grad_mask != nullptr)
+    render_bwd_masked_kernel<MINB, DEPTH, DET><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+  else
+    render_bwd_recmask_kernel<MINB, DEPTH, DET><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+}
+
+// The masked walk: first[] of every (owned) tile, then one of the four MASK instantiations of variant 15. 4 CTAs/SM for
+// all four except the atomic colour kernel, which keeps the default's 5 (see DESIGN.md section 3 for the register counts).
+// gm.mask == null: a tile owner of the sharded path, whose edit bits are the records' edit words.
 static int launch_render_bwd_masked(const BwdArgs& a, int ntiles, const float* dL_ddepth, const DetWS* det,
                                     const GradMaskWS& gm, bool debug, cudaStream_t st) {
-  grad_mask_first_kernel<<<(ntiles + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(
-      a.ranges, a.point_list, a.tile_last, gm.mask, gm.first, ntiles);
+  if (gm.mask != nullptr)
+    grad_mask_first_kernel<<<(ntiles + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(
+        a.ranges, a.point_list, a.tile_last, gm.mask, gm.first, ntiles);
+  else
+    grad_mask_first_owner_kernel<<<(ntiles + BW_WARPS - 1) / BW_WARPS, BW_WARPS * 32, 0, st>>>(
+        a.ranges, a.point_list, a.tile_last, a.records, gm.first, ntiles, a.gx, a.own_stride, a.own_phase);
   g_launches++;
   int rc = check_launch("grad_mask_first", debug, st);
   if (rc) return rc;
@@ -608,25 +662,25 @@ static int launch_render_bwd_masked(const BwdArgs& a, int ntiles, const float* d
       ma.dL_ddepth = dL_ddepth;
       ma.excl = det->excl; ma.rows = det->rows; ma.flags = det->flags;
       fill(ma);
-      render_bwd_masked_kernel<4, true, true><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+      launch_masked_form<4, true, true>(ma, blocks, ntiles, st);
     } else {
       BwdMaskArgs<BwdDetArgs<BwdArgs>> ma;
       static_cast<BwdArgs&>(ma) = a;
       ma.excl = det->excl; ma.rows = det->rows; ma.flags = det->flags;
       fill(ma);
-      render_bwd_masked_kernel<4, false, true><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+      launch_masked_form<4, false, true>(ma, blocks, ntiles, st);
     }
   } else if (dL_ddepth != nullptr) {
     BwdMaskArgs<BwdDepthArgs> ma;
     static_cast<BwdArgs&>(ma) = a;
     ma.dL_ddepth = dL_ddepth;
     fill(ma);
-    render_bwd_masked_kernel<4, true, false><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+    launch_masked_form<4, true, false>(ma, blocks, ntiles, st);
   } else {
     BwdMaskArgs<BwdArgs> ma;
     static_cast<BwdArgs&>(ma) = a;
     fill(ma);
-    render_bwd_masked_kernel<5, false, false><<<blocks, BW_WARPS * 32, 0, st>>>(ma, ntiles);
+    launch_masked_form<5, false, false>(ma, blocks, ntiles, st);
   }
   g_launches++;
   return check_launch("render_bwd (masked)", debug, st);
@@ -645,7 +699,7 @@ int launch_render_bwd(const gsr_settings& s, const GeometryWS& g, const BinningW
   a.bg = s.bg; a.final_T = im.final_T; a.n_contrib = im.n_contrib; a.dL_dpix = dL_dpix; a.acc = acc;
   const int ntiles = a.gx * own.owned_rows(a.gy);  // tiles this rank walks (all of them when own = {1,0})
   if (ntiles == 0) return GSR_OK;
-  if (gm != nullptr) {  // masked backward (single-GPU entry points only): variant 15, atomic or deterministic
+  if (gm != nullptr) {  // masked backward: variant 15, atomic or deterministic
     int rc = det ? launch_det_prepare(P, R, 2, g, *det, st) : GSR_OK;
     if (rc) return rc;
     if ((rc = launch_render_bwd_masked(a, ntiles, dL_ddepth, det, *gm, s.debug != 0, st))) return rc;

@@ -542,10 +542,12 @@ size_t gsr_sparse_candidate_bytes(int32_t world, int32_t seg_cap) {
   return sc.total;
 }
 
-// gsr_sparse_preprocess and, with `raw`, gsr_sparse_preprocess_raw (`shard` unused)
+// gsr_sparse_preprocess and, with `raw`, gsr_sparse_preprocess_raw (`shard` unused); with `grad_mask` their masked
+// twins: the masked preprocess writes the records' edit words, and the push carries them with the records
 static int sparse_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard, const gsr_raw_cloud* raw,
                                   const gsr_sparse_plan* plan, void* local_ws, size_t local_bytes, int32_t* radii_local,
-                                  void* const* peer_cand, size_t cand_bytes, int32_t* counts_row, void* stream) {
+                                  void* const* peer_cand, size_t cand_bytes, int32_t* counts_row, void* stream,
+                                  const uint8_t* grad_mask = nullptr) {
   int rc = check_plan(plan);
   if (rc) return rc;
   const int32_t P = raw ? raw->P : (shard ? shard->P : -1);
@@ -575,7 +577,8 @@ static int sparse_preprocess_impl(const gsr_settings* s, const gsr_cloud* shard,
   if (n == 0) return check_cuda(cudaMemsetAsync(counts_row, 0, GSR_MAX_PEERS * sizeof(int32_t), st), "counts memset");
   {
     StageScope t(ST_PRE_FWD, st);
-    rc = launch_preprocess_fwd(*s, c, g, radii_local, st, nullptr, 0, raw != nullptr, raw ? raw->features_rest : nullptr);
+    rc = launch_preprocess_fwd(*s, c, g, radii_local, st, nullptr, 0, raw != nullptr, raw ? raw->features_rest : nullptr,
+                               false, grad_mask);
     if (rc) return rc;
     const int nblocks = (n + SP_THREADS - 1) / SP_THREADS;
     sparse_mask_kernel<<<nblocks, SP_THREADS, 0, st>>>(n, g.records, gx, gy, plan->world, sl.dest_mask, sl.blk_base);
@@ -599,6 +602,24 @@ int gsr_sparse_preprocess_raw(const gsr_settings* s, const gsr_raw_cloud* shard,
                               size_t cand_bytes, int32_t* counts_row, void* stream) {
   return sparse_preprocess_impl(s, nullptr, shard, plan, local_ws, local_bytes, radii_local, peer_cand, cand_bytes,
                                 counts_row, stream);
+}
+
+int gsr_sparse_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
+                                 void* local_ws, size_t local_bytes, int32_t* radii_local, void* const* peer_cand,
+                                 size_t cand_bytes, int32_t* counts_row, const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return sparse_preprocess_impl(s, shard, nullptr, plan, local_ws, local_bytes, radii_local, peer_cand, cand_bytes,
+                                counts_row, stream, grad_mask);
+}
+
+int gsr_sparse_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, const gsr_sparse_plan* plan,
+                                     void* local_ws, size_t local_bytes, int32_t* radii_local, void* const* peer_cand,
+                                     size_t cand_bytes, int32_t* counts_row, const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return sparse_preprocess_impl(s, nullptr, shard, plan, local_ws, local_bytes, radii_local, peer_cand, cand_bytes,
+                                counts_row, stream, grad_mask);
 }
 
 // gsr_sparse_order and, with host_out == nullptr, gsr_sparse_order_static (no host words: the static forward's status
@@ -682,7 +703,7 @@ static int sparse_backward_preprocess_impl(const gsr_settings* s, const gsr_clou
                                            const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
                                            void* acc_slice, size_t acc_bytes, const gsr_grads* gr,
                                            const gsr_raw_grads* rgr, bool depth, void* stream,
-                                           const gsr_camera_grads* cam = nullptr) {
+                                           const gsr_camera_grads* cam = nullptr, const uint8_t* grad_mask = nullptr) {
   int rc = check_plan(plan);
   if (rc) return rc;
   const int32_t P = raw ? raw->P : (shard ? shard->P : -1);
@@ -728,13 +749,14 @@ static int sparse_backward_preprocess_impl(const gsr_settings* s, const gsr_clou
   if (raw) {
     const RawBackward rb{raw->features_rest, rgr->dL_dfeatures_rest};
     return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, raw_grads_as_full(*rgr), st, &rb,
-                                 nullptr, depth);
+                                 nullptr, depth, grad_mask);
   }
   if (cam) {
     const CameraBackward cb{cam->dL_dviewmatrix, cam->dL_dprojmatrix, cam->dL_dcampos, (float*)cam->scratch};
     return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, *gr, st, nullptr, &cb, depth);
   }
-  return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, *gr, st, nullptr, nullptr, depth);
+  return launch_preprocess_bwd(*s, c, g, radii_local, (const float*)acc_slice, *gr, st, nullptr, nullptr, depth,
+                               grad_mask);
 }
 
 int gsr_sparse_backward_preprocess_camera(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
@@ -769,6 +791,29 @@ int gsr_sparse_backward_preprocess_raw(const gsr_settings* s, const gsr_raw_clou
                                        const gsr_raw_grads* gr, int32_t depth, void* stream) {
   return sparse_backward_preprocess_impl(s, nullptr, shard, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
                                          acc_slice, acc_bytes, nullptr, gr, depth != 0, stream);
+}
+
+// masked twins: the rank's local workspace is indexed by its own rows, so grad_mask holds them [shard.P]
+int gsr_sparse_backward_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
+                                          const void* local_ws, size_t local_bytes, const int32_t* radii_local,
+                                          const void* cand_ws, size_t cand_bytes, void* acc_slice, size_t acc_bytes,
+                                          const gsr_grads* gr, int32_t depth, const gsr_camera_grads* camera,
+                                          const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, camera);
+  if (rc) return rc;
+  return sparse_backward_preprocess_impl(s, shard, nullptr, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
+                                         acc_slice, acc_bytes, gr, nullptr, depth != 0, stream, nullptr, grad_mask);
+}
+
+int gsr_sparse_backward_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard,
+                                              const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,
+                                              const int32_t* radii_local, const void* cand_ws, size_t cand_bytes,
+                                              void* acc_slice, size_t acc_bytes, const gsr_raw_grads* gr, int32_t depth,
+                                              const uint8_t* grad_mask, void* stream) {
+  const int rc = check_mask_args(grad_mask, nullptr);
+  if (rc) return rc;
+  return sparse_backward_preprocess_impl(s, nullptr, shard, plan, local_ws, local_bytes, radii_local, cand_ws, cand_bytes,
+                                         acc_slice, acc_bytes, nullptr, gr, depth != 0, stream, nullptr, grad_mask);
 }
 
 int gsr_sparse_apply_weights_gather(const gsr_sparse_plan* plan, const void* local_ws, size_t local_bytes,

@@ -256,7 +256,7 @@ def sharded_scene(cloud: synth.Cloud, device, plan) -> EditScene:
 
 
 def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0, mode=None, deterministic=False,
-                          group=None, max_densify_percent=0.01, min_opacity=0.005):
+                          group=None, max_densify_percent=0.01, min_opacity=0.005, grad_mask=None):
     """The config-5 step of ``run_edit_loop`` on a Gaussian-sharded cloud, one process per GPU (collective: every rank
     of `group` calls it with the same arguments; the process group must exist, NCCL).
 
@@ -269,16 +269,24 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
     ``optim_surgery`` (clones start with zero moments, kept rows keep theirs: the reference's behaviour), ``rebalance``
     with K = 2 moves rows, Adam state and the mask to their new owners, the statistics restart at zero and the
     rasterizer is re-created for the new size. `mode` and `deterministic` go to the rasterizer.
+    ``grad_mask`` trains under the mask as ``run_edit_loop`` does: ``"hooks"`` registers ``EditScene.apply_grad_mask`` on
+    the local rows (again after every densification, which swaps the parameters), ``"kernel"`` passes this rank's
+    ``scene.mask`` to forward #1 (``ShardedGaussianRasterizer.forward(..., grad_mask=...)``); both zero the unmasked
+    view-space statistics before ``global_top_k``. ``None`` (default): no mask.
 
     Returns ``run_edit_loop``'s dict (counts are global) plus ``densify`` (per densification: ms of selection, surgery,
     rebalance and re-creation, bytes moved across ranks), ``params`` (this rank's final rows), ``plan`` and ``mode``."""
     from .gaussian_renderer import _settings_for
     from .sharded import Exchange, ShardPlan, ShardedGaussianRasterizer
+    if grad_mask not in (None, "hooks", "kernel"):
+        raise ValueError(f'grad_mask must be None, "hooks" or "kernel", got {grad_mask!r}')
     device = torch.device("cuda", torch.cuda.current_device())
     ex = Exchange(group)
     cloud, cams = synth.make_config("c5", P=P)
     plan = ShardPlan(cloud.means3D.shape[0], ex.world, ex.rank)
     scene = sharded_scene(cloud, device, plan)
+    if grad_mask == "hooks":
+        scene.apply_grad_mask()
     views = [make_view(c, device) for c in cams]
     bg = torch.zeros(3, device=device)
     settings = lambda v: _settings_for(v, bg, 1.0, scene.active_sh_degree)
@@ -287,12 +295,14 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
     rast = make(plan)
     mode = rast.mode
 
-    def forward(view, colors=None):
+    def forward(view, colors=None, mask=None):
         rast.raster_settings = settings(view)
         means2D = torch.zeros_like(scene._xyz, requires_grad=True) + 0   # viewspace_points, as render() makes it
         if means2D.requires_grad:   # not under no_grad (the targets)
             means2D.retain_grad()
         kw = dict(shs=scene.get_features) if colors is None else dict(colors_precomp=colors)
+        if mask is not None:
+            kw["grad_mask"] = mask.contiguous()
         color, radii, _ = rast(means3D=scene.get_xyz, means2D=means2D, opacities=scene.get_opacity,
                                scales=scene.get_scaling, rotations=scene.get_rotation, **kw)
         return color, radii, means2D
@@ -314,7 +324,7 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
             k = int(rng.integers(len(views)))
             e0, e1, e2, e3 = ev(), ev(), ev(), ev()
             e0.record()
-            color, radii, means2D = forward(views[k])                                          # forward #1
+            color, radii, means2D = forward(views[k], mask=scene.mask if grad_mask == "kernel" else None)  # #1
             sem, _, _ = forward(views[k], scene.mask[..., None].float().repeat(1, 3))          # forward #2
             e1.record()
             semantic = torch.norm(sem, dim=0) > 0.8
@@ -334,7 +344,10 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
             losses.append(loss.detach())
             if step % densification_interval == 0 and step < steps:
                 radii_trace.append(scene.max_radii2D.clone())
-                plan, phase = sharded_densify(scene, ex, plan, rast, max_densify_percent, min_opacity)
+                plan, phase = sharded_densify(scene, ex, plan, rast, max_densify_percent, min_opacity,
+                                              masked=grad_mask is not None)
+                if grad_mask == "hooks":
+                    scene.apply_grad_mask()   # the new parameters take the hooks
                 rast = make(plan)
                 torch.cuda.synchronize()
                 phase["recreate"] = (time.perf_counter() - phase.pop("_t")) * 1e3
@@ -354,10 +367,11 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
                 mask=scene.mask, optimizer=scene.optimizer)
 
 
-def sharded_densify(scene, ex, plan, rast=None, max_densify_percent=0.01, min_opacity=0.005):
+def sharded_densify(scene, ex, plan, rast=None, max_densify_percent=0.01, min_opacity=0.005, masked=False):
     """One densification of run_sharded_edit_loop (collective) on this rank's rows of `scene`: global top-k, local prune
     and clone, rebalance (K = 2, the mask carried along), statistics reset; closes `rast`. Returns (new plan, phase
-    times in ms and bytes moved); the caller re-creates the rasterizer and times that from ``phase["_t"]``."""
+    times in ms and bytes moved); the caller re-creates the rasterizer and times that from ``phase["_t"]``. ``masked``:
+    an edit under a gradient mask, whose unmasked view-space gradients are zeroed before the selection."""
     from . import optim_surgery
     from . import shard_rebalance as SR
     phase = {}
@@ -371,6 +385,8 @@ def sharded_densify(scene, ex, plan, rast=None, max_densify_percent=0.01, min_op
 
     with torch.no_grad():
         grads = (scene.xyz_gradient_accum / scene.denom).squeeze(1)     # NaN where denom == 0: counts as 0
+        if masked:
+            grads.masked_fill_(~scene.mask, 0.0)
         k = max(1, int(plan.P_total * max_densify_percent))
         sel = SR.global_top_k(ex, plan, grads, k)
         lap("select")

@@ -294,13 +294,27 @@ class WorkspacePool:
 class ShardBuffers:
     """Per-rank device state of one sharded forward (all arrays indexed by global Gaussian index)."""
     __slots__ = ("plan", "geom", "radii", "binning", "img", "R", "M", "W", "H", "inputs", "s", "own", "keep", "peer",
-                 "ws", "__weakref__")
+                 "ws", "grad_mask", "__weakref__")
 
     def alloc(self, name: str, numel: int, dtype, device, grow: float = 1.0) -> torch.Tensor:
         """A scratch buffer: from the persistent StepWorkspace when there is one, else from the caching allocator."""
         if self.ws is not None:
             return self.ws.get(name, numel, dtype, grow)
         return torch.empty(numel, dtype=dtype, device=device)
+
+
+_mask_stand_in = {}
+
+
+def mask_ptr(mask: torch.Tensor):
+    """The pointer of a rank's grad_mask rows for the masked entry points, which reject NULL: an empty shard (whose
+    mask has no storage) passes a 1-byte stand-in that nothing reads."""
+    if mask.numel() > 0:
+        return _ptr(mask)
+    t = _mask_stand_in.get(mask.device)
+    if t is None:
+        t = _mask_stand_in[mask.device] = torch.zeros(1, dtype=torch.uint8, device=mask.device)
+    return _ptr(t)
 
 
 def _view_bytes(base: torch.Tensor, ptr: int, nbytes: int) -> torch.Tensor:
@@ -325,13 +339,16 @@ def exchange_view(buf: ShardBuffers) -> torch.Tensor:
 def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D, sh, colors_precomp, opacities,
                      scales, rotations, cov3Ds_precomp, *, geom: Optional[torch.Tensor] = None,
                      radii: Optional[torch.Tensor] = None, peer: Optional[PeerWorkspace] = None,
-                     ws: Optional[StepWorkspace] = None, raw_rest: Optional[torch.Tensor] = None) -> ShardBuffers:
+                     ws: Optional[StepWorkspace] = None, raw_rest: Optional[torch.Tensor] = None,
+                     grad_mask: Optional[torch.Tensor] = None) -> ShardBuffers:
     """Stage 1: project this rank's Gaussians into its slice of the global arrays. `geom` / `radii` may be passed
     in to share one set of global arrays between virtual ranks of a single process. With `peer` (a PeerWorkspace of
     gsr_geometry_bytes(P_pad) bytes) the kernel pushes its records into every rank's workspace itself: no all-gather
     follows, only a barrier. `ws` (a StepWorkspace) supplies all scratch buffers persistently, its `peer` included.
     With `raw_rest` (features_rest [n,K,3]) the shard is the scene model's raw parameters (fused activations): `sh` is
-    features_dc [n,1,3], `opacities` / `scales` / `rotations` are the logits, log-scales and raw rotations."""
+    features_dc [n,1,3], `opacities` / `scales` / `rotations` are the logits, log-scales and raw rotations. With
+    `grad_mask` (uint8 [n], this rank's rows) the masked twin writes each edited Gaussian's edit word into its record,
+    for the masked blend backward of every tile owner."""
     lib = _lib.load()
     if ws is not None and ws.peer is not None:
         peer = ws.peer
@@ -345,7 +362,7 @@ def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D
     if raw_rest is not None:
         M = 1 + raw_rest.size(1)
     buf = ShardBuffers()
-    buf.plan, buf.M, buf.W, buf.H, buf.ws = plan, M, W, H, ws
+    buf.plan, buf.M, buf.W, buf.H, buf.ws, buf.grad_mask = plan, M, W, H, ws, grad_mask
     with torch.cuda.device(device):
         means3D = _f32c(means3D, device); opacities = _f32c(opacities, device)
         sh = _f32c(sh, device); colors_precomp = _f32c(colors_precomp, device)
@@ -367,15 +384,17 @@ def shard_preprocess(plan: ShardPlan, rs: GaussianRasterizationSettings, means3D
         buf.own = plan.owner()
         c = _shard_cloud(plan.count, buf.inputs)
         raw = "_raw" if len(buf.inputs) == 8 else ""
+        masked = () if grad_mask is None else (mask_ptr(grad_mask),)
+        sfx = raw + ("_masked" if masked else "")
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         if peer is not None:
-            _lib.check(getattr(lib, "gsr_shard_preprocess_p2p" + raw)(
+            _lib.check(getattr(lib, "gsr_shard_preprocess_p2p" + sfx)(
                 C.byref(s), C.byref(c), plan.P_pad, plan.base, plan.slice_len, peer.ptr_array, plan.world, plan.rank,
-                peer.nbytes, _ptr(buf.radii), st), "gsr_shard_preprocess_p2p" + raw)
+                peer.nbytes, _ptr(buf.radii), *masked, st), "gsr_shard_preprocess_p2p" + sfx)
         else:
-            _lib.check(getattr(lib, "gsr_shard_preprocess" + raw)(
+            _lib.check(getattr(lib, "gsr_shard_preprocess" + sfx)(
                 C.byref(s), C.byref(c), plan.P_pad, plan.base, plan.slice_len, _ptr(buf.geom), gbytes,
-                _ptr(buf.radii), st), "gsr_shard_preprocess" + raw)
+                _ptr(buf.radii), *masked, st), "gsr_shard_preprocess" + sfx)
     return buf
 
 
@@ -556,16 +575,33 @@ def static_status_error(status, capacity: int, segment_capacity: Optional[int], 
 
 def owner_backward_render(s, own, P: int, R: int, geom: torch.Tensor, binning: torch.Tensor, img: torch.Tensor,
                           grad_out_color: torch.Tensor, acc: torch.Tensor, deterministic: bool, get,
-                          grad_depth: Optional[torch.Tensor] = None, grad_alpha: Optional[torch.Tensor] = None):
+                          grad_depth: Optional[torch.Tensor] = None, grad_alpha: Optional[torch.Tensor] = None,
+                          masked: bool = False):
     """gsr_shard_backward_render (or its deterministic form) of the owned tiles of a P-record workspace into
     acc [P, 12]; `get(name, numel, dtype, grow)` supplies the deterministic scratch. With `grad_depth` [1,H,W]
     (gsr_shard_backward_render_depth) float 9 of each row also gets dL/dz. With `grad_alpha` [1,H,W]
-    (gsr_shard_backward_render_alpha, `grad_depth` optional) the alpha image's gradient enters too."""
+    (gsr_shard_backward_render_alpha, `grad_depth` optional) the alpha image's gradient enters too. `masked`: the
+    records come from a masked preprocess, and gsr_shard_backward_render_masked skips the unedited splats' work (their
+    rows stay +0.0)."""
     lib = _lib.load()
     device = geom.device
     with torch.cuda.device(device):
         grad_out_color = _f32c(grad_out_color, device)
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        if masked:
+            grad_alpha = None if grad_alpha is None else _f32c(grad_alpha, device)
+            grad_depth = None if grad_depth is None else _f32c(grad_depth, device)
+            det, dbytes = None, 0
+            if deterministic:
+                dbytes = lib.gsr_deterministic_scratch_bytes(P, R, 0)
+                det = get("det", dbytes, torch.uint8, 1.25)
+            mbytes = lib.gsr_grad_mask_scratch_bytes(int(s.image_width), int(s.image_height))
+            first = get("grad_mask_first", mbytes, torch.uint8, 1.0)
+            _lib.check(lib.gsr_shard_backward_render_masked(
+                C.byref(s), C.byref(own), P, R, _ptr(geom), geom.numel(), _ptr(binning), binning.numel(), _ptr(img),
+                img.numel(), _ptr(grad_out_color), _ptr(grad_alpha), _ptr(grad_depth), _ptr(acc), acc.numel() * 4,
+                _ptr(det), dbytes, _ptr(first), mbytes, st), "gsr_shard_backward_render_masked")
+            return
         if grad_alpha is not None:
             grad_alpha = _f32c(grad_alpha, device)
             grad_depth = None if grad_depth is None else _f32c(grad_depth, device)
@@ -605,12 +641,13 @@ def shard_backward_render(buf: ShardBuffers, grad_out_color: torch.Tensor, deter
                           grad_alpha: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Backward stage 1: this rank's tiles -> partial accumulators [P_pad, 12] (zero for untouched Gaussians). With
     `deterministic` each row is the same bits on every call (no float atomics). With `grad_depth` [1,H,W] the depth
-    image's gradient enters too (dL/dz in float 9), with `grad_alpha` [1,H,W] the alpha image's."""
+    image's gradient enters too (dL/dz in float 9), with `grad_alpha` [1,H,W] the alpha image's. After a masked
+    shard_preprocess only the edited Gaussians' rows are nonzero."""
     device = buf.geom.device
     acc = buf.alloc("acc", buf.plan.P_pad * ACC_STRIDE, torch.float32, device).view(buf.plan.P_pad, ACC_STRIDE)
     owner_backward_render(buf.s, buf.own, buf.plan.P_pad, buf.R, buf.geom, buf.binning, buf.img, grad_out_color, acc,
                           deterministic, lambda name, n, dtype, grow: buf.alloc(name, n, dtype, device, grow),
-                          grad_depth, grad_alpha)
+                          grad_depth, grad_alpha, buf.grad_mask is not None)
     return acc
 
 
@@ -650,7 +687,8 @@ def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor, depth:
     """Backward stage 2 (after the reduce-scatter): gradients of this rank's Gaussians, reference slot order (or the
     raw parameters' order of GaussianRasterizer.forward_raw for a raw shard). `depth`: the rows carry dL/dz (the
     blending backward had a depth gradient). `camera` (from camera_row, activated shards only): this rank's camera
-    partial is written too (gsr_shard_backward_preprocess_camera)."""
+    partial is written too (gsr_shard_backward_preprocess_camera). After a masked shard_preprocess the masked twin
+    writes +0.0 into every gradient of an unedited Gaussian (``buf.grad_mask`` as it holds now)."""
     lib = _lib.load()
     device = buf.geom.device
     plan = buf.plan
@@ -659,7 +697,14 @@ def shard_backward_preprocess(buf: ShardBuffers, acc_slice: torch.Tensor, depth:
         st = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
         args = (C.byref(buf.s), C.byref(c), plan.P_pad, plan.base, _ptr(buf.geom), buf.geom.numel(), _ptr(buf.radii),
                 _ptr(acc_slice), C.byref(gr))
-        if camera is not None:
+        if buf.grad_mask is not None:
+            if raw:
+                _lib.check(lib.gsr_shard_backward_preprocess_raw_masked(*args, int(depth), mask_ptr(buf.grad_mask), st),
+                           "gsr_shard_backward_preprocess_raw_masked")
+            else:
+                _lib.check(lib.gsr_shard_backward_preprocess_masked(*args, int(depth), None, mask_ptr(buf.grad_mask),
+                                                                    st), "gsr_shard_backward_preprocess_masked")
+        elif camera is not None:
             _lib.check(lib.gsr_shard_backward_preprocess_camera(*args, int(depth), C.byref(camera), st),
                        "gsr_shard_backward_preprocess_camera")
         elif raw:
@@ -787,15 +832,16 @@ class _ShardedRasterize(torch.autograd.Function):
     """Dense exchange. `raw_rest` (features_rest) makes it the fused-activation call (see shard_preprocess);
     `depth_grad` makes the depth output differentiable, with GaussianRasterizer(depth_grad=True)'s semantics;
     `return_alpha` adds the alpha output (a fifth frame plane); `viewmatrix` / `projmatrix` / `campos` (the settings'
-    camera arrays, or None) are the camera inputs of camera_grad."""
+    camera arrays, or None) are the camera inputs of camera_grad; `grad_mask` (uint8 [n] or None) selects the masked
+    preprocess and backward."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, plan,
                 exchange, pool, deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False,
-                viewmatrix=None, projmatrix=None, campos=None):
+                viewmatrix=None, projmatrix=None, campos=None, grad_mask=None):
         ws = pool.take(means3D.device) if pool is not None else None
         buf = shard_preprocess(plan, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                               ws=ws, raw_rest=raw_rest)
+                               ws=ws, raw_rest=raw_rest, grad_mask=grad_mask)
         if ws is not None:
             weakref.finalize(buf, pool.give, ws)     # back to the pool when the last user of this forward is gone
         if buf.peer is not None:
@@ -844,7 +890,7 @@ class _ShardedRasterize(torch.autograd.Function):
         else:
             grads = shard_backward_preprocess(buf, acc_slice, grad_depth is not None)
         grads, d_rest = grads_in_slots(grads, len(buf.inputs) == 8)
-        return (*grads, None, None, None, None, None, None, d_rest, None, *cam_grads)
+        return (*grads, None, None, None, None, None, None, d_rest, None, *cam_grads, None)
 
 
 class _ShardedRasterizeStatic(torch.autograd.Function):
@@ -855,10 +901,10 @@ class _ShardedRasterizeStatic(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, plan,
                 exchange, pool, deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False,
-                viewmatrix=None, projmatrix=None, campos=None, capacity=1, status=None):
+                viewmatrix=None, projmatrix=None, campos=None, capacity=1, status=None, grad_mask=None):
         ws = pool.take(means3D.device)
         buf = shard_preprocess(plan, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                               ws=ws, raw_rest=raw_rest)
+                               ws=ws, raw_rest=raw_rest, grad_mask=grad_mask)
         weakref.finalize(buf, pool.give, ws)
         buf.ws = StaticScratch(ws)                     # scratch of its own, never grown by apply_weights
         if buf.peer is not None:
@@ -933,6 +979,25 @@ def p2p_available(exchange: "Exchange") -> bool:
     return bool(int(flag[0]))
 
 
+def check_sharded_grad_mask(mask, plan: ShardPlan, means3D, camera_grad: bool, raster_settings) -> torch.Tensor:
+    """The checks of ``ShardedGaussianRasterizer.forward(..., grad_mask=...)``, made before any collective: this rank's
+    rows [plan.count], bool or uint8, contiguous, on means3D's device; not with camera_grad. Returns the uint8 view."""
+    if not isinstance(mask, torch.Tensor):
+        raise ValueError(f"grad_mask must be a torch.Tensor, got {type(mask).__name__}")
+    if mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"grad_mask must be a bool or uint8 tensor, got {mask.dtype}")
+    if mask.dim() != 1 or mask.numel() != plan.count:
+        raise ValueError(f"grad_mask must be this rank's rows [{plan.count}] (rank {plan.rank}), got shape "
+                         f"{tuple(mask.shape)}")
+    if not mask.is_contiguous():
+        raise ValueError("grad_mask must be contiguous")
+    if camera_grad:
+        raise ValueError("grad_mask cannot be combined with camera_grad: the camera gradient sums over every Gaussian")
+    if mask.device != means3D.device:
+        raise ValueError(f"grad_mask is on {mask.device}, means3D on {means3D.device}")
+    return mask.view(torch.uint8) if mask.dtype == torch.bool else mask
+
+
 def check_forward_raw_flags(module):
     """forward_raw has neither the alpha output nor camera gradients (the fused-activation preprocess backward has no
     camera form, and the single-GPU forward_raw offers neither). Raised before any collective, so that the peers are
@@ -997,6 +1062,17 @@ class ShardedGaussianRasterizer(nn.Module):
     ``check_capacity()`` synchronises and raises. Otherwise frames, radii and alpha are the default path's bits and
     gradients agree with it (bit for bit with ``deterministic=True``). ``apply_weights`` keeps its exact, host-sized path.
     Not combinable with ``raster_settings.debug``.
+    ``grad_mask`` (opt-in, a per-call argument of ``forward`` and ``forward_raw``, not a constructor option: the mask
+    changes whenever the cloud is densified): THIS RANK's rows [n] of ``GaussianRasterizer``'s ``grad_mask``, a bool
+    (viewed as uint8, not copied) or uint8 CUDA tensor, contiguous. Only the Gaussians with ``grad_mask[i] != 0`` take
+    gradients; every gradient row of the others is +0.0. The edit bit travels to the tile owners inside the splat
+    records, whose exchange already exists, and their blend backward skips the unedited splats' work. Frames, radii,
+    depth and alpha are unchanged; the edited rows equal the unmasked backward's (bit for bit with
+    ``deterministic=True``). It is part of the collective contract: every rank passes a mask, or none does, exactly as
+    every rank renders the same camera. The mask must hold the same values at the backward as at the forward (the blend
+    backward uses the forward's bits, the preprocess backward reads the mask). It combines with both modes,
+    ``deterministic``, ``depth_grad``, ``return_alpha`` and ``static_capacity`` (captured in a CUDA graph, the mask's
+    storage is fixed and its contents may change between replays); not with ``camera_grad`` (ValueError).
     """
 
     def __init__(self, raster_settings: GaussianRasterizationSettings, P_total: int, group=None,
@@ -1055,7 +1131,9 @@ class ShardedGaussianRasterizer(nn.Module):
         self.closed = True
 
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
-                cov3D_precomp=None):
+                cov3D_precomp=None, grad_mask=None):
+        if grad_mask is not None:
+            grad_mask = check_sharded_grad_mask(grad_mask, self.plan, means3D, self.camera_grad, self.raster_settings)
         if not getattr(self, "deterministic", False):
             _check_deterministic_flag()
         if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
@@ -1069,23 +1147,28 @@ class ShardedGaussianRasterizer(nn.Module):
         scales = empty if scales is None else scales
         rotations = empty if rotations is None else rotations
         cov3D_precomp = empty if cov3D_precomp is None else cov3D_precomp
-        return self._apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, None)
+        return self._apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp, None,
+                           grad_mask)
 
-    def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations):
+    def forward_raw(self, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
+                    grad_mask=None):
         """``GaussianRasterizer.forward_raw`` of a sharded cloud (collective): THIS RANK's rows of the scene model's raw
         parameters (``_xyz, _opacity, _features_dc, _features_rest, _scaling, _rotation``); the activations and the SH
         concatenation happen inside the preprocess kernels. Returns ``(color, radii_local, depth)`` as ``forward``;
-        gradients land on the raw local leaves (``means2D`` included)."""
+        gradients land on the raw local leaves (``means2D`` included). ``grad_mask``: as in ``forward``."""
         check_forward_raw_flags(self)
+        if grad_mask is not None:
+            grad_mask = check_sharded_grad_mask(grad_mask, self.plan, means3D, self.camera_grad, self.raster_settings)
         if not getattr(self, "deterministic", False):
             _check_deterministic_flag()
         if means3D.dim() != 2 or means3D.size(1) != 3:
             raise RuntimeError("means3D must have dimensions (num_points, 3)")
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
         return self._apply(means3D, means2D, features_dc, empty, opacity_logits, log_scales, raw_rotations, empty,
-                           features_rest)
+                           features_rest, grad_mask)
 
-    def _apply(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest):
+    def _apply(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest,
+               grad_mask=None):
         if getattr(self, "closed", False):
             raise RuntimeError("this ShardedGaussianRasterizer was closed: construct a new one")
         rs = self.raster_settings
@@ -1094,7 +1177,7 @@ class ShardedGaussianRasterizer(nn.Module):
         cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if getattr(self, "camera_grad", False) else (None, None, None)
         if getattr(self, "static_capacity", None) is not None:
             return self._apply_static(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                      raw_rest, depth_grad, return_alpha, cam)
+                                      raw_rest, depth_grad, return_alpha, cam, grad_mask)
         if self.mode == "sparse":
             from . import sparse_sharded as SS
             rk0 = self.sparse_pool.all[0]
@@ -1102,13 +1185,14 @@ class ShardedGaussianRasterizer(nn.Module):
                 raise RuntimeError("sparse mode: the image size is fixed at construction (peer-mapped frames)")
             return SS._SparseShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                                     cov3D_precomp, rs, self.sparse_pool, self.exchange,
-                                                    self.deterministic, depth_grad, raw_rest, return_alpha, *cam)
+                                                    self.deterministic, depth_grad, raw_rest, return_alpha, *cam,
+                                                    grad_mask)
         return _ShardedRasterize.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                        cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic,
-                                       depth_grad, raw_rest, return_alpha, *cam)
+                                       depth_grad, raw_rest, return_alpha, *cam, grad_mask)
 
     def _apply_static(self, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, raw_rest,
-                      depth_grad, return_alpha, cam):
+                      depth_grad, return_alpha, cam, grad_mask=None):
         rs = self.raster_settings
         if rs.debug:
             raise ValueError("static_capacity cannot be combined with debug=True: debug synchronises after every launch")
@@ -1123,11 +1207,11 @@ class ShardedGaussianRasterizer(nn.Module):
             return SS._SparseShardedRasterizeStatic.apply(
                 means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3D_precomp, rs, self.sparse_pool,
                 self.exchange, self.deterministic, depth_grad, raw_rest, return_alpha, *cam, self.static_capacity,
-                seg_cap, self.status)
+                seg_cap, self.status, grad_mask)
         return _ShardedRasterizeStatic.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                              cov3D_precomp, rs, self.plan, self.exchange, self.pool, self.deterministic,
                                              depth_grad, raw_rest, return_alpha, *cam, self.static_capacity,
-                                             self.status)
+                                             self.status, grad_mask)
 
     def check_capacity(self) -> int:
         """Synchronise with the last static forward and raise RuntimeError if it overflowed anywhere (that frame was

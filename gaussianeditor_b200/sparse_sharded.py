@@ -32,8 +32,8 @@ import torch.nn as nn
 
 from . import _lib
 from .rasterizer import GaussianRasterizationSettings, _f32c, _make_settings, _ptr, _wait_count
-from .sharded import (ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, _shard_cloud, grads_in_slots, preprocess_grads,
-                      shard_slice)
+from .sharded import (ACC_STRIDE, Exchange, PeerWorkspace, ShardPlan, _shard_cloud, grads_in_slots, mask_ptr,
+                      preprocess_grads, shard_slice)
 
 MAXP = 8  # GSR_MAX_PEERS
 CTRL_BYTES, CTRL_MATRIX_OFFSET, CTRL_ERROR_OFFSET = 512, 64, 32   # GSR_PEER_CTRL_{BYTES,MATRIX_OFFSET,ERROR_OFFSET}
@@ -163,7 +163,7 @@ def link_virtual(ranks: List[SparseRank]):
 class SparseStep:
     """One forward in flight on one rank."""
     __slots__ = ("rk", "cap", "s", "keep", "inputs", "M", "R", "max_count", "binning", "img", "radii_cand", "cplan", "n",
-                 "__weakref__")
+                 "grad_mask", "__weakref__")
 
 
 def _cplan(plan: ShardPlan, cap: int) -> "_lib.SparsePlan":
@@ -171,10 +171,11 @@ def _cplan(plan: ShardPlan, cap: int) -> "_lib.SparsePlan":
 
 
 def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D, sh, colors_precomp, opacities, scales,
-                      rotations, cov3Ds_precomp, cap: int, raw_rest: Optional[torch.Tensor] = None) -> SparseStep:
+                      rotations, cov3Ds_precomp, cap: int, raw_rest: Optional[torch.Tensor] = None,
+                      grad_mask: Optional[torch.Tensor] = None) -> SparseStep:
     """Owner side: preprocess the shard and push every record to the candidate arrays of the ranks it touches. Writes
     row `rank` of ``rk.matrix`` (the other rows must be zero before the all-reduce that follows). `raw_rest`: a raw
-    shard, as in sharded.shard_preprocess."""
+    shard, `grad_mask`: this rank's edit mask [n] (the records carry the edit words), as in sharded.shard_preprocess."""
     lib = _lib.load()
     plan, device = rk.plan, rk.device
     if not means3D.is_cuda:
@@ -184,7 +185,7 @@ def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D
     if not (1 <= cap <= rk.cap_alloc):
         raise RuntimeError(f"segment capacity {cap} outside [1, {rk.cap_alloc}]")
     st = SparseStep()
-    st.rk, st.cap, st.n = rk, int(cap), plan.count
+    st.rk, st.cap, st.n, st.grad_mask = rk, int(cap), plan.count, grad_mask
     st.M = sh.size(1) if sh.numel() != 0 else 0
     if raw_rest is not None:
         st.M = 1 + raw_rest.size(1)
@@ -196,7 +197,8 @@ def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D
         st.inputs = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
         if raw_rest is not None:   # a slice whose rows start off a 16-byte boundary is cloned by _f32c
             st.inputs = st.inputs + (_f32c(raw_rest, device),)
-        raw = "_raw" if raw_rest is not None else ""
+        raw = ("_raw" if raw_rest is not None else "") + ("_masked" if grad_mask is not None else "")
+        masked = () if grad_mask is None else (mask_ptr(grad_mask),)
         st.keep = []
         st.s = _make_settings(rs, st.M, device, st.keep)
         st.cplan = _cplan(plan, cap)
@@ -207,7 +209,7 @@ def sparse_preprocess(rk: SparseRank, rs: GaussianRasterizationSettings, means3D
         cand_bytes = lib.gsr_sparse_candidate_bytes(plan.world, cap)
         _lib.check(getattr(lib, "gsr_sparse_preprocess" + raw)(
             C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local), rk.local_bytes, _ptr(rk.radii_local),
-            rk.cand_ptr_array, cand_bytes, C.c_void_p(rk.matrix[plan.rank].data_ptr()), stream),
+            rk.cand_ptr_array, cand_bytes, C.c_void_p(rk.matrix[plan.rank].data_ptr()), *masked, stream),
             "gsr_sparse_preprocess" + raw)
     return st
 
@@ -322,7 +324,7 @@ def sparse_backward_render(st: SparseStep, grad_out_color: torch.Tensor, determi
     gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
     owner_backward_render(st.s, rk.plan.owner(), M, st.R, rk.cand[:gb], st.binning, st.img, grad_out_color, acc,
                           deterministic, lambda name, n, dtype, grow: rk.get(name, n, dtype, grow), grad_depth,
-                          grad_alpha)
+                          grad_alpha, st.grad_mask is not None)
     return acc
 
 
@@ -350,7 +352,14 @@ def sparse_backward_preprocess(st: SparseStep, depth: bool = False, camera: Opti
         gb = lib.gsr_sparse_candidate_bytes(rk.plan.world, st.cap)
         args = (C.byref(st.s), C.byref(c), C.byref(st.cplan), _ptr(rk.local), rk.local_bytes, _ptr(rk.radii_local),
                 _ptr(rk.cand), gb, _ptr(acc_slice), acc_slice.numel() * 4, C.byref(gr))
-        if camera is not None:
+        if st.grad_mask is not None:
+            if raw:
+                _lib.check(lib.gsr_sparse_backward_preprocess_raw_masked(*args, int(depth), mask_ptr(st.grad_mask),
+                                                                         stream), "gsr_sparse_backward_preprocess_raw_masked")
+            else:
+                _lib.check(lib.gsr_sparse_backward_preprocess_masked(*args, int(depth), None, mask_ptr(st.grad_mask),
+                                                                     stream), "gsr_sparse_backward_preprocess_masked")
+        elif camera is not None:
             _lib.check(lib.gsr_sparse_backward_preprocess_camera(*args, int(depth), C.byref(camera), stream),
                        "gsr_sparse_backward_preprocess_camera")
         elif raw:
@@ -460,12 +469,12 @@ def _mark(name: str):
 
 
 def _preprocess_and_order(rk: SparseRank, pool: SparsePool, rs, means3D, sh, colors_precomp, opacities, scales, rotations,
-                          cov3Ds_precomp, raw_rest=None):
+                          cov3Ds_precomp, raw_rest=None, grad_mask=None):
     """preprocess + push -- barrier with the count row -- order, redone with the exact capacity while a segment
     overflows; then the capacity of the next step. Returns (step, num_rendered of this rank, largest segment)."""
     while True:
         st = sparse_preprocess(rk, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                               pool.cap, raw_rest)
+                               pool.cap, raw_rest, grad_mask)
         _mark("preprocess+push")
         peer_barrier(rk, with_row=True)                # counts + barrier: every push has landed
         rk.queue_barrier_check()                       # sticky error word (this and earlier barriers) -> pinned
@@ -546,7 +555,7 @@ class _SparseShardedRasterize(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange,
                 deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False, viewmatrix=None,
-                projmatrix=None, campos=None):
+                projmatrix=None, campos=None, grad_mask=None):
         rk0 = pool.all[0]
         if (return_alpha and rk0.planes != 5) or (viewmatrix is not None and not rk0.camera):
             raise RuntimeError("return_alpha / camera gradients need a SparsePool built with alpha=True / camera=True")
@@ -555,7 +564,7 @@ class _SparseShardedRasterize(torch.autograd.Function):
         _mark("start")
         try:
             st, R, max_count = _preprocess_and_order(rk, pool, rs, means3D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp, raw_rest)
+                                                     rotations, cov3Ds_precomp, raw_rest, grad_mask)
         except BaseException:
             pool.give(rk)                                       # a failed forward must not leak its workspace
             raise
@@ -611,7 +620,7 @@ class _SparseShardedRasterize(torch.autograd.Function):
         grads, d_rest = grads_in_slots(grads, len(st.inputs) == 8)
         _mark("gather+preprocess backward")
         ctx.st = None   # the workspace goes back to the pool now, not when the output tensors die
-        return (*grads, None, None, None, None, None, d_rest, None, *cam_grads)
+        return (*grads, None, None, None, None, None, d_rest, None, *cam_grads, None)
 
 
 class _SparseShardedRasterizeStatic(torch.autograd.Function):
@@ -624,7 +633,7 @@ class _SparseShardedRasterizeStatic(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, pool, exchange,
                 deterministic=False, depth_grad=False, raw_rest=None, return_alpha=False, viewmatrix=None,
-                projmatrix=None, campos=None, capacity=1, seg_cap=1, status=None):
+                projmatrix=None, campos=None, capacity=1, seg_cap=1, status=None, grad_mask=None):
         from .sharded import StaticScratch
         rk0 = pool.all[0]
         if (return_alpha and rk0.planes != 5) or (viewmatrix is not None and not rk0.camera) or not rk0.device_epoch:
@@ -633,7 +642,7 @@ class _SparseShardedRasterizeStatic(torch.autograd.Function):
         rk = pool.take()
         try:
             st = sparse_preprocess(rk, rs, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                   seg_cap, raw_rest)
+                                   seg_cap, raw_rest, grad_mask)
             st.rk = StaticScratch(rk)                       # scratch of its own, never grown by apply_weights
             peer_barrier(rk, with_row=True)                # counts + barrier: every push has landed
             sparse_order_static(st, capacity)

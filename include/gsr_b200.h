@@ -709,6 +709,78 @@ GSR_API int gsr_shard_static_gate(const gsr_settings* s, int32_t P_total, void* 
                                   const int32_t* error_word /* may be NULL */, float* frame, int32_t planes,
                                   int32_t* status /* [4] device */, void* stream);
 
+/* ---- masked backward on the Gaussian-sharded path (opt-in; the sharded form of gsr_backward_masked) ----------
+ * A tile owner's lists hold global indices (dense) or candidate slots (sparse), never the rows of a per-rank mask, so the
+ * edit bit travels in the record: the masked preprocess twins below take the same arguments as their unmasked forms
+ * plus grad_mask [shard.P] (this rank's rows, one byte each, device memory) and write a nonzero edit word into the
+ * record of every visible Gaussian with grad_mask[i] != 0 (0 otherwise). Every exchange already moves whole records
+ * (all-gather, p2p push, sparse push), so the bit reaches every tile owner in its own index space at no extra cost;
+ * the sparse twins then run the unchanged mask / scan / push kernels. The forward outputs are unchanged.
+ *   gsr_shard_backward_render_masked: gsr_shard_backward_render_alpha on records from a masked preprocess, with the
+ *     work of unedited splats skipped as in gsr_backward_masked; dL_dout_alpha, dL_dout_depth and det_scratch may be
+ *     NULL; mask_scratch holds gsr_grad_mask_scratch_bytes(W, H) bytes (contents irrelevant). Takes no mask: the bits
+ *     are in the records. It serves the dense geometry and the sparse candidate workspace alike. Rows of unedited
+ *     Gaussians are +0.0.
+ *   gsr_{shard,sparse}_backward_preprocess[_raw]_masked: the unmasked forms' arguments (`depth` != 0: the rows carry
+ *     dL/dz) plus grad_mask [shard.P]; an unedited Gaussian gets +0.0 in every gradient slot. camera must be NULL.
+ * A NULL grad_mask or a non-NULL camera returns GSR_ERR_INVALID before any device work. */
+GSR_API int gsr_shard_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total, int32_t index_base,
+                                        int32_t slice_len, void* geometry, size_t geometry_bytes, int32_t* radii_total,
+                                        const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_shard_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                            int32_t index_base, int32_t slice_len, void* geometry,
+                                            size_t geometry_bytes, int32_t* radii_total, const uint8_t* grad_mask,
+                                            void* stream);
+GSR_API int gsr_shard_preprocess_p2p_masked(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                            int32_t index_base, int32_t slice_len, void* const* peer_geometry,
+                                            int32_t world, int32_t rank, size_t geometry_bytes, int32_t* radii_total,
+                                            const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_shard_preprocess_p2p_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                                int32_t index_base, int32_t slice_len, void* const* peer_geometry,
+                                                int32_t world, int32_t rank, size_t geometry_bytes,
+                                                int32_t* radii_total, const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_sparse_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, const gsr_sparse_plan* plan,
+                                         void* local_ws, size_t local_bytes, int32_t* radii_local,
+                                         void* const* peer_cand, size_t cand_bytes, int32_t* counts_row,
+                                         const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_sparse_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard,
+                                             const gsr_sparse_plan* plan, void* local_ws, size_t local_bytes,
+                                             int32_t* radii_local, void* const* peer_cand, size_t cand_bytes,
+                                             int32_t* counts_row, const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_shard_backward_render_masked(const gsr_settings* s, const gsr_tile_owner* owner, int32_t P_total,
+                                             int32_t R, const void* geometry, size_t geometry_bytes,
+                                             const void* binning, size_t binning_bytes, const void* image,
+                                             size_t image_bytes, const float* dL_dout_color,
+                                             const float* dL_dout_alpha /* may be NULL */,
+                                             const float* dL_dout_depth /* may be NULL */, void* acc_total,
+                                             size_t acc_bytes, void* det_scratch /* may be NULL */,
+                                             size_t det_scratch_bytes, void* mask_scratch, size_t mask_scratch_bytes,
+                                             void* stream);
+GSR_API int gsr_shard_backward_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard, int32_t P_total,
+                                                 int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                                 const int32_t* radii_total, const void* acc_slice,
+                                                 const gsr_grads* grads, int32_t depth,
+                                                 const gsr_camera_grads* camera /* must be NULL */,
+                                                 const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_shard_backward_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard, int32_t P_total,
+                                                     int32_t index_base, const void* geometry, size_t geometry_bytes,
+                                                     const int32_t* radii_total, const void* acc_slice,
+                                                     const gsr_raw_grads* grads, int32_t depth,
+                                                     const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_sparse_backward_preprocess_masked(const gsr_settings* s, const gsr_cloud* shard,
+                                                  const gsr_sparse_plan* plan, const void* local_ws,
+                                                  size_t local_bytes, const int32_t* radii_local, const void* cand_ws,
+                                                  size_t cand_bytes, void* acc_slice, size_t acc_bytes,
+                                                  const gsr_grads* grads, int32_t depth,
+                                                  const gsr_camera_grads* camera /* must be NULL */,
+                                                  const uint8_t* grad_mask, void* stream);
+GSR_API int gsr_sparse_backward_preprocess_raw_masked(const gsr_settings* s, const gsr_raw_cloud* shard,
+                                                      const gsr_sparse_plan* plan, const void* local_ws,
+                                                      size_t local_bytes, const int32_t* radii_local,
+                                                      const void* cand_ws, size_t cand_bytes, void* acc_slice,
+                                                      size_t acc_bytes, const gsr_raw_grads* grads, int32_t depth,
+                                                      const uint8_t* grad_mask, void* stream);
+
 /* ---- tuning / instrumentation ---------------------------------------------------------------------------
  * gsr_set_option("render_variant", v) etc.; unknown names return GSR_ERR_INVALID.
  * gsr_launch_count(): number of this library's kernel launches (CUB's included) since process start. */
