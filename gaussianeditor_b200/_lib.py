@@ -46,6 +46,7 @@ SYMBOLS = [
     "gsr_shard_preprocess_p2p_raw_masked", "gsr_sparse_preprocess_masked", "gsr_sparse_preprocess_raw_masked",
     "gsr_shard_backward_render_masked", "gsr_shard_backward_preprocess_masked", "gsr_shard_backward_preprocess_raw_masked",
     "gsr_sparse_backward_preprocess_masked", "gsr_sparse_backward_preprocess_raw_masked",
+    "gsr_adam_masked",
 ]
 
 
@@ -117,6 +118,15 @@ class SparsePlan(C.Structure):
 
 class SparseView(C.Structure):
     _fields_ = [("records", C.c_void_p), ("ret", C.c_void_p), ("geometry_bytes", C.c_size_t)]
+
+
+class AdamGroup(C.Structure):
+    _fields_ = [("p", C.c_void_p), ("g", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p), ("D", C.c_int32),
+                ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double),
+                ("step", C.c_double), ("step_dev", C.c_void_p)]
+
+
+ADAM_MAX_GROUPS = 16   # GSR_ADAM_MAX_GROUPS
 
 
 _lib = None
@@ -329,6 +339,8 @@ def load():
                                                           CG, u8, vp]
     lib.gsr_sparse_backward_preprocess_raw_masked.restype = C.c_int
     lib.gsr_sparse_backward_preprocess_raw_masked.argtypes = [S, RC, SP, vp, sz, vp, vp, sz, vp, sz, RG, i32, u8, vp]
+    lib.gsr_adam_masked.restype = C.c_int
+    lib.gsr_adam_masked.argtypes = [C.POINTER(AdamGroup), i32, i32, u8, vp]
     if lib.gsr_abi_version() != 2:
         raise RuntimeError("libgsr_b200.so ABI version mismatch")
     _lib = lib

@@ -37,8 +37,9 @@ from .rasterizer import GaussianRasterizationSettings
 
 
 class EditScene:
-    def __init__(self, cloud: synth.Cloud, device, capturable: bool = False):
+    def __init__(self, cloud: synth.Cloud, device, capturable: bool = False, optimizer: str = "adam"):
         self.capturable = capturable   # Adam(capturable=True): the optimizer step can be captured in a CUDA graph
+        self.optimizer_kind = optimizer   # "adam": torch.optim.Adam, "masked": MaskedAdam on `mask`
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
         eps = 1e-6
         self._xyz = t(cloud.means3D).requires_grad_(True)
@@ -73,7 +74,10 @@ class EditScene:
 
     def _make_optimizer(self):
         groups = [{"params": [p], "lr": lr, "name": n} for n, p, lr in self._params()]
-        if self.capturable:
+        if self.optimizer_kind == "masked":   # built after every densification, so it always holds the current mask
+            from .masked_adam import MaskedAdam
+            self.optimizer = MaskedAdam(groups, eps=1e-15, capturable=self.capturable, mask=self.mask)
+        elif self.capturable:
             self.optimizer = torch.optim.Adam(groups, eps=1e-15, capturable=True)
         else:
             self.optimizer = torch.optim.Adam(groups, eps=1e-15)
@@ -138,7 +142,7 @@ def make_view(cam: synth.Camera, device):
 
 def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densification_interval=100, seed=0,
                   log=None, fused_activations=False, cuda_graph=False, static_capacity=False, deterministic=None,
-                  grad_mask=None):
+                  grad_mask=None, optimizer="adam"):
     """Returns a dict with total / render wall times (CUDA-event timed) and the per-step Gaussian counts.
     ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only).
     ``cuda_graph=True`` captures one step per Gaussian count and replays it (see the module docstring);
@@ -149,13 +153,17 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
     ``grad_mask`` trains under the scene's mask ("20 % nearest the origin") as a GaussianEditor edit does: ``"hooks"``
     registers ``EditScene.apply_grad_mask`` (GaussianEditor's hooks, on all six parameters), ``"kernel"`` passes
     ``grad_mask=scene.mask`` to the SH render instead; both zero the unmasked view-space gradients before densifying.
-    ``None`` (default): no mask."""
+    ``None`` (default): no mask.
+    ``optimizer``: ``"adam"`` (default) steps ``torch.optim.Adam``; ``"masked"`` steps ``MaskedAdam`` on the scene's
+    mask (rebuilt with the new mask at every densification, inside the captured graph with ``cuda_graph``), which
+    needs a ``grad_mask``."""
     from . import gaussian_renderer as GR
     if grad_mask not in (None, "hooks", "kernel"):
         raise ValueError(f'grad_mask must be None, "hooks" or "kernel", got {grad_mask!r}')
+    _check_optimizer(optimizer, grad_mask)
     fixed = bool(cuda_graph or static_capacity)
     cloud, cams = synth.make_config("c5", P=P)
-    scene = EditScene(cloud, device, capturable=fixed)
+    scene = EditScene(cloud, device, capturable=fixed, optimizer=optimizer)
     if grad_mask == "hooks":
         scene.apply_grad_mask()
     # the SH render's mask argument, looked up per step: densification replaces scene.mask
@@ -229,20 +237,29 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                ms_per_step=total_ms / steps, P_first=counts[0], P_last=counts[-1], final_loss=float(loss.detach()),
                counts=counts, losses=torch.stack(losses).cpu().tolist(), max_radii2D=scene.max_radii2D.cpu(),
                max_radii2D_at_densify=[r.cpu() for r in radii_trace],
-               params={n: getattr(scene, a).detach() for n, a in _SCENE_ATTR.items()}, optimizer=scene.optimizer)
+               params={n: getattr(scene, a).detach() for n, a in _SCENE_ATTR.items()}, optimizer=scene.optimizer,
+               mask=scene.mask)
     if fixed:   # the step is not split by events: no render time
         out.update(render_ms=None, render_fraction=None, capacities=loop.capacities)
     return out
+
+
+def _check_optimizer(optimizer, grad_mask):
+    if optimizer not in ("adam", "masked"):
+        raise ValueError(f'optimizer must be "adam" or "masked", got {optimizer!r}')
+    if optimizer == "masked" and grad_mask is None:
+        raise ValueError('optimizer="masked" updates only the masked rows: it needs grad_mask="hooks" or "kernel"')
 
 
 _SCENE_ATTR = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity",
                "scaling": "_scaling", "rotation": "_rotation"}   # EditScene's param-group names -> attributes
 
 
-def sharded_scene(cloud: synth.Cloud, device, plan) -> EditScene:
-    """The EditScene of the whole `cloud` (mask included) cut to `plan`'s rows, with zero statistics and a fresh Adam."""
+def sharded_scene(cloud: synth.Cloud, device, plan, optimizer="adam") -> EditScene:
+    """The EditScene of the whole `cloud` (mask included) cut to `plan`'s rows, with zero statistics and a fresh
+    optimizer (`optimizer` as in ``EditScene``)."""
     from .sharded import shard_slice
-    scene = EditScene(cloud, device)
+    scene = EditScene(cloud, device, optimizer=optimizer)
     with torch.no_grad():
         for attr in _SCENE_ATTR.values():
             setattr(scene, attr, shard_slice(getattr(scene, attr).detach(), plan).clone().requires_grad_(True))
@@ -256,7 +273,8 @@ def sharded_scene(cloud: synth.Cloud, device, plan) -> EditScene:
 
 
 def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0, mode=None, deterministic=False,
-                          group=None, max_densify_percent=0.01, min_opacity=0.005, grad_mask=None):
+                          group=None, max_densify_percent=0.01, min_opacity=0.005, grad_mask=None,
+                          optimizer="adam"):
     """The config-5 step of ``run_edit_loop`` on a Gaussian-sharded cloud, one process per GPU (collective: every rank
     of `group` calls it with the same arguments; the process group must exist, NCCL).
 
@@ -272,7 +290,9 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
     ``grad_mask`` trains under the mask as ``run_edit_loop`` does: ``"hooks"`` registers ``EditScene.apply_grad_mask`` on
     the local rows (again after every densification, which swaps the parameters), ``"kernel"`` passes this rank's
     ``scene.mask`` to forward #1 (``ShardedGaussianRasterizer.forward(..., grad_mask=...)``); both zero the unmasked
-    view-space statistics before ``global_top_k``. ``None`` (default): no mask.
+    view-space statistics before ``global_top_k``. ``None`` (default): no mask. ``optimizer`` as in ``run_edit_loop``:
+    ``"masked"`` steps ``MaskedAdam`` on this rank's mask, re-set to the mask ``rebalance`` carries after every
+    densification.
 
     Returns ``run_edit_loop``'s dict (counts are global) plus ``densify`` (per densification: ms of selection, surgery,
     rebalance and re-creation, bytes moved across ranks), ``params`` (this rank's final rows), ``plan`` and ``mode``."""
@@ -280,11 +300,12 @@ def run_sharded_edit_loop(steps=200, P=None, densification_interval=100, seed=0,
     from .sharded import Exchange, ShardPlan, ShardedGaussianRasterizer
     if grad_mask not in (None, "hooks", "kernel"):
         raise ValueError(f'grad_mask must be None, "hooks" or "kernel", got {grad_mask!r}')
+    _check_optimizer(optimizer, grad_mask)
     device = torch.device("cuda", torch.cuda.current_device())
     ex = Exchange(group)
     cloud, cams = synth.make_config("c5", P=P)
     plan = ShardPlan(cloud.means3D.shape[0], ex.world, ex.rank)
-    scene = sharded_scene(cloud, device, plan)
+    scene = sharded_scene(cloud, device, plan, optimizer)
     if grad_mask == "hooks":
         scene.apply_grad_mask()
     views = [make_view(c, device) for c in cams]
@@ -399,6 +420,8 @@ def sharded_densify(scene, ex, plan, rast=None, max_densify_percent=0.01, min_op
         lap("surgery")
         stats = {}
         new_plan, (scene.mask,) = SR.rebalance(ex, plan, counts, scene.optimizer, extras=(mask,), stats=stats)
+        if scene.optimizer_kind == "masked":
+            scene.optimizer.set_mask(scene.mask)
         for group in scene.optimizer.param_groups:
             setattr(scene, _SCENE_ATTR[group["name"]], group["params"][0])
         n = new_plan.count

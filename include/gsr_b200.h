@@ -361,6 +361,35 @@ GSR_API int gsr_backward_raw_masked(const gsr_settings* s, const gsr_raw_cloud* 
                             void* det_scratch /* may be NULL */, size_t det_scratch_bytes, const uint8_t* grad_mask,
                             void* mask_scratch, size_t mask_scratch_bytes, void* stream);
 
+/* ---- masked Adam (one optimizer step over the Gaussians under edit) ------------------------------------------
+ * One Adam step (torch.optim.Adam without weight decay, amsgrad or maximize) over n_groups row-aligned fp32 tensors
+ * p, g, m, v of shape [P, D] (row-major, D may differ per group), in one launch, restricted to the rows with
+ * mask[i] != 0. Of an unedited row nothing is read or written: p, m and v keep their bits whatever g, m and v hold.
+ * Edited elements, in fp32:  m += (1 - beta1) * (g - m);  v = v * beta2 + (1 - beta2) * g * g;
+ *                            p -= step_size * m / (sqrt(v) / bc2_sqrt + eps)
+ * step_dev == NULL: step is the step count after this update (host), and step_size = lr / (1 - beta1^step),
+ * bc2_sqrt = (1 - beta2^step)^0.5 are computed on the host in double, as torch computes them for a CPU step.
+ * step_dev != NULL (capturable): the call adds 1 to the device float *step_dev first, then the update computes
+ * step_size and bc2_sqrt in fp32 from it on the device, as torch's capturable Adam does. No host synchronisation, no
+ * atomics: the call can be captured in a CUDA graph, and each replay advances the step once.
+ * Groups with P * D == 0 are skipped (their pointers may be NULL; a device step is still advanced).
+ * GSR_ERR_INVALID, before any device work: n_groups outside [1, GSR_ADAM_MAX_GROUPS], NULL groups or mask, P < 0,
+ * D < 0 or D > GSR_ADAM_MAX_D, a NULL p, g, m or v in a group with P * D > 0, beta1 or beta2 outside [0, 1), eps < 0. */
+#define GSR_ADAM_MAX_GROUPS 16
+#define GSR_ADAM_MAX_D (1 << 24)
+typedef struct gsr_adam_group {
+  float* p;
+  const float* g;
+  float* m;          /* exp_avg */
+  float* v;          /* exp_avg_sq */
+  int32_t D;         /* floats per row */
+  double lr, beta1, beta2, eps;
+  double step;       /* used when step_dev == NULL */
+  float* step_dev;   /* capturable: device step, incremented by the call */
+} gsr_adam_group;
+GSR_API int gsr_adam_masked(const gsr_adam_group* groups, int32_t n_groups, int32_t P, const uint8_t* mask,
+                            void* stream);
+
 /* ---- Gaussian-sharded multi-GPU path (BASELINE config 4; SURVEY.md 8(e)) ----------------------------------
  * The reference has no multi-GPU rasterizer; these entry points split the single-GPU pipeline at the two places
  * where the Gaussian-index decomposition (preprocess, fused preprocess backward) meets the tile decomposition
