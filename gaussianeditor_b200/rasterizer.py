@@ -133,7 +133,7 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
     device = means3D.device
     P = means3D.size(0)
     H, W = int(rs.image_height), int(rs.image_width)
-    M = sh.size(1) if sh.numel() != 0 else 0
+    M = sh.size(1) if sh.dim() >= 2 else 0   # from the shape: an empty cloud's dL/dsh is [0, M, 3] like its input
     raw = raw_rest is not None
     if raw:
         M = 1 + raw_rest.size(1)

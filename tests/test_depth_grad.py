@@ -22,8 +22,8 @@ A_MAX = float(np.float32(0.99))   # the alpha clamp 0.99f of the forward
 
 # ---- the fp64 truth ------------------------------------------------------------------------------------------------
 
-def _forward64(cloud, cam, bg, colors_precomp=None, cov3D_precomp=None):
-    kw = {}
+def _forward64(cloud, cam, bg, colors_precomp=None, cov3D_precomp=None, scale_modifier=1.0):
+    kw = dict(scale_modifier=scale_modifier)
     if colors_precomp is not None:
         kw["colors_precomp"] = colors_precomp
     if cov3D_precomp is not None:
@@ -31,10 +31,11 @@ def _forward64(cloud, cam, bg, colors_precomp=None, cov3D_precomp=None):
     return O.forward_from(cloud, cam, bg, f32=False, **kw)
 
 
-def depth_truth(cloud, cam, bg, gC=None, gD=None, gA=None, colors_precomp=None, cov3D_precomp=None):
+def depth_truth(cloud, cam, bg, gC=None, gD=None, gA=None, colors_precomp=None, cov3D_precomp=None,
+                scale_modifier=1.0):
     """fp64 gradients of  sum gC*colour + sum gD*depth + sum gA*alpha  (each upstream optional). Returns the oracle's
     gradient dict plus ``ddepth`` [P] (dL/dz per Gaussian), and the colour-pass forward as ``fwd``."""
-    f = _forward64(cloud, cam, bg, colors_precomp, cov3D_precomp)
+    f = _forward64(cloud, cam, bg, colors_precomp, cov3D_precomp, scale_modifier)
     P, M, H, W = f.P, f.M, f.H, f.W
     if gC is not None:
         g = f.backward(np.asarray(gC, np.float32))
@@ -47,7 +48,7 @@ def depth_truth(cloud, cam, bg, gC=None, gD=None, gA=None, colors_precomp=None, 
         hi = f.depths.astype(np.float32)
         lo = (f.depths - hi.astype(np.float64)).astype(np.float32)
         cols = np.stack([hi, lo, np.ones(P, np.float32)], 1)
-        fd = _forward64(cloud, cam, (0.0, 0.0, 0.0), cols, cov3D_precomp)
+        fd = _forward64(cloud, cam, (0.0, 0.0, 0.0), cols, cov3D_precomp, scale_modifier)
         assert np.array_equal(fd.n_contrib, f.n_contrib) and np.array_equal(fd.point_list, f.point_list)
         up = np.zeros((3, H, W), np.float32)
         if gD is not None:
