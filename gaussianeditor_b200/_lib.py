@@ -47,6 +47,8 @@ SYMBOLS = [
     "gsr_shard_backward_render_masked", "gsr_shard_backward_preprocess_masked", "gsr_shard_backward_preprocess_raw_masked",
     "gsr_sparse_backward_preprocess_masked", "gsr_sparse_backward_preprocess_raw_masked",
     "gsr_adam_masked",
+    "gsr_forward_render_mask", "gsr_forward_render_speculative_mask", "gsr_forward_static_mask",
+    "gsr_forward_static_raw_mask",
 ]
 
 
@@ -248,6 +250,11 @@ def load():
     lib.gsr_forward_static.argtypes = [S, Cl, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp]
     lib.gsr_forward_static_raw.restype = C.c_int
     lib.gsr_forward_static_raw.argtypes = [S, RC, i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp]
+    # the _mask twins: the same arguments plus (mask, out_mask_render) before the stream
+    for name in ("gsr_forward_render", "gsr_forward_render_speculative", "gsr_forward_static", "gsr_forward_static_raw"):
+        twin = getattr(lib, name + "_mask")
+        twin.restype = C.c_int
+        twin.argtypes = list(getattr(lib, name).argtypes[:-1]) + [vp, vp, vp]
     lib.gsr_backward_raw.restype = C.c_int
     lib.gsr_backward_raw.argtypes = [S, C.POINTER(RawCloud), i32, vp, sz, vp, sz, vp, sz, vp, vp, vp, sz,
                                      C.POINTER(RawGrads), vp]

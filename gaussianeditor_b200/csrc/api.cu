@@ -267,15 +267,16 @@ static int carve_all(const gsr_settings* s, const gsr_cloud* c, int64_t R, void*
 static int forward_render_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, bool speculative, void* geometry,
                                size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
                                size_t image_bytes, const int32_t* radii, float* out_color, float* out_depth,
-                               void* stream) {
+                               void* stream, const uint8_t* mask = nullptr, float* out_mask = nullptr) {
   int rc = validate_cloud(s, c);
   if (rc) return rc;
   if (!out_color || !out_depth) { set_error("output images are null"); return GSR_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   const size_t npix = (size_t)s->image_width * s->image_height;
-  if (c->P == 0) {  // rasterize_points.cu:72 -- outputs stay zero
+  if (c->P == 0) {  // rasterize_points.cu:72 -- outputs stay zero (the mask image too: it is a forward's colour)
     cudaError_t e = cudaMemsetAsync(out_color, 0, 3 * npix * sizeof(float), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(out_depth, 0, npix * sizeof(float), st);
+    if (e == cudaSuccess && out_mask) e = cudaMemsetAsync(out_mask, 0, 3 * npix * sizeof(float), st);
     return check_cuda(e, "zero outputs");
   }
   GeometryWS g; BinningWS b; ImageWS im;
@@ -284,7 +285,7 @@ static int forward_render_impl(const gsr_settings* s, const gsr_cloud* c, int32_
   rc = run_binning(*s, *c, R, speculative, g, b, im, radii, st);
   if (rc) return rc;
   StageScope t(ST_RENDER_FWD, st);
-  return launch_render_fwd(*s, g, b, im, out_color, out_depth, st);
+  return launch_render_fwd(*s, g, b, im, out_color, out_depth, st, TileOwner(), mask, out_mask);
 }
 
 int gsr_forward_render(const gsr_settings* s, const gsr_cloud* c, int32_t R, void* geometry, size_t geometry_bytes,
@@ -303,6 +304,32 @@ int gsr_forward_render_speculative(const gsr_settings* s, const gsr_cloud* c, in
                              radii, out_color, out_depth, stream);
 }
 
+// the mask image's two arguments of a gsr_*_mask entry point, checked before anything else
+static int check_mask_render(const uint8_t* mask, const float* out_mask_render) {
+  if (!mask) { set_error("mask_render: mask is null"); return GSR_ERR_INVALID; }
+  if (!out_mask_render) { set_error("mask_render: out_mask_render is null"); return GSR_ERR_INVALID; }
+  return GSR_OK;
+}
+
+int gsr_forward_render_mask(const gsr_settings* s, const gsr_cloud* c, int32_t R, void* geometry, size_t geometry_bytes,
+                            void* binning, size_t binning_bytes, void* image, size_t image_bytes, const int32_t* radii,
+                            float* out_color, float* out_depth, const uint8_t* mask, float* out_mask_render,
+                            void* stream) {
+  if (const int rc = check_mask_render(mask, out_mask_render)) return rc;
+  return forward_render_impl(s, c, R, false, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                             out_color, out_depth, stream, mask, out_mask_render);
+}
+
+int gsr_forward_render_speculative_mask(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
+                                        size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                                        size_t image_bytes, const int32_t* radii, float* out_color, float* out_depth,
+                                        const uint8_t* mask, float* out_mask_render, void* stream) {
+  if (const int rc = check_mask_render(mask, out_mask_render)) return rc;
+  if (capacity <= 0) { set_error("speculative capacity must be positive"); return GSR_ERR_INVALID; }
+  return forward_render_impl(s, c, capacity, true, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes,
+                             radii, out_color, out_depth, stream, mask, out_mask_render);
+}
+
 // Both forward halves for a caller-given capacity, with R kept on the device (gsr_forward_static and, with `raw`,
 // gsr_forward_static_raw; `c` is then the raw cloud seen through raw_to_cloud). Every argument is checked before the
 // first launch; the second half is the speculative one, and launch_static_status reports R and empties an overflowing
@@ -310,7 +337,8 @@ int gsr_forward_render_speculative(const gsr_settings* s, const gsr_cloud* c, in
 static int forward_static_impl(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
                                size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
                                size_t image_bytes, int32_t* radii, float* out_color, float* out_depth, int32_t* status,
-                               void* stream, bool raw, const float* features_rest) {
+                               void* stream, bool raw, const float* features_rest, const uint8_t* mask = nullptr,
+                               float* out_mask = nullptr) {
   if (capacity <= 0) { set_error("static capacity must be positive"); return GSR_ERR_INVALID; }
   if (!status) { set_error("status is null"); return GSR_ERR_INVALID; }
   if (!out_color || !out_depth) { set_error("output images are null"); return GSR_ERR_INVALID; }
@@ -320,6 +348,7 @@ static int forward_static_impl(const gsr_settings* s, const gsr_cloud* c, int32_
     cudaError_t e = cudaMemsetAsync(status, 0, 2 * sizeof(int32_t), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(out_color, 0, 3 * npix * sizeof(float), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(out_depth, 0, npix * sizeof(float), st);
+    if (e == cudaSuccess && out_mask) e = cudaMemsetAsync(out_mask, 0, 3 * npix * sizeof(float), st);
     return check_cuda(e, "zero outputs");
   }
   if (!radii || !geometry) { set_error("radii / geometry workspace is null"); return GSR_ERR_INVALID; }
@@ -329,8 +358,8 @@ static int forward_static_impl(const gsr_settings* s, const gsr_cloud* c, int32_
   if ((rc = first_half(*s, *c, g, radii, nullptr, st, raw, features_rest))) return rc;
   if ((rc = run_binning(*s, *c, capacity, true, g, b, im, radii, st))) return rc;
   if ((rc = launch_static_status(*s, c->P, (uint32_t)capacity, g, im, status, st))) return rc;
-  StageScope t(ST_RENDER_FWD, st);
-  return launch_render_fwd(*s, g, b, im, out_color, out_depth, st);
+  StageScope t(ST_RENDER_FWD, st);  // an overflowing frame has empty ranges: both images are the background
+  return launch_render_fwd(*s, g, b, im, out_color, out_depth, st, TileOwner(), mask, out_mask);
 }
 
 int gsr_forward_static(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
@@ -350,6 +379,28 @@ int gsr_forward_static_raw(const gsr_settings* s, const gsr_raw_cloud* r, int32_
   if (rc) return rc;
   return forward_static_impl(s, &c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes,
                              radii, out_color, out_depth, status, stream, true, r->features_rest);
+}
+
+int gsr_forward_static_mask(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
+                            size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                            int32_t* radii, float* out_color, float* out_depth, int32_t* status, const uint8_t* mask,
+                            float* out_mask_render, void* stream) {
+  int rc = check_mask_render(mask, out_mask_render);
+  if (rc || (rc = validate_cloud(s, c))) return rc;
+  return forward_static_impl(s, c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes, radii,
+                             out_color, out_depth, status, stream, false, nullptr, mask, out_mask_render);
+}
+
+int gsr_forward_static_raw_mask(const gsr_settings* s, const gsr_raw_cloud* r, int32_t capacity, void* geometry,
+                                size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                                size_t image_bytes, int32_t* radii, float* out_color, float* out_depth, int32_t* status,
+                                const uint8_t* mask, float* out_mask_render, void* stream) {
+  int rc = check_mask_render(mask, out_mask_render);
+  if (rc) return rc;
+  gsr_cloud c;
+  if ((rc = raw_to_cloud(s, r, c))) return rc;
+  return forward_static_impl(s, &c, capacity, geometry, geometry_bytes, binning, binning_bytes, image, image_bytes,
+                             radii, out_color, out_depth, status, stream, true, r->features_rest, mask, out_mask_render);
 }
 
 static int backward_impl(const gsr_settings* s, const gsr_cloud* c, int32_t R, const void* geometry, size_t geometry_bytes,

@@ -215,8 +215,10 @@ int run_tile_binning(const gsr_settings& s, int P, int R, bool speculative, cons
 int clear_tile_counts(const GeometryWS& g, int gx, int gy, cudaStream_t st);
 // g.R_dev[0] = number of instances in the owned tile rows = a weighted sum over the difference array (no prefix needed)
 int launch_tile_count(const GeometryWS& g, int gx, int gy, const TileOwner& own, cudaStream_t st);
+// mask [P] != nullptr: also the mask image out_mask [3,H,W] (see render_fwd.cu)
 int launch_render_fwd(const gsr_settings& s, const GeometryWS& g, const BinningWS& b, const ImageWS& im,
-                      float* out_color, float* out_depth, cudaStream_t st, const TileOwner& own = TileOwner());
+                      float* out_color, float* out_depth, cudaStream_t st, const TileOwner& own = TileOwner(),
+                      const uint8_t* mask = nullptr, float* out_mask = nullptr);
 // dL_ddepth != nullptr: also the depth image's upstream [H*W]; dL/dz of each splat goes to acc slot 9 (variant 15 only)
 // det != nullptr: deterministic mode: rows + reduction instead of atomics; acc needs no memset (all P rows written)
 // Masked backward (gsr_backward_masked): only Gaussians with grad_mask[i] != 0 take gradients. first[tile] is the

@@ -4,6 +4,7 @@ that is not this repository's hot path stubbed (BASELINE.json configs[4], SURVEY
 Per step, as threestudio/systems/GassuianEditor.py:155-224 + GassuianEditorEdit.py:64-150 + :251-281 do it:
   render(cam, gaussians, pipe, bg)                       forward #1 (SH colours, grad)
   render(cam, ..., override_color=mask)                  forward #2 (colors_precomp path; never back-propagated)
+                                                         (semantic="fused": forward #1's mask_render output instead)
   loss = L1(render, cached edited frame of that view)    (InstructPix2Pix + LPIPS replaced by a fixed target)
   loss.backward()                                        one rasterizer backward
   densification stats from viewspace_points.grad, max_radii2D from radii
@@ -142,7 +143,7 @@ def make_view(cam: synth.Camera, device):
 
 def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densification_interval=100, seed=0,
                   log=None, fused_activations=False, cuda_graph=False, static_capacity=False, deterministic=None,
-                  grad_mask=None, optimizer="adam"):
+                  grad_mask=None, optimizer="adam", semantic="render", semantic_log=None):
     """Returns a dict with total / render wall times (CUDA-event timed) and the per-step Gaussian counts.
     ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only).
     ``cuda_graph=True`` captures one step per Gaussian count and replays it (see the module docstring);
@@ -156,10 +157,17 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
     ``None`` (default): no mask.
     ``optimizer``: ``"adam"`` (default) steps ``torch.optim.Adam``; ``"masked"`` steps ``MaskedAdam`` on the scene's
     mask (rebuilt with the new mask at every densification, inside the captured graph with ``cuda_graph``), which
-    needs a ``grad_mask``."""
+    needs a ``grad_mask``.
+    ``semantic``: where the step's semantic map (the mask drawn in white, thresholded) comes from. ``"render"``
+    (default) renders it as GaussianEditor does, with a second forward ``render(..., override_color=mask)``;
+    ``"fused"`` takes it from forward #1's ``mask_render`` output (``render(..., mask_render=scene.mask)``, this
+    repository's rasterizer only): the same bits without the second forward.
+    ``semantic_log``: None, or a list that receives every step's thresholded semantic map (bool [H,W])."""
     from . import gaussian_renderer as GR
     if grad_mask not in (None, "hooks", "kernel"):
         raise ValueError(f'grad_mask must be None, "hooks" or "kernel", got {grad_mask!r}')
+    if semantic not in ("render", "fused"):
+        raise ValueError(f'semantic must be "render" or "fused", got {semantic!r}')
     _check_optimizer(optimizer, grad_mask)
     fixed = bool(cuda_graph or static_capacity)
     cloud, cams = synth.make_config("c5", P=P)
@@ -168,6 +176,9 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
         scene.apply_grad_mask()
     # the SH render's mask argument, looked up per step: densification replaces scene.mask
     mask_kw = (lambda: {"grad_mask": scene.mask}) if grad_mask == "kernel" else (lambda: {})
+    fused_sem = semantic == "fused"
+    if fused_sem:   # forward #1 also draws the mask
+        mask_kw = (lambda kw=mask_kw: {**kw(), "mask_render": scene.mask})
     views = [make_view(c, device) for c in cams]
     pipe = SimpleNamespace(convert_SHs_python=False, compute_cov3D_python=False, debug=False)
     bg = torch.zeros(3, device=device)
@@ -184,7 +195,8 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                 img = GR.render(v, scene, pipe, bg)["render"]
                 targets.append((img + 0.05 * torch.randn(img.shape, generator=g, device=device)).clamp(0, 1))
         if fixed:
-            loop = _FixedCapacityStep(GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw)
+            loop = _FixedCapacityStep(GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw,
+                                      fused_sem, semantic_log is not None)
         render_ms = 0.0
         counts, losses, radii_trace = [], [], []
         rng = np.random.default_rng(seed)
@@ -196,15 +208,20 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
             k = int(rng.integers(len(views)))
             if fixed:
                 loss = loop.step(k)
+                sem_map = loop.semantic
             else:
                 e0, e1, e2, e3 = ev(), ev(), ev(), ev()
                 e0.record()
-                pkg = GR.render(views[k], scene, pipe, bg, fused_activations=fused_activations, **mask_kw())  # #1
-                sem = GR.render(views[k], scene, pipe, bg,
-                                override_color=scene.mask[..., None].float().repeat(1, 3))["render"]  # forward #2
+                pkg = GR.render(views[k], scene, pipe, bg, fused_activations=fused_activations, **opt,
+                                **mask_kw())                                                          # forward #1
+                if fused_sem:
+                    sem = pkg["mask_render"]
+                else:
+                    sem = GR.render(views[k], scene, pipe, bg,
+                                    override_color=scene.mask[..., None].float().repeat(1, 3))["render"]  # forward #2
                 e1.record()
-                semantic = torch.norm(sem, dim=0) > 0.8                                               # thresholded: no grad
-                loss = 10.0 * (pkg["render"] - targets[k]).abs().mean() + 0.0 * semantic.float().mean()
+                sem_map = torch.norm(sem, dim=0) > 0.8                                                # thresholded: no grad
+                loss = 10.0 * (pkg["render"] - targets[k]).abs().mean() + 0.0 * sem_map.float().mean()
                 scene.optimizer.zero_grad(set_to_none=True)
                 e2.record()
                 loss.backward()                                                                       # rasterizer backward
@@ -216,6 +233,8 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                     scene.add_densification_stats(pkg["viewspace_points"].grad, vis)
                 scene.optimizer.step()
             losses.append(loss.detach())
+            if semantic_log is not None:
+                semantic_log.append(sem_map)
             if step % densification_interval == 0 and step < steps:
                 if fixed:
                     loop.check_capacity()
@@ -443,11 +462,14 @@ class _FixedCapacityStep:
     The capacity is sized once per Gaussian count (`reset`). With `cuda_graph`, the first step after a reset runs eagerly
     on a side stream (it creates Adam's state and warms every lazy initialisation), the second is captured, and every
     step copies its camera and target into the captured input tensors and replays. Overflows are accumulated on the
-    device and read only by `check_capacity`."""
+    device and read only by `check_capacity`. With `fused_semantic` the semantic map comes from forward #1's `mask_render`
+    output (there is no forward #2); with `keep_semantic` each step leaves its own copy of the map in `semantic`."""
 
-    def __init__(self, GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw=dict):
+    def __init__(self, GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw=dict,
+                 fused_semantic=False, keep_semantic=False):
         self.GR, self.scene, self.views, self.targets, self.pipe, self.bg = GR, scene, views, targets, pipe, bg
         self.fused, self.opt, self.cuda_graph, self.mask_kw = fused_activations, opt, cuda_graph, mask_kw
+        self.fused_semantic, self.keep_semantic, self.semantic = fused_semantic, keep_semantic, None
         dev = bg.device
         self.overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         v0 = views[0]
@@ -476,9 +498,15 @@ class _FixedCapacityStep:
         GR, scene = self.GR, self.scene
         pkg = GR.render(view, scene, self.pipe, self.bg, fused_activations=self.fused, static_capacity=self.capacity,
                         **self.opt, **self.mask_kw())                                                 # forward #1
-        sem_pkg = GR.render(view, scene, self.pipe, self.bg, override_color=scene.mask[..., None].float().repeat(1, 3),
-                            static_capacity=self.capacity, **self.opt)                                 # forward #2
-        semantic = torch.norm(sem_pkg["render"], dim=0) > 0.8
+        if self.fused_semantic:   # forward #1's mask image: one status covers both
+            sem_pkg, sem = None, pkg["mask_render"]
+        else:
+            sem_pkg = GR.render(view, scene, self.pipe, self.bg,
+                                override_color=scene.mask[..., None].float().repeat(1, 3),
+                                static_capacity=self.capacity, **self.opt)                             # forward #2
+            sem = sem_pkg["render"]
+        semantic = torch.norm(sem, dim=0) > 0.8
+        self.semantic = semantic
         loss = 10.0 * (pkg["render"] - target).abs().mean() + 0.0 * semantic.float().mean()
         scene.optimizer.zero_grad(set_to_none=True)
         loss.backward()
@@ -488,7 +516,8 @@ class _FixedCapacityStep:
                                                 scene.max_radii2D))
             scene.add_densification_stats_dense(pkg["viewspace_points"].grad, vis)
             torch.maximum(self.overflow, pkg["status"][1:], out=self.overflow)
-            torch.maximum(self.overflow, sem_pkg["status"][1:], out=self.overflow)
+            if sem_pkg is not None:
+                torch.maximum(self.overflow, sem_pkg["status"][1:], out=self.overflow)
         scene.optimizer.step()
         return loss.detach()
 
@@ -512,7 +541,10 @@ class _FixedCapacityStep:
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
                 self.captured = self._body(self.view, self.target)
+            self.captured_semantic = self.semantic
         self.graph.replay()
+        if self.keep_semantic:   # the captured map is overwritten by the next replay
+            self.semantic = self.captured_semantic.clone()
         return self.captured.clone()
 
     def check_capacity(self):

@@ -64,7 +64,7 @@ def _python_sh_colors(pc, camera_center) -> torch.Tensor:
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
            fused_activations: bool = False, depth_grad: bool = False, deterministic=None, static_capacity=None,
-           grad_mask=None):
+           grad_mask=None, mask_render=None):
     """Render the scene; background tensor must be on the GPU. Returns the reference's dictionary:
     render [3,H,W], viewspace_points [P,3] (grad sink for densification), visibility_filter, radii, depth_3dgs.
 
@@ -90,7 +90,13 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     ``grad_mask`` (opt-in, not in the reference; a bool or uint8 CUDA tensor [P], e.g. ``pc.mask``): only the masked
     Gaussians take gradients, every gradient row of the others is +0.0, and the rasterizer skips their backward work
     (``GaussianRasterizer(grad_mask=...)``). It replaces GaussianEditor's ``apply_grad_mask`` hooks; see INTEGRATION.md
-    for the differences."""
+    for the differences.
+
+    ``mask_render`` (opt-in, not in the reference; a bool or uint8 CUDA tensor [P], usually ``pc.mask``): the result
+    also holds ``mask_render`` [3,H,W], the image of the masked Gaussians drawn in white, bit for bit what
+    ``render(..., override_color=mask.float()[:, None].repeat(1, 3))["render"]`` returns, from the same blend pass as
+    ``render`` (``GaussianRasterizer(mask_render=...)``): GaussianEditor's semantic map without its second render. Not
+    differentiable. See INTEGRATION.md 5d."""
     xyz = pc.get_xyz
     # gradient sink for the 2-D means: densification reads its .grad (gaussian_renderer/__init__.py:60-69)
     screenspace_points = torch.zeros_like(xyz, requires_grad=True) + 0
@@ -98,7 +104,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         screenspace_points.retain_grad()
     except Exception:
         pass
-    # depth_grad / deterministic / static_capacity / grad_mask are passed only when asked for: by default the rasterizer is constructed exactly as the
+    # depth_grad / deterministic / static_capacity / grad_mask / mask_render are passed only when asked for: by default the rasterizer is constructed exactly as the
     # reference's render() does, so any class with the reference's constructor (raster_settings only) can stand in for it
     opt = {"depth_grad": True} if depth_grad else {}
     if deterministic is not None:
@@ -107,6 +113,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         opt["static_capacity"] = static_capacity
     if grad_mask is not None:
         opt["grad_mask"] = grad_mask
+    if mask_render is not None:
+        opt["mask_render"] = mask_render
     rasterizer = GaussianRasterizer(
         raster_settings=_settings_for(viewpoint_camera, bg_color, scaling_modifier, pc.active_sh_degree), **opt)
     python_sh = getattr(pipe, "convert_SHs_python", False)
@@ -115,7 +123,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     if fused_activations:
         if override_color is not None or python_sh or python_cov:
             raise ValueError("fused_activations needs the plain SH + scale/rotation path")
-        image, radii, depth = rasterizer.forward_raw(
+        outs = rasterizer.forward_raw(
             means3D=xyz, means2D=screenspace_points, opacity_logits=pc._opacity, features_dc=pc._features_dc,
             features_rest=pc._features_rest, log_scales=pc._scaling, raw_rotations=pc._rotation)
     else:
@@ -130,9 +138,12 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             kw["colors_precomp"] = _python_sh_colors(pc, viewpoint_camera.camera_center)
         else:
             kw["shs"] = pc.get_features.float()
-        image, radii, depth = rasterizer(**kw)
+        outs = rasterizer(**kw)
+    image, radii, depth = outs[:3]
     out = {"render": image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
            "depth_3dgs": depth}
+    if mask_render is not None:
+        out["mask_render"] = outs[-1]
     if static_capacity is not None:
         out["status"] = rasterizer.status
     return out

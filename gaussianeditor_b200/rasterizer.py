@@ -119,12 +119,29 @@ class _ForwardState:
     __slots__ = ("geom", "binning", "img", "radii", "num_rendered", "cap", "P", "M", "W", "H", "mask_first")
 
 
+def _mask_twin(lib, name, mask_render, keep):
+    """(entry point, its name, trailing arguments before the stream): ``name`` itself, or with ``mask_render = (mask,
+    out)`` its _mask twin, which also writes the mask image into ``out`` [3,H,W]. The twins take no NULL pointer, so an
+    empty mask (P = 0) or image (W*H = 0) is handed over as a one-element buffer that is never read or written."""
+    if mask_render is None:
+        return getattr(lib, name), name, ()
+    ptrs = []
+    for t in mask_render:
+        if t.numel() == 0:
+            t = torch.zeros(1, dtype=t.dtype, device=t.device)
+        keep.append(t)
+        ptrs.append(C.c_void_p(t.data_ptr()))
+    return getattr(lib, name + "_mask"), name + "_mask", tuple(ptrs)
+
+
 def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, rs, *, render=True,
-                  raw_rest=None, static=None):
+                  raw_rest=None, static=None, mask_render=None):
     """Both forward halves. With ``raw_rest`` (features_rest [P,K,3]) the call is the fused-activation variant:
     ``sh`` is features_dc [P,1,3] and opacities / scales / rotations are the raw parameters.
     With ``static = (capacity, status)`` both halves run in one gsr_forward_static call sized for ``capacity``: no
-    pinned word, no host wait; num_rendered and the overflow flag land in the device tensor ``status`` int32[2]."""
+    pinned word, no host wait; num_rendered and the overflow flag land in the device tensor ``status`` int32[2].
+    With ``mask_render = (mask, out)`` (uint8 [P], float32 [3,H,W]) the second half also writes the mask image into
+    ``out`` (the _mask twin of each forward entry point)."""
     lib = _lib.load()
     if means3D.dim() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:46-48
@@ -158,7 +175,7 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
         if static is not None:
             cap, status = static
             color, depth = _forward_static(lib, s, c, P, W, H, cap, status, gbytes, state, st, device,
-                                           raw_rest if raw else None)
+                                           raw_rest if raw else None, mask_render)
             inputs = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
             return color, depth, state, inputs + ((raw_rest,) if raw else ())
         pinned = _pinned_i32(device)
@@ -190,10 +207,9 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
             cap = int(hint * 1.25) + 4096
             bbytes = lib.gsr_binning_bytes(P, cap, W, H)
             state.binning = torch.empty(bbytes, **u8)
-            _lib.check(lib.gsr_forward_render_speculative(C.byref(s), C.byref(c), cap, _ptr(state.geom), gbytes,
-                                                          _ptr(state.binning), bbytes, _ptr(state.img), ibytes,
-                                                          _ptr(state.radii), _ptr(color), _ptr(depth), st),
-                       "gsr_forward_render_speculative")
+            fn, name, mr = _mask_twin(lib, "gsr_forward_render_speculative", mask_render, keep)
+            _lib.check(fn(C.byref(s), C.byref(c), cap, _ptr(state.geom), gbytes, _ptr(state.binning), bbytes,
+                          _ptr(state.img), ibytes, _ptr(state.radii), _ptr(color), _ptr(depth), *mr, st), name)
             R = _wait_count(pinned, ev.synchronize)
             SPEC_STATS["launched"] += 1
             if R <= cap:
@@ -206,9 +222,9 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
             bbytes = lib.gsr_binning_bytes(P, R, W, H) if R > 0 else 0
             state.binning = torch.empty(bbytes, **u8)
             if render:
-                _lib.check(lib.gsr_forward_render(C.byref(s), C.byref(c), R, _ptr(state.geom), gbytes,
-                                                  _ptr(state.binning), bbytes, _ptr(state.img), ibytes,
-                                                  _ptr(state.radii), _ptr(color), _ptr(depth), st), "gsr_forward_render")
+                fn, name, mr = _mask_twin(lib, "gsr_forward_render", mask_render, keep)
+                _lib.check(fn(C.byref(s), C.byref(c), R, _ptr(state.geom), gbytes, _ptr(state.binning), bbytes,
+                              _ptr(state.img), ibytes, _ptr(state.radii), _ptr(color), _ptr(depth), *mr, st), name)
         if P > 0:
             _bounded_put(_r_hint, key, max(R, int(0.9 * _r_hint.get(key, 0))))
     inputs = (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
@@ -217,7 +233,7 @@ def _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations, cov
     return color, depth, state, inputs
 
 
-def _forward_static(lib, s, c, P, W, H, cap, status, gbytes, state, st, device, raw_rest):
+def _forward_static(lib, s, c, P, W, H, cap, status, gbytes, state, st, device, raw_rest, mask_render=None):
     """Second half of _forward_impl on the static-capacity path (gsr_forward_static / gsr_forward_static_raw).
     Returns (colour, depth); the state keeps no reference to them (the autograd node holds the state)."""
     u8 = dict(dtype=torch.uint8, device=device)
@@ -230,20 +246,28 @@ def _forward_static(lib, s, c, P, W, H, cap, status, gbytes, state, st, device, 
     color = torch.empty(3, H, W, dtype=torch.float32, device=device)
     depth = torch.empty(1, H, W, dtype=torch.float32, device=device)
     state.num_rendered, state.cap = None, cap   # R is on the device only (status[0])
+    keep = []
+    fn, name, mr = _mask_twin(lib, "gsr_forward_static" if raw_rest is None else "gsr_forward_static_raw", mask_render,
+                              keep)
     args = (cap, _ptr(state.geom), gbytes, _ptr(state.binning), bbytes, _ptr(state.img), ibytes, _ptr(state.radii),
-            _ptr(color), _ptr(depth), C.c_void_p(status.data_ptr()), st)
+            _ptr(color), _ptr(depth), C.c_void_p(status.data_ptr())) + mr + (st,)
     if raw_rest is not None:
         rc = _lib.RawCloud(P, c.means3D, c.opacities, c.shs, _ptr(raw_rest), c.scales, c.rotations)
-        _lib.check(lib.gsr_forward_static_raw(C.byref(s), C.byref(rc), *args), "gsr_forward_static_raw")
+        _lib.check(fn(C.byref(s), C.byref(rc), *args), name)
     else:
-        _lib.check(lib.gsr_forward_static(C.byref(s), C.byref(c), *args), "gsr_forward_static")
+        _lib.check(fn(C.byref(s), C.byref(c), *args), name)
     return color, depth
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, return_alpha=False, camera_grad=False, depth_grad=False, deterministic=False,
-                        static=None):
+                        static=None, mask_render=None):
     rs = raster_settings
+    if mask_render is not None:   # uint8 [P]: the mask image as a trailing output; always the longest argument form
+        cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if camera_grad else (None, None, None)
+        return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                         cov3Ds_precomp, rs, return_alpha, *cam, bool(depth_grad), bool(deterministic),
+                                         static, mask_render)
     if static is not None:   # (capacity, status): gsr_forward_static; always the long argument form
         cam = (rs.viewmatrix, rs.projmatrix, rs.campos) if camera_grad else (None, None, None)
         return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
@@ -272,14 +296,24 @@ def _alpha_image(lib, state, device):
     return alpha
 
 
+def _mask_render_out(mask_render, rs, device):
+    """(mask, out) for _forward_impl, with out the mask image [3,H,W] to be written; None without a mask."""
+    if mask_render is None:
+        return None
+    return mask_render, torch.empty(3, int(rs.image_height), int(rs.image_width), dtype=torch.float32, device=device)
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, return_alpha=False, viewmatrix=None, projmatrix=None, campos=None, depth_grad=False,
-                deterministic=None, static=None):
+                deterministic=None, static=None, mask_render=None):
+        mr = _mask_render_out(mask_render, raster_settings, means3D.device)
         color, depth, state, inputs = _forward_impl(means3D, sh, colors_precomp, opacities, scales, rotations,
-                                                    cov3Ds_precomp, raster_settings, static=static)
+                                                    cov3Ds_precomp, raster_settings, static=static, mask_render=mr)
         ctx.static_form = static is not None
+        ctx.mask_form = mr is not None   # the mask image is a trailing output without a gradient
+        ctx.return_alpha = bool(return_alpha)
         ctx.raster_settings = raster_settings
         ctx.camera_grad = viewmatrix is not None
         ctx.depth_grad = bool(depth_grad)
@@ -294,13 +328,18 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.save_for_backward(*inputs, state.radii, state.geom, state.binning, state.img)
         ctx.mark_non_differentiable(state.radii)
         _RasterizeGaussians.last_state = state  # for parity tests / instrumentation only
+        out = (color, state.radii, depth)
         if return_alpha:   # opt-in fourth output (not in the reference's tuple): alpha = 1 - final_T, differentiable
             with torch.cuda.device(means3D.device):
-                return color, state.radii, depth, _alpha_image(_lib.load(), state, means3D.device)
-        return color, state.radii, depth
+                out = out + (_alpha_image(_lib.load(), state, means3D.device),)
+        if mr is not None:
+            ctx.mark_non_differentiable(mr[1])
+            out = out + (mr[1],)
+        return out
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, *grad_rest):
+        grad_alpha = grad_rest[0] if ctx.return_alpha else None   # the mask image's (last) entry is ignored
         lib = _lib.load()
         rs = ctx.raster_settings
         state = ctx.state
@@ -396,7 +435,9 @@ class _RasterizeGaussians(torch.autograd.Function):
             grads = grads + cam_grads
         if ctx.long_form:   # depth_grad, deterministic
             grads = grads + ((None, None, None) if not ctx.camera_grad else ()) + (None, None)
-        if ctx.static_form:
+        if ctx.static_form or ctx.mask_form:
+            grads = grads + (None,)
+        if ctx.mask_form:
             grads = grads + (None,)
         return grads
 
@@ -407,12 +448,14 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
-                raster_settings, depth_grad=False, deterministic=None, static=None):
+                raster_settings, depth_grad=False, deterministic=None, static=None, mask_render=None):
         empty = torch.empty(0, dtype=torch.float32, device=means3D.device)
+        mr = _mask_render_out(mask_render, raster_settings, means3D.device)
         color, depth, state, inputs = _forward_impl(means3D, features_dc, empty, opacity_logits, log_scales,
                                                     raw_rotations, empty, raster_settings, raw_rest=features_rest,
-                                                    static=static)
+                                                    static=static, mask_render=mr)
         ctx.static_form = static is not None
+        ctx.mask_form = mr is not None
         ctx.raster_settings = raster_settings
         ctx.state = state
         ctx.depth_grad = bool(depth_grad)
@@ -424,10 +467,13 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
         ctx.save_for_backward(m3, dc, rest, op, sc, ro, state.radii, state.geom, state.binning, state.img)
         ctx.mark_non_differentiable(state.radii)
         _RasterizeGaussians.last_state = state
+        if mr is not None:
+            ctx.mark_non_differentiable(mr[1])
+            return color, state.radii, depth, mr[1]
         return color, state.radii, depth
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth):
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_mask_render=None):
         lib = _lib.load()
         rs, state = ctx.raster_settings, ctx.state
         (means3D, dc, rest, logits, log_scales, raw_rot, radii, geom, binning, img) = ctx.saved_tensors
@@ -470,6 +516,8 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                                                     _ptr(binning), binning.numel(), _ptr(img), img.numel(), _ptr(radii),
                                                     _ptr(grad_out_color), _ptr(scratch), sbytes, C.byref(gr), st),
                                "gsr_backward_raw")
+        if ctx.mask_form:   # depth_grad, deterministic, static, mask_render
+            return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None, None, None
         if ctx.static_form:   # depth_grad, deterministic, static
             return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None, None
         if ctx.long_form:   # depth_grad, deterministic
@@ -500,15 +548,16 @@ class _RasterizeGaussiansMasked(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, return_alpha, depth_grad, deterministic, static, grad_mask):
+                raster_settings, return_alpha, depth_grad, deterministic, static, grad_mask, mask_render=None):
         out = _RasterizeGaussians.forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                                           cov3Ds_precomp, raster_settings, return_alpha, None, None, None, depth_grad,
-                                          deterministic, static)
+                                          deterministic, static, mask_render)
         ctx.grad_mask = grad_mask
         return out
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_alpha=None):
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, *grad_rest):
+        grad_alpha = grad_rest[0] if ctx.return_alpha else None   # the mask image's (last) entry is ignored
         lib = _lib.load()
         rs, state = ctx.raster_settings, ctx.state
         (means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, radii, geom, binning,
@@ -544,7 +593,7 @@ class _RasterizeGaussiansMasked(torch.autograd.Function):
                 if scales.numel() == 0:  # cov3D_precomp path: the reference leaves these at their zero-fill
                     dL_dscales.zero_(); dL_drotations.zero_()
         return (dL_dmeans3D, dL_dmeans2D, dL_dsh, dL_dcolors, dL_dopacity, dL_dscales, dL_drotations, dL_dcov3D,
-                None, None, None, None, None, None)
+                None, None, None, None, None, None) + ((None,) if ctx.mask_form else ())
 
 
 class _RasterizeGaussiansRawMasked(torch.autograd.Function):
@@ -553,15 +602,15 @@ class _RasterizeGaussiansRawMasked(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest, log_scales, raw_rotations,
-                raster_settings, depth_grad, deterministic, static, grad_mask):
+                raster_settings, depth_grad, deterministic, static, grad_mask, mask_render=None):
         out = _RasterizeGaussiansRaw.forward(ctx, means3D, means2D, opacity_logits, features_dc, features_rest,
                                              log_scales, raw_rotations, raster_settings, depth_grad, deterministic,
-                                             static)
+                                             static, mask_render)
         ctx.grad_mask = grad_mask
         return out
 
     @staticmethod
-    def backward(ctx, grad_out_color, grad_radii, grad_depth):
+    def backward(ctx, grad_out_color, grad_radii, grad_depth, grad_mask_render=None):
         lib = _lib.load()
         rs, state = ctx.raster_settings, ctx.state
         (means3D, dc, rest, logits, log_scales, raw_rot, radii, geom, binning, img) = ctx.saved_tensors
@@ -591,26 +640,28 @@ class _RasterizeGaussiansRawMasked(torch.autograd.Function):
                                                        sbytes, C.byref(gr), None, _ptr(dscratch), dbytes,
                                                        _ptr(ctx.grad_mask), _ptr(mscratch), mbytes, st),
                            "gsr_backward_raw_masked")
-        return d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None, None, None
+        return (d_m3, d_m2, d_op, d_dc, d_rest, d_sc, d_ro, None, None, None, None, None) + (
+            (None,) if ctx.mask_form else ())
 
 
-def _check_grad_mask(mask, camera_grad, raster_settings):
-    """Constructor checks of ``grad_mask``; returns the mask as uint8 (a bool mask is viewed, not copied)."""
+def _check_grad_mask(mask, camera_grad, raster_settings, name="grad_mask"):
+    """Constructor checks of ``grad_mask`` (or, by ``name``, of another per-Gaussian mask such as ``mask_render``);
+    returns the mask as uint8 (a bool mask is viewed, not copied)."""
     if not isinstance(mask, torch.Tensor):
-        raise ValueError(f"grad_mask must be a torch.Tensor, got {type(mask).__name__}")
+        raise ValueError(f"{name} must be a torch.Tensor, got {type(mask).__name__}")
     if mask.dtype not in (torch.bool, torch.uint8):
-        raise ValueError(f"grad_mask must be a bool or uint8 tensor, got {mask.dtype}")
+        raise ValueError(f"{name} must be a bool or uint8 tensor, got {mask.dtype}")
     if mask.dim() != 1:
-        raise ValueError(f"grad_mask must be 1-D [P], got shape {tuple(mask.shape)}")
+        raise ValueError(f"{name} must be 1-D [P], got shape {tuple(mask.shape)}")
     if not mask.is_cuda:
-        raise ValueError(f"grad_mask must be on the rasterizer's CUDA device, got {mask.device}")
+        raise ValueError(f"{name} must be on the rasterizer's CUDA device, got {mask.device}")
     view = getattr(raster_settings, "viewmatrix", None)
     if isinstance(view, torch.Tensor) and view.is_cuda and view.device != mask.device:
-        raise ValueError(f"grad_mask is on {mask.device}, the camera on {view.device}")
+        raise ValueError(f"{name} is on {mask.device}, the camera on {view.device}")
     if not mask.is_contiguous():
-        raise ValueError("grad_mask must be contiguous")
+        raise ValueError(f"{name} must be contiguous")
     if camera_grad:
-        raise ValueError("grad_mask cannot be combined with camera_grad: the camera gradient sums over every Gaussian")
+        raise ValueError(f"{name} cannot be combined with camera_grad: the camera gradient sums over every Gaussian")
     return mask.view(torch.uint8) if mask.dtype == torch.bool else mask
 
 
@@ -634,7 +685,7 @@ def mark_visible(rs, positions):
 
 class GaussianRasterizer(nn.Module):
     def __init__(self, raster_settings, return_alpha: bool = False, camera_grad: bool = False, depth_grad: bool = False,
-                 deterministic=None, static_capacity=None, grad_mask=None):
+                 deterministic=None, static_capacity=None, grad_mask=None, mask_render=None):
         """``return_alpha=True`` (opt-in, not in the reference) appends a fourth output to ``forward``: the alpha image
         ``1 - final_T`` [1,H,W] (the reference keeps final_T as ``accum_alpha`` but never returns it); it is
         differentiable like the colour.
@@ -667,7 +718,16 @@ class GaussianRasterizer(nn.Module):
         to the rounding of the float atomics otherwise. The forward is unchanged. Combines with ``return_alpha``,
         ``depth_grad``, ``deterministic`` and ``static_capacity``; not with ``camera_grad`` (ValueError). The backward
         reads the tensor given here when it runs: changing it in place between forward and backward is the caller's
-        business, as it is for the hooks."""
+        business, as it is for the hooks.
+        ``mask_render`` (opt-in, for ``forward`` and ``forward_raw``; a bool or uint8 CUDA tensor [P], usually the same
+        tensor as ``grad_mask``): the forward appends one more output after everything it returns otherwise,
+        ``(color, radii, depth[, alpha], mask_render)``, where ``mask_render`` [3,H,W] is the image of the Gaussians with
+        ``mask_render[i] != 0`` drawn in white over the background -- the second forward GaussianEditor runs for its
+        semantic map (``render(..., override_color=mask.float()[:, None].repeat(1, 3))["render"]``), bit for bit, but
+        written by the same blend pass as the colour (gsr_forward_*_mask). Every other output and every gradient is
+        unchanged; ``mask_render`` itself is not differentiable. Combines with every other option, ``camera_grad``
+        included. On ``forward_raw`` the opacity is the in-kernel sigmoid of the logits, so the image matches that
+        second forward on the activated parameters to the last bits only (the rounding note of INTEGRATION.md 5b)."""
         super().__init__()
         self.raster_settings = raster_settings
         self.return_alpha = bool(return_alpha)
@@ -682,14 +742,19 @@ class GaussianRasterizer(nn.Module):
         self.static_capacity = static_capacity
         self.status = None   # device int32[2] {num_rendered, overflow} of the last static-capacity call
         self.grad_mask = None if grad_mask is None else _check_grad_mask(grad_mask, self.camera_grad, raster_settings)
+        self.mask_render = None if mask_render is None else _check_grad_mask(mask_render, False, raster_settings,
+                                                                             "mask_render")
 
-    def _grad_mask(self, means3D):
-        """The uint8 mask for a forward on `means3D`, checked against its device and P."""
-        m = self.grad_mask
+    def _grad_mask(self, means3D, name="grad_mask"):
+        """The uint8 mask ``name`` (grad_mask or mask_render) for a forward on `means3D`, checked against its device and
+        P; None when it is not set."""
+        m = getattr(self, name)
+        if m is None:
+            return None
         if m.device != means3D.device:
-            raise ValueError(f"grad_mask is on {m.device}, means3D on {means3D.device}")
+            raise ValueError(f"{name} is on {m.device}, means3D on {means3D.device}")
         if m.numel() != means3D.size(0):
-            raise ValueError(f"grad_mask has {m.numel()} entries for P = {means3D.size(0)} Gaussians")
+            raise ValueError(f"{name} has {m.numel()} entries for P = {means3D.size(0)} Gaussians")
         return m
 
     def _static(self, device):
@@ -724,10 +789,14 @@ class GaussianRasterizer(nn.Module):
         and the SH concatenation happen inside the preprocess kernels. Same return tuple as ``forward``."""
         det = self._deterministic()
         static = self._static(means3D.device)
+        mr = self._grad_mask(means3D, "mask_render")
         if self.grad_mask is not None:
             return _RasterizeGaussiansRawMasked.apply(means3D, means2D, opacity_logits, features_dc, features_rest,
                                                       log_scales, raw_rotations, self.raster_settings, self.depth_grad,
-                                                      det, static, self._grad_mask(means3D))
+                                                      det, static, self._grad_mask(means3D), *(() if mr is None else (mr,)))
+        if mr is not None:
+            return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
+                                                raw_rotations, self.raster_settings, self.depth_grad, det, static, mr)
         if static is not None:
             return _RasterizeGaussiansRaw.apply(means3D, means2D, opacity_logits, features_dc, features_rest, log_scales,
                                                 raw_rotations, self.raster_settings, self.depth_grad, det, static)
@@ -765,13 +834,15 @@ class GaussianRasterizer(nn.Module):
         if cov3D_precomp is None:
             cov3D_precomp = empty
 
+        mr = self._grad_mask(means3D, "mask_render")
         if self.grad_mask is not None:
             return _RasterizeGaussiansMasked.apply(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                                    cov3D_precomp, raster_settings, self.return_alpha, self.depth_grad,
-                                                   self._deterministic(), static, self._grad_mask(means3D))
+                                                   self._deterministic(), static, self._grad_mask(means3D),
+                                                   *(() if mr is None else (mr,)))
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations,
                                    cov3D_precomp, raster_settings, self.return_alpha, self.camera_grad, self.depth_grad,
-                                   self._deterministic(), static)
+                                   self._deterministic(), static, mr)
 
     def apply_weights(self, means3D, means2D, opacities, shs=None, weights=None, scales=None, rotations=None,
                       cov3Ds_precomp=None, cnt=None, image_weights=None):

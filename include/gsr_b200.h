@@ -361,6 +361,32 @@ GSR_API int gsr_backward_raw_masked(const gsr_settings* s, const gsr_raw_cloud* 
                             void* det_scratch /* may be NULL */, size_t det_scratch_bytes, const uint8_t* grad_mask,
                             void* mask_scratch, size_t mask_scratch_bytes, void* stream);
 
+/* ---- mask image in the colour pass (opt-in; forward only) ---------------------------------------------------------
+ * The _mask twin of a forward entry point takes its arguments plus mask [P] (one byte per Gaussian, device memory) and
+ * out_mask_render [3,H,W] (device memory), and writes, next to its usual outputs, the image of the Gaussians with
+ * mask[i] != 0 drawn in white: what the same forward returns as out_color with colors_precomp[i] = (mask[i] != 0) in
+ * all three channels, bit for bit, including the background, an overflowing static frame (background) and P == 0
+ * (zeros). The blend walk is not repeated: the same pass accumulates one more value per pixel. Every other output is
+ * unchanged. gsr_forward_static_raw_mask takes its opacity from the in-kernel sigmoid, so its mask image matches a
+ * forward on the activated parameters to that rounding only. The image has no backward. A NULL mask or a NULL
+ * out_mask_render returns GSR_ERR_INVALID before any other check or device work. */
+GSR_API int gsr_forward_render_mask(const gsr_settings* s, const gsr_cloud* c, int32_t num_rendered, void* geometry,
+                            size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                            const int32_t* radii, float* out_color, float* out_depth, const uint8_t* mask,
+                            float* out_mask_render, void* stream);
+GSR_API int gsr_forward_render_speculative_mask(const gsr_settings* s, const gsr_cloud* c, int32_t capacity,
+                            void* geometry, size_t geometry_bytes, void* binning, size_t binning_bytes, void* image,
+                            size_t image_bytes, const int32_t* radii, float* out_color, float* out_depth,
+                            const uint8_t* mask, float* out_mask_render, void* stream);
+GSR_API int gsr_forward_static_mask(const gsr_settings* s, const gsr_cloud* c, int32_t capacity, void* geometry,
+                            size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                            int32_t* radii, float* out_color, float* out_depth, int32_t* status, const uint8_t* mask,
+                            float* out_mask_render, void* stream);
+GSR_API int gsr_forward_static_raw_mask(const gsr_settings* s, const gsr_raw_cloud* c, int32_t capacity, void* geometry,
+                            size_t geometry_bytes, void* binning, size_t binning_bytes, void* image, size_t image_bytes,
+                            int32_t* radii, float* out_color, float* out_depth, int32_t* status, const uint8_t* mask,
+                            float* out_mask_render, void* stream);
+
 /* ---- masked Adam (one optimizer step over the Gaussians under edit) ------------------------------------------
  * One Adam step (torch.optim.Adam without weight decay, amsgrad or maximize) over n_groups row-aligned fp32 tensors
  * p, g, m, v of shape [P, D] (row-major, D may differ per group), in one launch, restricted to the rows with

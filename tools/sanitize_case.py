@@ -164,5 +164,28 @@ for bvar in (1, 0):
         col, _, dep = sr.forward_raw(*raw)
         (col * torch.from_numpy(dL).to(dev)).sum().backward()
 _lib.set_option("binning_variant", 1)
+
+# mask image in the colour pass (render_fwd_mask_kernel): exact, speculative hit and miss, static capacity that fits and
+# that overflows, raw static; under a render_fwd_variant that has no mask form
+mk = torch.from_numpy(np.random.default_rng(2).uniform(size=3001) < 0.3).to(dev)
+_lib.set_option("render_fwd_variant", 1)
+for hint in (None, 10 ** 6, 10):
+    RZ._r_hint.pop((0, 3001, cam.image_width, cam.image_height), None)
+    if hint:
+        RZ._r_hint[(0, 3001, cam.image_width, cam.image_height)] = hint
+    ctg = cloud_tensors(cloud, dev, requires_grad=True)
+    out = GaussianRasterizer(rs, mask_render=mk, grad_mask=mk)(
+        means3D=ctg["means3D"], means2D=torch.zeros_like(ctg["means3D"]), opacities=ctg["opacities"], shs=ctg["shs"],
+        scales=ctg["scales"], rotations=ctg["rotations"])
+    (out[0] * torch.from_numpy(dL).to(dev)).sum().backward()
+_lib.set_option("render_fwd_variant", 3)
+for cap in (R_exact, R_exact // 2):
+    sr = GaussianRasterizer(rs, static_capacity=cap, mask_render=mk)
+    ctg = cloud_tensors(cloud, dev, requires_grad=True)
+    out = sr(means3D=ctg["means3D"], means2D=torch.zeros_like(ctg["means3D"]), opacities=ctg["opacities"],
+             shs=ctg["shs"], scales=ctg["scales"], rotations=ctg["rotations"])
+    (out[0] * torch.from_numpy(dL).to(dev)).sum().backward()
+    mk_raw = torch.ones(raw[0].shape[0], dtype=torch.bool, device=dev)   # `raw` is the last cloud of the raw loop above
+    out = GaussianRasterizer(rs, static_capacity=cap, mask_render=mk_raw).forward_raw(*raw)
 torch.cuda.synchronize()
 print("SANITIZE_CASE_DONE")
