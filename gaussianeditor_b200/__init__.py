@@ -8,3 +8,4 @@ Only the one hot path is here (see DESIGN.md): ``csrc/`` holds the hand-written 
 from .rasterizer import (GaussianRasterizationSettings, GaussianRasterizer,  # noqa: F401
                          rasterize_gaussians)
 from .masked_adam import MaskedAdam  # noqa: F401
+from .anchor_loss import anchor_loss  # noqa: F401

@@ -49,6 +49,7 @@ SYMBOLS = [
     "gsr_adam_masked",
     "gsr_forward_render_mask", "gsr_forward_render_speculative_mask", "gsr_forward_static_mask",
     "gsr_forward_static_raw_mask",
+    "gsr_anchor_loss_scratch_bytes", "gsr_anchor_loss_forward", "gsr_anchor_loss_backward",
 ]
 
 
@@ -129,6 +130,13 @@ class AdamGroup(C.Structure):
 
 
 ADAM_MAX_GROUPS = 16   # GSR_ADAM_MAX_GROUPS
+
+
+class AnchorTerm(C.Structure):
+    _fields_ = [("p", C.c_void_p), ("a", C.c_void_p), ("g", C.c_void_p), ("D", C.c_int32)]
+
+
+ANCHOR_TERMS = 6   # GSR_ANCHOR_TERMS
 
 
 _lib = None
@@ -348,6 +356,12 @@ def load():
     lib.gsr_sparse_backward_preprocess_raw_masked.argtypes = [S, RC, SP, vp, sz, vp, vp, sz, vp, sz, RG, i32, u8, vp]
     lib.gsr_adam_masked.restype = C.c_int
     lib.gsr_adam_masked.argtypes = [C.POINTER(AdamGroup), i32, i32, u8, vp]
+    AT = C.POINTER(AnchorTerm)
+    lib.gsr_anchor_loss_scratch_bytes.restype = sz; lib.gsr_anchor_loss_scratch_bytes.argtypes = [i32]
+    lib.gsr_anchor_loss_forward.restype = C.c_int
+    lib.gsr_anchor_loss_forward.argtypes = [AT, i32, u8, vp, vp, i32, vp, sz, vp, vp]
+    lib.gsr_anchor_loss_backward.restype = C.c_int
+    lib.gsr_anchor_loss_backward.argtypes = [AT, i32, u8, vp, vp, i32, vp, sz, vp, vp]
     if lib.gsr_abi_version() != 2:
         raise RuntimeError("libgsr_b200.so ABI version mismatch")
     _lib = lib

@@ -36,9 +36,20 @@ import torch.nn.functional as F
 from . import synth
 from .rasterizer import GaussianRasterizationSettings
 
+# GaussianEditor's anchor-loss settings, as the bear edit script (SURVEY.md's edit shape) sets them
+ANCHOR_WEIGHT_INIT_G0 = 0.01    # first weight of generation 0
+ANCHOR_WEIGHT_INIT = 0.01       # first weight of every later generation
+ANCHOR_WEIGHT_MULTIPLIER = 1.3  # every weight grows by this at each densification ...
+MAX_ANCHOR_WEIGHT = 10          # ... up to this
+ANCHOR_LAMBDA = {"loss_anchor_color": 0.0, "loss_anchor_geo": 50.0, "loss_anchor_opacity": 50.0,
+                 "loss_anchor_scale": 50.0}
+_ANCHOR_GROUP = {"_xyz": "loss_anchor_geo", "_rotation": "loss_anchor_geo", "_features_dc": "loss_anchor_color",
+                 "_features_rest": "loss_anchor_color", "_opacity": "loss_anchor_opacity", "_scaling": "loss_anchor_scale"}
+
 
 class EditScene:
-    def __init__(self, cloud: synth.Cloud, device, capturable: bool = False, optimizer: str = "adam"):
+    def __init__(self, cloud: synth.Cloud, device, capturable: bool = False, optimizer: str = "adam",
+                 track_anchor: bool = False):
         self.capturable = capturable   # Adam(capturable=True): the optimizer step can be captured in a CUDA graph
         self.optimizer_kind = optimizer   # "adam": torch.optim.Adam, "masked": MaskedAdam on `mask`
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
@@ -58,7 +69,37 @@ class EditScene:
         self.xyz_gradient_accum = torch.zeros(P, 1, device=device)
         self.denom = torch.zeros(P, 1, device=device)
         self.hooks = None   # apply_grad_mask: the registered gradient hooks
+        self.anchor = {}    # the reference's default: no anchor, anchor_loss() returns zeros
+        if track_anchor:    # GaussianModel's anchor bookkeeping (scene/gaussian_model.py:62-150)
+            self._generation = torch.zeros(P, dtype=torch.int64, device=device)
+            self._anchor_loss_schedule = torch.tensor([ANCHOR_WEIGHT_INIT_G0], dtype=torch.float32, device=device)
+            self.update_anchor()
         self._make_optimizer()
+
+    def update_anchor(self):
+        """Snapshot the six parameters: the anchor the loss pulls them back to."""
+        self.anchor = {a: getattr(self, a).detach().clone()
+                       for a in ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity")}
+
+    def update_anchor_loss_schedule(self):
+        """After a densification: every generation's weight grows by the multiplier (capped), the generation born
+        at the previous densification starts at the initial weight, and the one born now starts at 0."""
+        s = torch.clamp_max(self._anchor_loss_schedule * ANCHOR_WEIGHT_MULTIPLIER, MAX_ANCHOR_WEIGHT)
+        if s.numel() > 1:   # its last weight was 0 (the reference asserts it), so it multiplied to 0
+            s[-1] = ANCHOR_WEIGHT_INIT
+        self._anchor_loss_schedule = torch.cat([s, s.new_zeros(1)])
+
+    def anchor_loss_torch(self):
+        """GaussianModel.anchor_loss restated in plain torch (boolean indexing, so it synchronises with the host)."""
+        out = {k: 0 for k in ANCHOR_LAMBDA}
+        if not self.anchor:
+            return out
+        w = torch.gather(self._anchor_loss_schedule, 0, self._generation[self.mask])
+        for key, value in self.anchor.items():
+            delta = F.mse_loss(getattr(self, key)[self.mask], value[self.mask], reduction="none")
+            delta = delta * w.view((-1,) + (1,) * (delta.dim() - 1))
+            out[_ANCHOR_GROUP[key]] = out[_ANCHOR_GROUP[key]] + delta.mean()
+        return out
 
     def apply_grad_mask(self):
         """GaussianEditor's ``apply_grad_mask`` (scene/gaussian_model.py:837-856): a hook on each parameter multiplies its
@@ -119,7 +160,8 @@ class EditScene:
             sel = torch.topk(grads, k).indices
             keep = (torch.sigmoid(self._opacity).squeeze(1) >= min_opacity)
             keep[sel] = True
-            idx = torch.cat([torch.nonzero(keep).squeeze(1), sel])
+            kept = torch.nonzero(keep).squeeze(1)
+            idx = torch.cat([kept, sel])
             for name in ("_xyz", "_features_dc", "_features_rest", "_scaling", "_rotation", "_opacity"):
                 setattr(self, name, getattr(self, name).detach()[idx].clone().requires_grad_(True))
             self.mask = self.mask[idx]
@@ -128,6 +170,11 @@ class EditScene:
             self.max_radii2D = torch.zeros(n, device=dev)
             self.xyz_gradient_accum = torch.zeros(n, 1, device=dev)
             self.denom = torch.zeros(n, 1, device=dev)
+            if self.anchor:   # clones are the new generation; then re-anchor and advance the schedule (:712-807)
+                born = torch.full((sel.numel(),), self._anchor_loss_schedule.numel(), dtype=torch.int64, device=dev)
+                self._generation = torch.cat([self._generation[kept], born])
+                self.update_anchor()
+                self.update_anchor_loss_schedule()
             self._make_optimizer()   # the reference re-stitches Adam state; the harness restarts it
         if self.hooks is not None:
             self.apply_grad_mask()
@@ -143,7 +190,7 @@ def make_view(cam: synth.Camera, device):
 
 def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densification_interval=100, seed=0,
                   log=None, fused_activations=False, cuda_graph=False, static_capacity=False, deterministic=None,
-                  grad_mask=None, optimizer="adam", semantic="render", semantic_log=None):
+                  grad_mask=None, optimizer="adam", semantic="render", semantic_log=None, anchor=None):
     """Returns a dict with total / render wall times (CUDA-event timed) and the per-step Gaussian counts.
     ``fused_activations`` renders the SH pass through ``render(..., fused_activations=True)`` (this repository's rasterizer only).
     ``cuda_graph=True`` captures one step per Gaussian count and replays it (see the module docstring);
@@ -162,16 +209,34 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
     (default) renders it as GaussianEditor does, with a second forward ``render(..., override_color=mask)``;
     ``"fused"`` takes it from forward #1's ``mask_render`` output (``render(..., mask_render=scene.mask)``, this
     repository's rasterizer only): the same bits without the second forward.
-    ``semantic_log``: None, or a list that receives every step's thresholded semantic map (bool [H,W])."""
+    ``semantic_log``: None, or a list that receives every step's thresholded semantic map (bool [H,W]).
+    ``anchor``: GaussianEditor's anchor loss. ``None`` (default) leaves it out. ``"torch"`` (``EditScene.anchor_loss_torch``,
+    which synchronises: eager steps only) or ``"kernel"`` (``gaussianeditor_b200.anchor_loss``, capturable) adds
+    ``sum(ANCHOR_LAMBDA[k] * loss[k])`` to every step's loss, with the scene tracking generations, anchors and the weight
+    schedule across densifications; the result then also holds the final ``generation`` and ``anchor_schedule``."""
     from . import gaussian_renderer as GR
     if grad_mask not in (None, "hooks", "kernel"):
         raise ValueError(f'grad_mask must be None, "hooks" or "kernel", got {grad_mask!r}')
     if semantic not in ("render", "fused"):
         raise ValueError(f'semantic must be "render" or "fused", got {semantic!r}')
+    if anchor not in (None, "torch", "kernel"):
+        raise ValueError(f'anchor must be None, "torch" or "kernel", got {anchor!r}')
     _check_optimizer(optimizer, grad_mask)
     fixed = bool(cuda_graph or static_capacity)
+    if anchor == "torch" and fixed:
+        raise ValueError('anchor="torch" synchronises with the host (boolean indexing): it cannot run in the '
+                         'static-capacity or CUDA-graph step; use anchor="kernel"')
     cloud, cams = synth.make_config("c5", P=P)
-    scene = EditScene(cloud, device, capturable=fixed, optimizer=optimizer)
+    scene = EditScene(cloud, device, capturable=fixed, optimizer=optimizer, track_anchor=anchor is not None)
+    anchor_term = None
+    if anchor is not None:
+        from .anchor_loss import anchor_loss
+        anchor_fn = scene.anchor_loss_torch if anchor == "torch" else (lambda: anchor_loss(scene))
+
+        def anchor_term(loss):   # GassuianEditorEdit.training_step: loss += value * lambda, key by key
+            for k, v in anchor_fn().items():
+                loss = loss + v * ANCHOR_LAMBDA[k]
+            return loss
     if grad_mask == "hooks":
         scene.apply_grad_mask()
     # the SH render's mask argument, looked up per step: densification replaces scene.mask
@@ -196,7 +261,7 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                 targets.append((img + 0.05 * torch.randn(img.shape, generator=g, device=device)).clamp(0, 1))
         if fixed:
             loop = _FixedCapacityStep(GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw,
-                                      fused_sem, semantic_log is not None)
+                                      fused_sem, semantic_log is not None, anchor_term)
         render_ms = 0.0
         counts, losses, radii_trace = [], [], []
         rng = np.random.default_rng(seed)
@@ -222,6 +287,8 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                 e1.record()
                 sem_map = torch.norm(sem, dim=0) > 0.8                                                # thresholded: no grad
                 loss = 10.0 * (pkg["render"] - targets[k]).abs().mean() + 0.0 * sem_map.float().mean()
+                if anchor_term is not None:
+                    loss = anchor_term(loss)
                 scene.optimizer.zero_grad(set_to_none=True)
                 e2.record()
                 loss.backward()                                                                       # rasterizer backward
@@ -258,6 +325,8 @@ def run_edit_loop(rasterizer_cls, steps=200, P=None, device="cuda", densificatio
                max_radii2D_at_densify=[r.cpu() for r in radii_trace],
                params={n: getattr(scene, a).detach() for n, a in _SCENE_ATTR.items()}, optimizer=scene.optimizer,
                mask=scene.mask)
+    if anchor is not None:
+        out.update(generation=scene._generation, anchor_schedule=scene._anchor_loss_schedule)
     if fixed:   # the step is not split by events: no render time
         out.update(render_ms=None, render_fraction=None, capacities=loop.capacities)
     return out
@@ -463,13 +532,15 @@ class _FixedCapacityStep:
     on a side stream (it creates Adam's state and warms every lazy initialisation), the second is captured, and every
     step copies its camera and target into the captured input tensors and replays. Overflows are accumulated on the
     device and read only by `check_capacity`. With `fused_semantic` the semantic map comes from forward #1's `mask_render`
-    output (there is no forward #2); with `keep_semantic` each step leaves its own copy of the map in `semantic`."""
+    output (there is no forward #2); with `keep_semantic` each step leaves its own copy of the map in `semantic`.
+    `anchor_term`, when given, adds the anchor loss to the step's loss (it must not synchronise)."""
 
     def __init__(self, GR, scene, views, targets, pipe, bg, fused_activations, opt, cuda_graph, mask_kw=dict,
-                 fused_semantic=False, keep_semantic=False):
+                 fused_semantic=False, keep_semantic=False, anchor_term=None):
         self.GR, self.scene, self.views, self.targets, self.pipe, self.bg = GR, scene, views, targets, pipe, bg
         self.fused, self.opt, self.cuda_graph, self.mask_kw = fused_activations, opt, cuda_graph, mask_kw
         self.fused_semantic, self.keep_semantic, self.semantic = fused_semantic, keep_semantic, None
+        self.anchor_term = anchor_term
         dev = bg.device
         self.overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         v0 = views[0]
@@ -508,6 +579,8 @@ class _FixedCapacityStep:
         semantic = torch.norm(sem, dim=0) > 0.8
         self.semantic = semantic
         loss = 10.0 * (pkg["render"] - target).abs().mean() + 0.0 * semantic.float().mean()
+        if self.anchor_term is not None:
+            loss = self.anchor_term(loss)
         scene.optimizer.zero_grad(set_to_none=True)
         loss.backward()
         with torch.no_grad():

@@ -416,6 +416,39 @@ typedef struct gsr_adam_group {
 GSR_API int gsr_adam_masked(const gsr_adam_group* groups, int32_t n_groups, int32_t P, const uint8_t* mask,
                             void* stream);
 
+/* ---- anchor loss (GaussianEditor's per-step anchor regularizer, GaussianModel.anchor_loss) -------------------------
+ * terms: exactly GSR_ANCHOR_TERMS row-aligned fp32 [P, D] pairs, in GaussianModel.update_anchor's order
+ * (_xyz, _features_dc, _features_rest, _scaling, _rotation, _opacity): p the parameter, a its anchor snapshot, g its
+ * gradient (backward only). With w_i = schedule[generation[i]] and N_m the number of rows with mask[i] != 0:
+ *   L_k = sum over edited rows i, j < D_k of w_i * (p_k[i,j] - a_k[i,j])^2 / (N_m * D_k)
+ * accumulated in fp64 and rounded to fp32, and out4 = (L_dc + L_rest, L_xyz + L_rot, L_opacity, L_scale) added in
+ * fp32: the reference dict's (color, geo, opacity, scale). A term without elements (N_m == 0 or D == 0) is NaN, as
+ * torch's mean of an empty tensor. A generation outside [0, n_schedule) gives the row a NaN weight (never an
+ * out-of-bounds read; torch.gather would trap instead). The sums run in a fixed order over a grid that depends on P
+ * only, with no float atomics: the result is bit-reproducible.
+ * gsr_anchor_loss_forward writes out4 (device [4]) and keeps N_m in the scratch (device, at least
+ * gsr_anchor_loss_scratch_bytes(P)) for gsr_anchor_loss_backward, which takes that scratch unchanged and
+ * grad_out4 (device [4], the gradients of out4) and writes all six g in one launch: on an edited row
+ * g = 2 (p - a) ((grad_out4[group] / (float)(N_m D)) w), the order of torch's mean and mse backward, with -0 written as
+ * +0; on every other row +0.0, without reading p or a. Neither call synchronises with the host: both can be captured
+ * in a CUDA graph. GSR_ERR_INVALID, before any device work: NULL terms or schedule, P < 0, n_schedule < 1, NULL mask or
+ * generation with P > 0, D < 0 or D > GSR_ADAM_MAX_D, a NULL p or a (and g, backward) in a term with P * D > 0, a NULL
+ * out4 / grad_out4, a NULL or too small scratch. */
+#define GSR_ANCHOR_TERMS 6
+typedef struct gsr_anchor_term {
+  const float* p;
+  const float* a;
+  float* g;          /* backward only; may be NULL in the forward */
+  int32_t D;         /* floats per row */
+} gsr_anchor_term;
+GSR_API size_t gsr_anchor_loss_scratch_bytes(int32_t P);
+GSR_API int gsr_anchor_loss_forward(const gsr_anchor_term* terms, int32_t P, const uint8_t* mask,
+                            const int64_t* generation, const float* schedule, int32_t n_schedule, void* scratch,
+                            size_t scratch_bytes, float* out4, void* stream);
+GSR_API int gsr_anchor_loss_backward(const gsr_anchor_term* terms, int32_t P, const uint8_t* mask,
+                            const int64_t* generation, const float* schedule, int32_t n_schedule, const void* scratch,
+                            size_t scratch_bytes, const float* grad_out4, void* stream);
+
 /* ---- Gaussian-sharded multi-GPU path (BASELINE config 4; SURVEY.md 8(e)) ----------------------------------
  * The reference has no multi-GPU rasterizer; these entry points split the single-GPU pipeline at the two places
  * where the Gaussian-index decomposition (preprocess, fused preprocess backward) meets the tile decomposition
