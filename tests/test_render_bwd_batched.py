@@ -1,7 +1,7 @@
 """render_bwd variant 15 (csrc/render_bwd.cu: the per-splat moment reduction deferred and batched through shared
 memory) against the reference, the fp64 CPU oracle, variant 14 and the sharded path.
 
-Every test pins the variant with ``_options``: other tests leave render_bwd_variant at other values when they finish.
+Every test pins the variant with ``_options``, which restores the value it found.
 Reference values fall back to the ones recorded under tests/golden/parity/ when the compiled reference is absent; they do
 not depend on our variant.
 """
