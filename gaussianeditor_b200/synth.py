@@ -418,6 +418,148 @@ def one_tile_cloud(P: int, W: int = 1024, H: int = 1024, seed: int = 0):
     return Cloud(xyz, _tiny_splats(rng, P).astype(np.float32), _random_quats(rng, P), opac, _sh_dc(rng, P, 0), 0), cam
 
 
+# ---- camera models -----------------------------------------------------------------------------------------------
+# Cameras that look_at_camera cannot build: unequal focal lengths (PINHOLE intrinsics, resized frames), rolled and
+# arbitrary rotations, very wide and very narrow fields of view, and a camera inside the cloud. Scenes are sampled in
+# view space and carried to the world through the camera's inverse pose, so every pose sees its content.
+
+def pinhole_camera(R_w2c, t, W: int, H: int, fx: float, fy: float) -> Camera:
+    """GaussianEditor's ``Camera`` for the world-to-camera rotation ``R_w2c`` and translation ``t`` (camera coordinates
+    R_w2c @ x + t) and focal lengths fx, fy in pixels: FoVx = focal2fov(fx, W), FoVy = focal2fov(fy, H), the
+    projection of both FoVs, world_view_transform = W2C^T, full_proj_transform = world_view_transform @ P^T."""
+    R = np.asarray(R_w2c, np.float64)
+    t = np.asarray(t, np.float64)
+    W2C = np.eye(4)
+    W2C[:3, :3] = R
+    W2C[:3, 3] = t
+    tanx = math.tan(0.5 * (2.0 * math.atan(W / (2.0 * fx))))
+    tany = math.tan(0.5 * (2.0 * math.atan(H / (2.0 * fy))))
+    P = _projection(0.01, 100.0, tanx, tany)
+    view_t = np.ascontiguousarray(W2C.astype(np.float32).T)
+    proj_t = np.ascontiguousarray((view_t @ P.T).astype(np.float32))
+    return Camera(H, W, float(tanx), float(tany), view_t, proj_t, (-R.T @ t).astype(np.float32))
+
+
+def origin_aspect_focals(fx: float, fy: float, origin_w: int, origin_h: int, W: int, H: int):
+    """The focal lengths in pixels of a ``W`` x ``H`` render of a PINHOLE intrinsic (fx, fy) of an ``origin_w`` x
+    ``origin_h`` image, as GaussianEditor's COLMAP reader sets the FoVs when the aspect changes (readColmapCameras_hw:
+    the longer side is cropped to the new aspect)."""
+    aspect = H / W
+    if origin_h / origin_w > aspect:           # shrink height
+        fovy, fovx = 2 * math.atan(origin_w * aspect / (2 * fy)), 2 * math.atan(origin_w / (2 * fx))
+    else:                                      # shrink width
+        fovy, fovx = 2 * math.atan(origin_h / (2 * fy)), 2 * math.atan(origin_h / aspect / (2 * fx))
+    return W / (2 * math.tan(fovx / 2)), H / (2 * math.tan(fovy / 2))
+
+
+def random_rotation(rng, min_entry: float = 0.0) -> np.ndarray:
+    """A uniformly random rotation matrix (QR of a Gaussian matrix), redrawn until every entry has |R_ij| >= min_entry."""
+    while True:
+        Q, Rr = np.linalg.qr(rng.standard_normal((3, 3)))
+        Q = Q * np.sign(np.diag(Rr))[None, :]
+        if np.linalg.det(Q) < 0:
+            Q[:, 0] = -Q[:, 0]
+        if np.abs(Q).min() >= min_entry:
+            return Q
+
+
+def _sh3(rng, P):
+    shs = np.zeros((P, 16, 3), np.float32)
+    shs[:, 0, :] = ((rng.uniform(size=(P, 3)) - 0.5) / SH_C0).astype(np.float32)
+    k = 1
+    for ell in range(1, 4):
+        shs[:, k:k + 2 * ell + 1, :] = rng.standard_normal((P, 2 * ell + 1, 3)) * (0.15 / (1 + ell))
+        k += 2 * ell + 1
+    return shs
+
+
+def _to_world(cam: Camera, xyz_view):
+    """View-space points -> world space through the inverse of the camera's pose."""
+    W2C = cam.viewmatrix.astype(np.float64).T
+    R, t = W2C[:3, :3], W2C[:3, 3]
+    return (np.asarray(xyz_view, np.float64) - t[None, :]) @ R
+
+
+def view_space_cloud(cam: Camera, P: int, seed: int, near_frac: float = 0.1, clamp_frac: float = 0.2,
+                     beyond_frac: float = 0.05) -> Cloud:
+    """``P`` Gaussians sampled in ``cam``'s view space -> Cloud (world space), SH degree 3, random rotations:
+      * ``near_frac`` at view depths in (0.2, 0.3], just beyond the near cut, centres inside the frame;
+      * ``clamp_frac`` with |x/z|, |y/z| or both within 5 % of 1.3 tan(fov) (the Jacobian clamp), depths 0.5..20;
+      * ``beyond_frac`` with centres 1.4..1.8 tan(fov) off axis in x or y (beyond the clamp), their scale large enough
+        that the 3-sigma radius still reaches into the frame;
+      * the rest inside the frame at depths 0.3..30.
+    Projected sizes are 0.3..30 px per axis (in the larger focal length's pixels), opacities 0.05..0.95 (0.005..0.095
+    beyond the clamp)."""
+    rng = np.random.default_rng(seed)
+    tan = np.array([cam.tanfovx, cam.tanfovy])
+    f = max(cam.image_width / (2 * cam.tanfovx), cam.image_height / (2 * cam.tanfovy))
+    n_near, n_clamp, n_beyond = int(near_frac * P), int(clamp_frac * P), int(beyond_frac * P)
+    n_in = P - n_near - n_clamp - n_beyond
+    z = np.concatenate([rng.uniform(0.2, 0.3, n_near), np.exp(rng.uniform(np.log(0.3), np.log(30.0), n_in)),
+                        np.exp(rng.uniform(np.log(0.5), np.log(20.0), n_clamp + n_beyond))])
+    z[:n_near] = np.maximum(z[:n_near], np.nextafter(np.float32(0.2), np.float32(1)))
+    uv = rng.uniform(-0.9, 0.9, (P, 2)) * tan                         # x/z, y/z
+    sgn = np.where(rng.uniform(size=(P, 2)) < 0.5, -1.0, 1.0)
+    which = rng.integers(0, 3, P)                                     # x, y or both at the clamp / beyond
+    axis = np.stack([which != 1, which != 0], 1)
+    c0, c1 = n_near + n_in, n_near + n_in + n_clamp
+    uv[c0:c1] = np.where(axis[c0:c1], sgn[c0:c1] * 1.3 * tan * rng.uniform(0.95, 1.05, (n_clamp, 2)), uv[c0:c1])
+    off = rng.uniform(1.4, 1.8, (n_beyond, 2))
+    uv[c1:] = np.where(axis[c1:], sgn[c1:] * off * tan, uv[c1:])
+    sigma = np.exp(rng.uniform(np.log(0.3), np.log(30.0), (P, 1))) * np.exp(rng.uniform(-0.7, 0.7, (P, 3)))
+    scales = sigma * z[:, None] / f
+    # beyond: 3 sigma_min of the isotropic part at least 1.2x the distance from the centre to the frame's edge
+    reach = (np.where(axis[c1:], off - 1.0, 0.0) * tan * z[c1:, None]).max(1)
+    scales[c1:] = (1.2 * reach / 3.0)[:, None] * np.exp(rng.uniform(0.0, 0.5, (n_beyond, 3)))
+    xyz = _to_world(cam, np.concatenate([uv * z[:, None], z[:, None]], 1))
+    opac = rng.uniform(0.05, 0.95, (P, 1))
+    opac[c1:] *= 0.1                     # the large off-frame splats: translucent, or together they hide the frame
+    return Cloud(xyz.astype(np.float32), scales.astype(np.float32), _random_quats(rng, P), opac.astype(np.float32),
+                 _sh3(rng, P), 3)
+
+
+def camera_family(P: int = 3000, seed: int = 0) -> dict:
+    """Named (Cloud, Camera) cases, every frame at most 640x480, seeded:
+      aniso_0.5, aniso_2   fy / fx = 0.5 on 640x480 and 2 on 333x201, random poses;
+      pinhole_resized      a 1297x840 PINHOLE intrinsic with fx != fy rendered at 512x512 (origin_aspect_focals);
+      wide_120             fovx 120 degrees (tan 1.73), square pixels;
+      tele_4               fovx 4 degrees (focal length 9160 px);
+      roll_90              camera x = world +y, camera y = world -x: view[0] = 0, view[4] = 1;
+      general              a random rotation with every entry at least 0.05 in magnitude;
+      nadir                looking straight down world +y (look_at_camera with up (0, -1, 0) is degenerate there);
+      inside               the eye at the centre of a bicycle_cloud of 2P (size 0.3), Gaussians in every direction, a few
+                           of them large enough near the eye to cover the whole frame."""
+    rng = np.random.default_rng(seed)
+    out = {}
+
+    def add(name, R, W, H, fx, fy, t=None):
+        t = rng.normal(0.0, 2.0, 3) if t is None else t
+        cam = pinhole_camera(R, t, W, H, fx, fy)
+        out[name] = (view_space_cloud(cam, P, seed=int(rng.integers(1 << 30))), cam)
+
+    add("aniso_0.5", random_rotation(rng), 640, 480, 520.0, 260.0)
+    add("aniso_2", random_rotation(rng), 333, 201, 190.0, 380.0)
+    add("pinhole_resized", random_rotation(rng), 512, 512, *origin_aspect_focals(1160.0, 1090.0, 1297, 840, 512, 512))
+    fx = 320.0 / math.tan(math.radians(60.0))
+    add("wide_120", random_rotation(rng), 640, 480, fx, fx)
+    fx = 320.0 / math.tan(math.radians(2.0))
+    add("tele_4", random_rotation(rng), 640, 480, fx, fx)
+    add("roll_90", np.array([[0.0, 1, 0], [-1, 0, 0], [0, 0, 1]]), 640, 480, 500.0, 500.0)
+    add("general", random_rotation(rng, min_entry=0.05), 640, 480, 560.0, 480.0)
+    add("nadir", np.array([[1.0, 0, 0], [0, 0, -1], [0, 1, 0]]), 480, 360, 420.0, 420.0)
+    # inside: eye at the origin of the bicycle cloud; eight large Gaussians just in front of it cover the frame
+    cam = pinhole_camera(random_rotation(rng), np.zeros(3), 640, 480, 500.0, 450.0)
+    base = bicycle_cloud(2 * P, seed=int(rng.integers(1 << 30)), size=0.3)
+    n = 8
+    big_view = np.concatenate([rng.uniform(-0.1, 0.1, (n, 2)), rng.uniform(0.4, 1.5, (n, 1))], 1)
+    big = Cloud(_to_world(cam, big_view).astype(np.float32),
+                (big_view[:, 2:] * rng.uniform(1.0, 2.0, (n, 3))).astype(np.float32), _random_quats(rng, n),
+                rng.uniform(0.02, 0.1, (n, 1)).astype(np.float32), _sh3(rng, n), 3)
+    out["inside"] = (Cloud(*(np.ascontiguousarray(np.concatenate([getattr(base, k), getattr(big, k)]))
+                             for k in ("means3D", "scales", "rotations", "opacities", "shs")), 3), cam)
+    return out
+
+
 CONFIGS = {
     # name: (P, sh_degree, W, H)
     "c1": dict(P=10_000, sh_degree=0, W=256, H=256),

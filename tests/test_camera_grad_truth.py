@@ -737,9 +737,13 @@ def test_pose_chain():
     torch ops) equals the same chain in fp64 applied to the truth. Checks the layout and transposition of the returned
     .grad tensors."""
     cloud, cam = _base_cloud()
-    w2c0 = np.asarray(cam.viewmatrix, np.float64).T
+    pose_chain(cloud, cam, np.asarray(cam.viewmatrix, np.float64).T, np.array([0.02, -0.03, 0.015, 0.05, -0.02, 0.04]))
+
+
+def pose_chain(cloud, cam, w2c0, p0, case="pose_chain"):
+    """The camera of pose p0 (axis-angle, translation) applied to the world-to-camera matrix w2c0, with ``cam``'s frame
+    and fields of view: pose.grad on the GPU against the fp64 chain of the truth."""
     projT = np.asarray(synth._projection(0.01, 100.0, cam.tanfovx, cam.tanfovy), np.float64).T
-    p0 = np.array([0.02, -0.03, 0.015, 0.05, -0.02, 0.04])
     pose = torch.tensor(p0, dtype=torch.float32, device="cuda", requires_grad=True)
     view, full, campos = _pose_camera(pose, torch.tensor(w2c0, dtype=torch.float32, device="cuda"),
                                       torch.tensor(projT, dtype=torch.float32, device="cuda"))
@@ -762,5 +766,5 @@ def test_pose_chain():
     B = np.concatenate([r["B"][k].reshape(-1) for k in CAM])
     want, Bp = J.T @ t, np.abs(J).T @ B
     ratio, rel = float((np.abs(got - want) / Bp).max()), rel_l2(got, want)
-    print(f"CAMSTAT pose_chain max|got-truth|/B={ratio:.3e} relL2={rel:.3e}")
-    assert ratio <= TAU and rel <= RHO_POSE, (got, want, ratio, rel)
+    print(f"CAMSTAT {case} max|got-truth|/B={ratio:.3e} relL2={rel:.3e}")
+    assert ratio <= TAU and rel <= RHO_POSE, (case, got, want, ratio, rel)

@@ -22,20 +22,21 @@ A_MAX = float(np.float32(0.99))   # the alpha clamp 0.99f of the forward
 
 # ---- the fp64 truth ------------------------------------------------------------------------------------------------
 
-def _forward64(cloud, cam, bg, colors_precomp=None, cov3D_precomp=None, scale_modifier=1.0):
+def _forward64(cloud, cam, bg, colors_precomp=None, cov3D_precomp=None, scale_modifier=1.0, f32=False):
     kw = dict(scale_modifier=scale_modifier)
     if colors_precomp is not None:
         kw["colors_precomp"] = colors_precomp
     if cov3D_precomp is not None:
         kw.update(cov3D_precomp=cov3D_precomp, scales=None, rotations=None)
-    return O.forward_from(cloud, cam, bg, f32=False, **kw)
+    return O.forward_from(cloud, cam, bg, f32=f32, **kw)
 
 
 def depth_truth(cloud, cam, bg, gC=None, gD=None, gA=None, colors_precomp=None, cov3D_precomp=None,
-                scale_modifier=1.0):
+                scale_modifier=1.0, f32=False):
     """fp64 gradients of  sum gC*colour + sum gD*depth + sum gA*alpha  (each upstream optional). Returns the oracle's
-    gradient dict plus ``ddepth`` [P] (dL/dz per Gaussian), and the colour-pass forward as ``fwd``."""
-    f = _forward64(cloud, cam, bg, colors_precomp, cov3D_precomp, scale_modifier)
+    gradient dict plus ``ddepth`` [P] (dL/dz per Gaussian), and the colour-pass forward as ``fwd``. ``f32=True``: the
+    same construction on the fp32 oracle (the reference's arithmetic), to measure how far fp32 lies from the truth."""
+    f = _forward64(cloud, cam, bg, colors_precomp, cov3D_precomp, scale_modifier, f32)
     P, M, H, W = f.P, f.M, f.H, f.W
     if gC is not None:
         g = f.backward(np.asarray(gC, np.float32))
@@ -48,7 +49,7 @@ def depth_truth(cloud, cam, bg, gC=None, gD=None, gA=None, colors_precomp=None, 
         hi = f.depths.astype(np.float32)
         lo = (f.depths - hi.astype(np.float64)).astype(np.float32)
         cols = np.stack([hi, lo, np.ones(P, np.float32)], 1)
-        fd = _forward64(cloud, cam, (0.0, 0.0, 0.0), cols, cov3D_precomp, scale_modifier)
+        fd = _forward64(cloud, cam, (0.0, 0.0, 0.0), cols, cov3D_precomp, scale_modifier, f32)
         assert np.array_equal(fd.n_contrib, f.n_contrib) and np.array_equal(fd.point_list, f.point_list)
         up = np.zeros((3, H, W), np.float32)
         if gD is not None:

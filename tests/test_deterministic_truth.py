@@ -294,19 +294,20 @@ def _run(cloud, cam, bg, gC, gD=None, gA=None, colors_precomp=None, grad_mask=No
     return {k: v.grad.detach().cpu().numpy() for k, v in leaves.items()}, tt
 
 
-def _truth(cloud, cam, bg, form, gC, gD):
+def _truth(cloud, cam, bg, form, gC, gD, f32=False):
     """fp64 gradients of the loss of `form`. colour: the oracle's backward. depth: test_depth_grad.depth_truth. alpha:
     sum gC*colour + sum gC[0]*alpha has the gradient of sum gC*colour with background (bg0 - 1, bg1, bg2), because
-    colour_0 with that background is C_0 + alpha - 1 (test_parity_gpu: the alpha output test)."""
+    colour_0 with that background is C_0 + alpha - 1 (test_parity_gpu: the alpha output test). ``f32=True``: the same
+    on the fp32 oracle."""
     from oracle import cpu_oracle
     from test_depth_grad import depth_truth
     if form == "depth":
-        g = depth_truth(cloud, cam, bg, gC=gC, gD=gD)
+        g = depth_truth(cloud, cam, bg, gC=gC, gD=gD, f32=f32)
         g["fwd"].close()
         return g
     if form == "alpha":
         bg = (bg[0] - 1.0, bg[1], bg[2])
-    f = cpu_oracle.forward_from(cloud, cam, bg, f32=False)
+    f = cpu_oracle.forward_from(cloud, cam, bg, f32=f32)
     try:
         return f.backward(gC)
     finally:

@@ -217,7 +217,15 @@ def test_gradients_match_fp64_finite_differences():
     cloud = synth.Cloud(xyz.astype(np.float32), sc.astype(np.float32), q.astype(np.float32), op.astype(np.float32),
                         sh.astype(np.float32), 3)
     G = rng.uniform(size=(3, 32, 40)).astype(np.float32).astype(np.float64)
-    bg = (0.3, 0.1, 0.6)
+    g = check_finite_differences(cloud, cam, G, (0.3, 0.1, 0.6), rng)
+    # dmean2D is the gradient w.r.t. the NDC-scaled screen position: checked through its chain into dmean3D above;
+    # its z component is identically zero and invisible Gaussians get exact zeros
+    assert np.all(g["dmean2D"][:, 2] == 0)
+
+
+def check_finite_differences(cloud, cam, G, bg, rng):
+    """Directional fp64 finite differences of loss = sum(color * G) against the fp64 oracle's gradient of every
+    differentiable input (means3D, scales, rotations, opacities, shs); returns the oracle's gradients."""
     loss0, g, nc0, radii0 = _loss_and_grads(cloud, cam, G, bg)
     fields = [("means3D", "dmean3D"), ("scales", "dscale"), ("rotations", "drot"), ("opacities", "dopacity"),
               ("shs", "dsh")]
@@ -245,9 +253,7 @@ def test_gradients_match_fp64_finite_differences():
                     ok += 1
         # undetected alpha<1/255 crossings of non-final contributors can still spoil a direction; most must agree
         assert tried >= 6 and ok >= 0.7 * tried, (field, ok, tried)
-    # dmean2D is the gradient w.r.t. the NDC-scaled screen position: checked through its chain into dmean3D above;
-    # its z component is identically zero and invisible Gaussians get exact zeros
-    assert np.all(g["dmean2D"][:, 2] == 0)
+    return g
 
 
 def test_apply_weights_counts():

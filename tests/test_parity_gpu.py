@@ -99,9 +99,10 @@ class _Ref:
     """The reference's values for one test case: computed by ``compute()`` from oracle/_ref when it is built, otherwise
     read from tests/golden/parity/reference_outputs.npz (recorded from it by tools/make_golden.py). Recorded per value:
     its SHA-256 digest (bit-exact checks), size and max |value|; the value itself when it has at most 64 entries or is
-    named in ``full``; a seeded sample of REF_SAMPLE entries when it is named in ``close`` (compared to a tolerance)."""
+    named in ``full``; a seeded sample of REF_SAMPLE entries when it is named in ``close`` (compared to a tolerance).
+    ``golden``: the recorded file to read."""
 
-    def __init__(self, key, compute, close=(), full=()):
+    def __init__(self, key, compute, close=(), full=(), golden=REF_GOLDEN):
         self.key = key
         self.live = ref_cuda.available()
         if self.live:
@@ -116,9 +117,9 @@ class _Ref:
                     elif k in close:
                         RECORD[f"{key}/{k}#sample"] = a.ravel()[_sample_index(a.size)]
         else:
-            if not os.path.exists(REF_GOLDEN):
-                pytest.fail("tests/golden/parity/reference_outputs.npz missing (tools/make_golden.py writes it)")
-            self.z = np.load(REF_GOLDEN)
+            if not os.path.exists(golden):
+                pytest.fail(f"{os.path.relpath(golden)} missing (tools/make_golden.py writes it)")
+            self.z = np.load(golden)
             if f"{key}/" not in {k[:len(key) + 1] for k in self.z.files}:
                 pytest.fail(f"no recorded reference values for {key}")
 

@@ -8,7 +8,9 @@ are what pins the CPU oracle and our kernels to the reference's actual outputs w
                                   seeded sample of every gradient with its noise floor and max |value|;
   * reference_outputs.npz         (goes to tests/golden/parity/) every other reference value test_parity_gpu compares
                                   with: the tests that use test_parity_gpu._Ref are run here against the live reference
-                                  (their assertions included) and what they computed from it is recorded.
+                                  (their assertions included) and what they computed from it is recorded;
+  * camera_models_reference.npz   (goes to tests/golden/parity/) the same for tests/test_camera_models.py, written alone
+                                  by   python tools/make_golden.py OUT_DIR camera_models
 """
 import os
 import sys
@@ -68,6 +70,12 @@ def main():
     OUT = sys.argv[1]
     os.makedirs(OUT, exist_ok=True)
     assert T.ref_cuda.available(), "oracle/_ref/libdgr_ref.so is not built"
+    if sys.argv[2:] == ["camera_models"]:
+        import test_camera_models as CM
+        np.savez_compressed(os.path.join(OUT, "camera_models_reference.npz"),
+                            **record((CM.test_forward_mark_visible_apply_weights_match_reference,)))
+        print("golden written to", OUT)
+        return
     c3, _ = synth.make_config("c3", P=400)
     case("c3_p400_deg3", c3, synth.ring_cameras(8, 4.5, 15.0, 72, 56, 61.0)[2], (0.1, 0.3, 0.6), seed=1)
     c1, _ = synth.make_config("c1", P=300)
