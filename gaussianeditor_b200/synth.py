@@ -418,6 +418,76 @@ def one_tile_cloud(P: int, W: int = 1024, H: int = 1024, seed: int = 0):
     return Cloud(xyz, _tiny_splats(rng, P).astype(np.float32), _random_quats(rng, P), opac, _sh_dc(rng, P, 0), 0), cam
 
 
+# ---- frame geometry ------------------------------------------------------------------------------------------------
+def grid_camera(W: int, H: int) -> Camera:
+    """_origin_camera with the 60-degree field of view across the frame's longer side (square pixels), so that frames
+    one tile tall and one tile wide alike keep their centres away from the Jacobian clamp."""
+    if W >= H:
+        return _origin_camera(W, H)
+    return look_at_camera((0, 0, 0), (0, 0, 1), (0, -1, 0), W, H, fovy_deg=60.0)
+
+
+def _iso_scales(cam: Camera, xyz, r):
+    """Isotropic scales that give splats centred at xyz (world = view up to signs, grid_camera) the integer radius r
+    with half a pixel to spare: 3 sqrt(lambda_max) = r - 0.5. With J J^T = (f/z)^2 [[1 + u^2, uv], [uv, 1 + v^2]] the
+    eigenvalues of s^2 J J^T + 0.3 are a + 0.3 and a (1 + u^2 + v^2) + 0.3 (a = (s f / z)^2), and the reference takes
+    mid + sqrt(max(0.1, spread^2))."""
+    f = cam.image_width / (2.0 * cam.tanfovx)
+    z = xyz[:, 2]
+    w2 = (xyz[:, 0] ** 2 + xyz[:, 1] ** 2) / z ** 2
+    lam = ((np.asarray(r, np.float64) - 0.5) / 3.0) ** 2
+    a = (lam - 0.3) / (1.0 + w2)
+    small = a * w2 / 2.0 < np.sqrt(0.1)
+    a = np.where(small, (lam - 0.3 - np.sqrt(0.1)) / (1.0 + w2 / 2.0), a)
+    assert (a > 0).all()
+    return np.sqrt(a) * z / f
+
+
+def tile_grid_cloud(W: int, H: int, seed: int = 0, fill: int = 16384):
+    """Isotropic Gaussians for a W x H frame of grid_camera -> (Cloud, Camera), laid out for the tile-binning tests:
+      * one splat of radius 3..12 px in every tile row and one in every tile column, so every row and column of the tile
+        grid holds instances;
+      * ``fill`` splats of radius 3..24 px in the left 60 % of the frame, so R spans several 4096-instance sort tiles
+        at every frame size while tiles in the right part stay empty (on grids of 50 tiles or more, at least two wide and
+        tall);
+      * three splats of radius 0.4 x the long side (at most 4000 px) and opacity 0.03..0.1 behind the others, each over
+        hundreds of tiles along the long axis where the grid has them;
+      * depths drawn from 97 values, so equal depth keys meet in many tiles.
+    Centres sit at half-pixels and radii have half a pixel to spare, so fp32 rounding cannot move a tile edge. The rows
+    are shuffled: kinds and tied depths interleave in index order. SH degree 0."""
+    rng = np.random.default_rng(seed)
+    cam = grid_camera(W, H)
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    half = lambda lo, hi: np.floor(rng.uniform(lo, hi)) + 0.5          # half-pixel centres in [lo, hi)
+    ty, tx = np.arange(gy), np.arange(gx)
+    rows_py = half(16.0 * ty, np.minimum(16.0 * ty + 16.0, H))
+    cols_px = half(16.0 * tx, np.minimum(16.0 * tx + 16.0, W))
+    px = np.concatenate([half(np.zeros(gy), np.full(gy, W)), cols_px, half(np.zeros(fill), np.full(fill, 0.6 * W))])
+    py = np.concatenate([rows_py, half(np.zeros(gx), np.full(gx, H)), half(np.zeros(fill), np.full(fill, H))])
+    n_small = gy + gx
+    r = np.concatenate([rng.integers(3, 13, n_small), rng.integers(3, 25, fill)])
+    z = rng.choice(np.linspace(2.0, 8.0, 97), n_small + fill)
+    opac = np.concatenate([rng.uniform(0.2, 0.8, n_small), rng.uniform(0.05, 0.5, fill)])
+    long_side = max(W, H)
+    rb = max(3, min(4000, int(0.4 * long_side)))
+    big = 3
+    bx = half(np.full(big, 0.25 * W), np.full(big, 0.35 * W))
+    by = half(np.full(big, 0.4 * H), np.full(big, 0.6 * H))
+    px, py = np.concatenate([px, bx]), np.concatenate([py, by])
+    r = np.concatenate([r, np.full(big, rb)])
+    z = np.concatenate([z, [8.5, 9.0, 9.5]])
+    opac = np.concatenate([opac, rng.uniform(0.03, 0.1, big)])
+    perm = rng.permutation(px.size)
+    px, py, r, z, opac = px[perm], py[perm], r[perm], z[perm], opac[perm]
+    P = px.size
+    xyz = _at_pixels(cam, px, py, z)
+    s = _iso_scales(cam, xyz, r)
+    cloud = Cloud(xyz.astype(np.float32), np.repeat(s[:, None], 3, 1).astype(np.float32),
+                  np.tile(np.array([[1.0, 0.0, 0.0, 0.0]], np.float32), (P, 1)), opac.astype(np.float32)[:, None],
+                  _sh_dc(rng, P, 0), 0)
+    return cloud, cam
+
+
 # ---- camera models -----------------------------------------------------------------------------------------------
 # Cameras that look_at_camera cannot build: unequal focal lengths (PINHOLE intrinsics, resized frames), rolled and
 # arbitrary rotations, very wide and very narrow fields of view, and a camera inside the cloud. Scenes are sampled in

@@ -11,6 +11,8 @@ are what pins the CPU oracle and our kernels to the reference's actual outputs w
                                   (their assertions included) and what they computed from it is recorded;
   * camera_models_reference.npz   (goes to tests/golden/parity/) the same for tests/test_camera_models.py, written alone
                                   by   python tools/make_golden.py OUT_DIR camera_models
+  * tile_grid_reference.npz       (goes to tests/golden/parity/) the same for tests/test_tile_grid.py, written alone by
+                                  python tools/make_golden.py OUT_DIR tile_grid
 """
 import os
 import sys
@@ -74,6 +76,13 @@ def main():
         import test_camera_models as CM
         np.savez_compressed(os.path.join(OUT, "camera_models_reference.npz"),
                             **record((CM.test_forward_mark_visible_apply_weights_match_reference,)))
+        print("golden written to", OUT)
+        return
+    if sys.argv[2:] == ["tile_grid"]:
+        import test_tile_grid as TG
+        np.savez_compressed(os.path.join(OUT, "tile_grid_reference.npz"),
+                            **record((TG.test_lists_and_forward, TG.test_backward_against_truth,
+                                     TG.test_wide_backward_against_reference)))
         print("golden written to", OUT)
         return
     c3, _ = synth.make_config("c3", P=400)
