@@ -372,13 +372,28 @@ using std::max;
 using std::min;
 #endif
 
+// float -> int as the device converts it (cvt.rzi.s32.f32): toward zero, saturating at INT_MIN / INT_MAX, NaN -> 0.
+// On the device this is the plain cast; a host cast of an out-of-range value is undefined (INT_MIN on x86), so the host
+// build spells the device's rule out. A radius of INT_MAX (an overflowed 2-D covariance) then covers the whole grid on
+// both sides.
+__host__ __device__ __forceinline__ int f2i_rz(float v) {
+#ifdef __CUDA_ARCH__
+  return (int)v;
+#else
+  if (v != v) return 0;
+  if (v >= 2147483648.0f) return 2147483647;
+  if (v <= -2147483648.0f) return -2147483647 - 1;
+  return (int)v;
+#endif
+}
+
 // tile rectangle [rmin, rmax) of a splat (auxiliary.h:46-56); binning and the deterministic kernels share it
 __host__ __device__ __forceinline__ void tile_rect(float px, float py, int radius, int gx, int gy, uint2& rmin,
                                                    uint2& rmax) {
-  rmin.x = (unsigned)min(gx, max((int)0, (int)((px - radius) / TILE)));
-  rmin.y = (unsigned)min(gy, max((int)0, (int)((py - radius) / TILE)));
-  rmax.x = (unsigned)min(gx, max((int)0, (int)((px + radius + TILE - 1) / TILE)));
-  rmax.y = (unsigned)min(gy, max((int)0, (int)((py + radius + TILE - 1) / TILE)));
+  rmin.x = (unsigned)min(gx, max((int)0, f2i_rz((px - radius) / TILE)));
+  rmin.y = (unsigned)min(gy, max((int)0, f2i_rz((py - radius) / TILE)));
+  rmax.x = (unsigned)min(gx, max((int)0, f2i_rz((px + radius + TILE - 1) / TILE)));
+  rmax.y = (unsigned)min(gy, max((int)0, f2i_rz((py + radius + TILE - 1) / TILE)));
 }
 // Rows of the rectangle [ymin, ymax) this rank owns (ty % stride == phase): first owned row and their number.
 __host__ __device__ __forceinline__ void owned_rows(uint32_t ymin, uint32_t ymax, int stride, int phase, uint32_t& y0,

@@ -167,7 +167,9 @@ __device__ __forceinline__ void finish_and_add(float* dst, float tot, float sw, 
   const float nBx = -B * ddelx_dx, nBy = -B * ddely_dy;
   const float ka = role.is_x ? -A * ddelx_dx : (role.is_y ? -C * ddely_dy : role.kconst);
   const float kb = role.is_x ? nBx : (role.is_y ? nBy : 0.0f);
-  const float v = fmaf(kb, other, ka * tot);
+  // only the two mean moments take the other axis: kb = 0 elsewhere, and 0 * other would turn a NaN moment of the conic
+  // (a splat whose overflowed 2-D covariance gives a NaN conic) into a NaN colour gradient the reference does not have
+  const float v = (role.is_x || role.is_y) ? fmaf(kb, other, ka * tot) : ka * tot;
   if (role.writer) atomicAdd(dst + role.slot, v);
   if (role.opac) atomicAdd(dst + 8, __fdividef(sw, o));  // dL/dopacity = sum G*dL_dalpha = (sum w) / o
 }
@@ -436,8 +438,10 @@ __device__ __forceinline__ void flush_moments(const float4* part4, uint32_t jpac
     const float nAx = -s0.z * ddelx_dx, nCy = -s1.x * ddely_dy, nBx = -s0.w * ddelx_dx, nBy = -s0.w * ddely_dy;
     const float ka = is_x ? nAx : (is_y ? nCy : (m < 3 ? 1.0f : -0.5f));
     const float kb = is_x ? nBx : (is_y ? nBy : 0.0f);
-    if constexpr (DET) dst[m] = fmaf(kb, other, ka * tot);
-    else atomicAdd(dst + m, fmaf(kb, other, ka * tot));
+    // kb * other only on the two mean moments (see finish_and_add: a NaN conic moment must not reach the colour rows)
+    const float v = (is_x || is_y) ? fmaf(kb, other, ka * tot) : ka * tot;
+    if constexpr (DET) dst[m] = v;
+    else atomicAdd(dst + m, v);
     if constexpr (DEPTH) {
       if (m < 2) {  // lane m = 0: opacity into slot 8, lane m = 1: dL/dz into slot 9
         float rcp;

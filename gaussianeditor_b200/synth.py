@@ -630,6 +630,282 @@ def camera_family(P: int = 3000, seed: int = 0) -> dict:
     return out
 
 
+# ---- magnitude scenes ----------------------------------------------------------------------------------------------
+# Inputs at the magnitudes trained clouds reach: scales that vanish or overflow in fp32, screen radii past 2^24 and
+# 2^31, 2-D covariances whose determinant is decided by rounding, scenes far from the origin or in other units.
+
+def _fma32(a, b, c):
+    """fp32 fma: the product of two floats is exact in fp64, the sum rounds once in fp64 and again to fp32 (the double
+    rounding differs from the device only on an exact fp32 tie, which does not occur in these scenes)."""
+    return np.asarray(np.asarray(a, np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64), np.float32)
+
+
+def preprocess_fp32(cloud: Cloud, cam: Camera) -> dict:
+    """The forward preprocess's covariance, conic and radius arithmetic, operation for operation as the kernels (and the
+    reference's CUDA build) round it at sm_90a (csrc/preprocess_fwd_body.inc), in numpy: the generators use it to put
+    Gaussians on rounding edges. Keys: depth, means2D, cov3D [P,6], cov2 [P,3] (a, b, c), det, conic [P,3],
+    radius_f (3 sqrt(lambda_max) rounded up, before the conversion), radius (saturated as cvt.rzi.s32.f32; 0 where
+    the near cut or det == 0 culls)."""
+    f32 = lambda a: np.asarray(a, np.float32)
+    with np.errstate(all="ignore"):
+        m, v, pm = f32(cloud.means3D), f32(cam.viewmatrix).reshape(-1), f32(cam.projmatrix).reshape(-1)
+        x, y, z = m[:, 0], m[:, 1], m[:, 2]
+        tp = lambda M, i: f32(_fma32(M[8 + i], z, _fma32(M[0 + i], x, np.float32(M[4 + i] * y))) + M[12 + i])
+        t = [tp(v, 0), tp(v, 1), tp(v, 2)]
+        hx, hy, hw = tp(pm, 0), tp(pm, 1), tp(pm, 3)
+        pw = f32(1) / f32(hw + f32(1e-7))
+        ndc = lambda p, S: f32(((p.astype(np.float64) + 1.0) * S - 1.0) * 0.5)
+        means2D = np.stack([ndc(f32(hx * pw), cam.image_width), ndc(f32(hy * pw), cam.image_height)], 1)
+        s = f32(cloud.scales)
+        q = f32(cloud.rotations)
+        r, qx, qy, qz = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+        xz, rx, rz, yy, zz = qx * qz, r * qx, r * qz, qy * qy, qz * qz
+        e02, e20, e12 = _fma32(r, qy, xz), _fma32(-r, qy, xz), _fma32(qy, qz, -rx)
+        e21, e01, e10 = _fma32(qy, qz, rx), _fma32(qx, qy, -rz), _fma32(qx, qy, rz)
+        q00, q11, q22 = f32(yy + zz), _fma32(qx, qx, zz), _fma32(qx, qx, yy)
+        R = [[f32(1) - (q00 + q00), e01 + e01, e02 + e02], [e10 + e10, f32(1) - (q11 + q11), e12 + e12],
+             [e20 + e20, e21 + e21, f32(1) - (q22 + q22)]]
+        Mm = [[s[:, k] * R[c][k] for k in range(3)] for c in range(3)]
+        sig = lambda c, k: _fma32(Mm[k][2], Mm[c][2], _fma32(Mm[k][0], Mm[c][0], Mm[k][1] * Mm[c][1]))
+        V = [sig(0, 0), sig(0, 1), sig(0, 2), sig(1, 1), sig(1, 2), sig(2, 2)]
+        focal_x = f32(cam.image_width / f32(2.0 * f32(cam.tanfovx)))
+        focal_y = f32(cam.image_height / f32(2.0 * f32(cam.tanfovy)))
+        limx, limy = f32(1.3) * f32(cam.tanfovx), f32(1.3) * f32(cam.tanfovy)
+        tx = np.minimum(limx, np.maximum(-limx, t[0] / t[2])) * t[2]
+        ty = np.minimum(limy, np.maximum(-limy, t[1] / t[2])) * t[2]
+        tz2 = t[2] * t[2]
+        J00, J02 = focal_x / t[2], (-tx * focal_x) / tz2
+        J11, J12 = focal_y / t[2], (-ty * focal_y) / tz2
+        T00, T01, T02 = _fma32(v[2], J02, v[0] * J00), _fma32(v[6], J02, v[4] * J00), _fma32(v[10], J02, v[8] * J00)
+        T10, T11, T12 = _fma32(v[2], J12, v[1] * J11), _fma32(v[6], J12, v[5] * J11), _fma32(v[10], J12, v[9] * J11)
+        V00, V01, V02, V11, V12, V22 = V
+        A00 = _fma32(T02, V02, _fma32(T00, V00, T01 * V01))
+        A01 = _fma32(T12, V02, _fma32(T10, V00, T11 * V01))
+        A10 = _fma32(T02, V12, _fma32(T00, V01, T01 * V11))
+        A11 = _fma32(T12, V12, _fma32(T10, V01, T11 * V11))
+        A20 = _fma32(T02, V22, _fma32(T00, V02, T01 * V12))
+        A21 = _fma32(T12, V22, _fma32(T10, V02, T11 * V12))
+        ca = f32(_fma32(T02, A20, _fma32(T00, A00, T01 * A10)) + f32(0.3))
+        cb = _fma32(T02, A21, _fma32(T00, A01, T01 * A11))
+        cc = f32(_fma32(T12, A21, _fma32(T10, A01, T11 * A11)) + f32(0.3))
+        det = _fma32(ca, cc, -(cb * cb))
+        dinv = f32(1) / det
+        conic = np.stack([cc * dinv, cb * -dinv, ca * dinv], 1)
+        mid = (ca + cc) * f32(0.5)
+        disc = np.sqrt(np.fmax(f32(0.1), _fma32(mid, mid, -det)))
+        lam = np.fmax(mid + disc, mid - disc)
+        radius_f = np.ceil(f32(3) * np.sqrt(lam))
+        rad = np.where(np.isnan(radius_f), 0, np.clip(np.nan_to_num(radius_f.astype(np.float64), posinf=2.0 ** 31),
+                                                     -2.0 ** 31, 2.0 ** 31 - 1)).astype(np.int64)
+        rad = np.where((t[2] > f32(0.2)) & (det != 0), rad, 0)
+    return dict(depth=t[2], means2D=means2D, cov3D=np.stack(V, 1), cov2=np.stack([ca, cb, cc], 1), det=det,
+                conic=conic, radius_f=radius_f, radius=rad)
+
+
+def _pix_to_view(cam: Camera, px, py, z):
+    """View-space point that projects to pixel (px, py) at view depth z (ndc from the tangents, as _at_pixels)."""
+    vx = ((np.asarray(px, np.float64) + 0.5) * 2.0 / cam.image_width - 1.0) * cam.tanfovx * z
+    vy = ((np.asarray(py, np.float64) + 0.5) * 2.0 / cam.image_height - 1.0) * cam.tanfovy * z
+    return np.stack([vx, vy, np.asarray(z, np.float64)], -1)
+
+
+MAGNITUDE_RADII = (16777215.0, 16777216.0, 16777218.0, 2147483520.0, 2147483648.0, 2147483904.0, 1e10, 1e12)
+
+
+def magnitude_cloud(seed: int = 0):
+    """Gaussians at the magnitudes trained clouds reach, 320x200 (a partial last tile row), camera at the origin looking
+    down +z (view (x, y, z) = world (-x, -y, z) exactly), SH degree 3 -> (Cloud, Camera, groups), groups: name -> row
+    indices. Every input is finite; only intermediates overflow or underflow. Front to back:
+      opacity_*      opacities denormal, 0, fp32(1/255) and its two neighbours, 1; `sh_1e30` SH coefficients up to 1e30;
+                     `clamp_zero` colours whose `+ 0.5` lands on exactly 0 in every channel (not clamped: the test is < 0);
+      vanishing      isotropic scales 10^k, k = -30..-4: cov3D denormal or 0, the 2-D covariance the 0.3 dilation alone
+                     (radius 3); `vanishing_mixed`: two such axes and one ordinary;
+      cancel_tiny / cancel_negative   needles with axis ratios 1e4..1e8 and ~1e4 px long axes whose det a c - b^2
+                     rounds to a small positive value (a conic of 1e3 and more) and below 0 (power > 0 almost everywhere:
+                     binned, hardly ever blended); `cancel_zero`: needles with one non-zero axis whose det is exactly 0
+                     (culled), built as described below;
+      radius_edge    isotropic splats with 3 sqrt(lambda_max) = MAGNITUDE_RADII in fp32: just below, on and above 2^24,
+                     2^31 - 1 (2147483520, then 2^31 and 2147483904, which saturate to INT_MAX) and beyond;
+      overflow       isotropic scales 1e12 .. 1.8e19 (cov3D stays finite, sqrt(FLT_MAX) = 1.84e19): the 2-D covariance
+                     reaches inf from 1e17 on, the conic is NaN and alpha = fminf(0.99, NaN) = 0.99 over the whole grid;
+                     `overflow_rotated`: anisotropic and rotated, b = +-inf or NaN as well.
+    The camera's tangents are 0.5 and 0.3125, so focal_x = focal_y = 320 exactly. Those far-back overflow splats are placed where no row of the scene's cov2 diagonal becomes NaN: a NaN radius converts
+    to 0 and leaves the reference's tile count without instances (its instance slots unwritten)."""
+    rng = np.random.default_rng(seed)
+    W, H = 320, 200
+    # tan(fovx / 2) = 0.5 and tan(fovy / 2) = 0.3125 exactly: focal_x = focal_y = 320 in fp32 (cancel_zero needs both)
+    cam = look_at_camera((0, 0, 0), (0, 0, 1), (0, -1, 0), W, H, fovx_deg=math.degrees(2.0 * math.atan(0.5)))
+    fx = W / (2.0 * cam.tanfovx)
+    rows, groups = [], {}
+
+    def add(name, view_xyz, scales, quats, opac, shs=None):
+        n = len(scales)
+        start = sum(len(r[1]) for r in rows)
+        groups[name] = np.arange(start, start + n)
+        world = np.asarray(view_xyz, np.float64) * np.array([-1.0, -1.0, 1.0])
+        sh = _sh3(rng, n) if shs is None else shs
+        rows.append((world.astype(np.float32), np.asarray(scales, np.float32), np.asarray(quats, np.float32),
+                     np.asarray(opac, np.float32).reshape(n, 1), sh.astype(np.float32)))
+
+    def on_frame(n, z0, z1):
+        z = rng.uniform(z0, z1, n)
+        return _pix_to_view(cam, rng.uniform(8, W - 8, n), rng.uniform(8, H - 8, n), z)
+
+    # colour and opacity extremes (front): splats of 4..10 px
+    o255 = np.float32(1.0 / 255.0)
+    ops = [np.float32(1e-40), np.float32(1e-45), np.float32(0.0), np.nextafter(o255, np.float32(0)), o255,
+           np.nextafter(o255, np.float32(1)), np.float32(1.0)]
+    names = ["opacity_denormal", "opacity_denormal_min", "opacity_zero", "opacity_255_below", "opacity_255",
+             "opacity_255_above", "opacity_one"]
+    for nm, o in zip(names, ops):
+        n = 4
+        p = on_frame(n, 1.0, 2.0)
+        add(nm, p, (p[:, 2:] * rng.uniform(4, 10, (n, 3)) / fx), _random_quats(rng, n), np.full(n, o))
+    n = 8
+    p = on_frame(n, 1.0, 2.0)
+    sh = _sh3(rng, n)
+    sh[:, :, :] *= np.float32(10.0) ** rng.integers(20, 31, (n, 16, 1))        # up to 1e30
+    add("sh_1e30", p, p[:, 2:] * rng.uniform(3, 8, (n, 3)) / fx, _random_quats(rng, n), rng.uniform(0.3, 0.9, n), sh)
+    # clamp_zero: DC only, fp32(SH_C0) * sh0 rounds to exactly -0.5, so the colour is -0.5 + 0.5 = +0 in every channel
+    c0 = np.float32(SH_C0)
+    cand = np.float32(-0.5 / SH_C0) + np.arange(-8, 9).astype(np.float32) * np.spacing(np.float32(-0.5 / SH_C0))
+    sh0 = cand[(c0 * cand) == np.float32(-0.5)]
+    assert sh0.size, "no fp32 coefficient with SH_C0 * c == -0.5"
+    n = 6
+    p = on_frame(n, 1.0, 2.0)
+    sh = np.zeros((n, 16, 3), np.float32)
+    sh[:, 0, :] = sh0[0]
+    add("clamp_zero", p, p[:, 2:] * rng.uniform(3, 8, (n, 3)) / fx, _random_quats(rng, n), rng.uniform(0.3, 0.9, n), sh)
+    # vanishing
+    k = np.arange(-30, -3)
+    n = k.size
+    p = on_frame(n, 2.0, 5.0)
+    add("vanishing", p, np.repeat((10.0 ** k)[:, None], 3, 1), _random_quats(rng, n), rng.uniform(0.3, 0.9, n))
+    p = on_frame(n, 2.0, 5.0)
+    s = np.repeat((10.0 ** k)[:, None], 3, 1)
+    s[np.arange(n), rng.integers(0, 3, n)] = p[:, 2] * rng.uniform(3, 8, n) / fx
+    add("vanishing_mixed", p, s, _random_quats(rng, n), rng.uniform(0.3, 0.9, n))
+    # cancelling determinant: needles in the image plane (rotation about the view axis, tilt <= 2 degrees)
+    N = 20000
+    p = on_frame(N, 8.0, 12.0)
+    s_long = 1e4 * p[:, 2] / fx
+    ratio = 10.0 ** rng.uniform(4, 8, N)
+    s = np.stack([s_long, s_long / ratio, s_long / ratio * rng.uniform(0.5, 2.0, N)], 1)
+    q = _quat_mul(_axis_quats((0, 0, 1), rng.uniform(0, np.pi, N)), _axis_quats((0, 1, 0), np.radians(rng.uniform(-2, 2, N))))
+    trial = Cloud((p * np.array([-1.0, -1.0, 1.0])).astype(np.float32), s.astype(np.float32), q.astype(np.float32),
+                  np.ones((N, 1), np.float32), np.zeros((N, 16, 3), np.float32), 3)
+    f = preprocess_fp32(trial, cam)
+    det, cmax = f["det"], np.abs(f["conic"]).max(1)
+    pick = {"cancel_tiny": np.flatnonzero((det > 0) & (cmax >= 1e3))[:8], "cancel_negative": np.flatnonzero(det < 0)[:8]}
+    for nm, idx in pick.items():
+        add(nm, p[idx], s[idx], q[idx], rng.uniform(0.2, 0.6, idx.size))
+    # cancel_zero: with fma the determinant is a*c - round(b^2) exactly, 0 only if a*c fits in fp32. A needle with one
+    # non-zero axis on the optical axis (J02 = J12 = 0) under an unnormalised quaternion (r, 0, 0, z) with
+    # 1 - 2 z^2 == 2 r z in fp32 has V00 = V11 = V01 = (s R00)^2; with s R00 = 2^k and view depth 320 / 2^j the three
+    # entries of the 2-D covariance are all 2^24 (the 0.3 rounds away), and det = 2^48 - 2^48 = 0
+    zq = (np.float32(math.sin(math.pi / 8)).view(np.int32) + np.arange(-60, 61)).astype(np.int32).view(np.float32)
+    rq = (np.float32(math.cos(math.pi / 8)).view(np.int32) + np.arange(-60, 61)).astype(np.int32).view(np.float32)
+    Z, Rq = np.meshgrid(zq, rq)
+    R00 = np.float32(1) - (Z * Z + Z * Z)
+    eq = R00 == (Rq * Z) + (Rq * Z)
+    zs, rs, rho = Z[eq], Rq[eq], R00[eq]
+    for i, (depth, m) in enumerate(((10.0, 128.0), (20.0, 256.0), (40.0, 512.0))):
+        sx = (np.float32(m / rho[i]).view(np.int32) + np.arange(-20, 21)).astype(np.int32).view(np.float32)
+        n = sx.size
+        tr = Cloud(np.tile(np.array([[0, 0, depth]], np.float32), (n, 1)),
+                   np.stack([sx, np.zeros(n, np.float32), np.zeros(n, np.float32)], 1),
+                   np.tile(np.array([[rs[i], 0, 0, zs[i]]], np.float32), (n, 1)), np.ones((n, 1), np.float32),
+                   np.zeros((n, 16, 3), np.float32), 3)
+        hit = np.flatnonzero(preprocess_fp32(tr, cam)["det"] == 0)
+        assert hit.size, "no exactly cancelling determinant"
+        sx = sx[hit[:1]]
+        add("cancel_zero" if i == 0 else f"cancel_zero_{i}", np.array([[0.0, 0.0, depth]]),
+            np.array([[sx[0], 0.0, 0.0]]), np.array([[rs[i], 0, 0, zs[i]]]), np.array([0.5]))
+    groups["cancel_zero"] = np.concatenate([groups.pop(k) for k in ("cancel_zero", "cancel_zero_1", "cancel_zero_2")])
+    # radius edges: isotropic splats at depth 30..40, the scale stepped by fp32 ulps until 3 sqrt(lambda_max) hits the
+    # target (the rounding of det and of mid^2 - det makes the radius jump by up to ~1e3 between neighbouring scales, so
+    # a target may need a few positions); beyond 2^31 the scale is only sized
+    n = len(MAGNITUDE_RADII)
+    p = np.zeros((n, 3))
+    s = np.zeros(n, np.float32)
+    steps = np.arange(-20000, 20001)
+    for i, target in enumerate(MAGNITUDE_RADII):
+        for attempt in range(40):
+            p[i] = on_frame(1, 30.0, 40.0)[0]
+
+            def radius_f(cs):
+                m = len(cs)
+                tr = Cloud(np.repeat((p[i:i + 1] * np.array([-1.0, -1.0, 1.0])).astype(np.float32), m, 0),
+                           np.repeat(np.asarray(cs, np.float32)[:, None], 3, 1),
+                           np.tile(np.array([[1, 0, 0, 0]], np.float32), (m, 1)), np.ones((m, 1), np.float32),
+                           np.zeros((m, 16, 3), np.float32), 3)
+                return preprocess_fp32(tr, cam)["radius_f"].astype(np.float64)
+            s[i] = np.float32(target / 3.0 * p[i, 2] / fx)
+            if target > 2.0 ** 32:
+                break
+            s0 = np.float32(s[i] * target / radius_f([s[i]])[0])     # the off-axis Jacobian term, removed
+            cs = (s0.view(np.int32) + steps).astype(np.int32).view(np.float32)
+            hit = np.flatnonzero(radius_f(cs) == target)
+            if hit.size:
+                s[i] = cs[hit[0]]
+                break
+        else:
+            raise AssertionError(("no scale reaches radius", target))
+    add("radius_edge", p, np.repeat(s[:, None], 3, 1), np.tile([1.0, 0, 0, 0], (n, 1)), rng.uniform(0.05, 0.15, n))
+    # overflow (back): isotropic, identity rotation (cov3D diagonal), and rotated anisotropic ones kept where the
+    # cov2 diagonal stays free of NaN
+    s_iso = np.array([1e12, 1e14, 1e16, 1e17, 3e17, 1e18, 3e18, 1e19, 1.8e19])
+    n = s_iso.size
+    p = on_frame(n, 60.0, 90.0)
+    add("overflow", p, np.repeat(s_iso[:, None], 3, 1), np.tile([1.0, 0, 0, 0], (n, 1)), rng.uniform(0.2, 0.9, n))
+    N = 4000
+    p = on_frame(N, 60.0, 90.0)
+    s = 10.0 ** rng.uniform(16.5, 19.2, (N, 3))
+    q = _random_quats(rng, N)
+    trial = Cloud((p * np.array([-1.0, -1.0, 1.0])).astype(np.float32), s.astype(np.float32), q,
+                  np.ones((N, 1), np.float32), np.zeros((N, 16, 3), np.float32), 3)
+    f = preprocess_fp32(trial, cam)
+    ok = ~np.isnan(f["cov2"][:, 0]) & ~np.isnan(f["cov2"][:, 2]) & np.isfinite(f["cov3D"]).all(1)
+    b_inf, b_nan = ok & np.isinf(f["cov2"][:, 1]), ok & np.isnan(f["cov2"][:, 1])
+    b_fin = ok & np.isfinite(f["cov2"][:, 1]) & np.isinf(f["cov2"][:, [0, 2]]).any(1)
+    idx = np.concatenate([np.flatnonzero(b_inf)[:4], np.flatnonzero(b_nan)[:2], np.flatnonzero(b_fin)[:4]])
+    add("overflow_rotated", p[idx], s[idx], q[idx], rng.uniform(0.2, 0.9, idx.size))
+    cloud = Cloud(*(np.ascontiguousarray(np.concatenate([r[i] for r in rows])) for i in range(5)), 3)
+    return cloud, cam, groups
+
+
+def rescaled_patch(kind: str, factor: float, seed: int = 0, P: int = 3000):
+    """A bicycle_cloud patch (SH degree 3) and a look-at camera, 240x160, moved together: kind "translate" adds
+    (factor, -factor/2, factor/3) to every centre, to the eye and to its target, kind "scale" multiplies centres, scales and
+    the eye by factor ("scale" with factor 1 is the patch itself). Fifty Gaussians sit straight in front of the eye at view depths from 1e-6
+    to 60 (log-uniform), so at every factor some fall on each side of the near cut (view z = 0.2, not scale-invariant,
+    nor is the 1e-7 in the projection's w) -> (Cloud, Camera)."""
+    rng = np.random.default_rng(seed)
+    base = bicycle_cloud(P, seed=seed + 1, size=0.5)
+    eye = np.array([0.0, -0.8, -6.0])
+    n = 50
+    z = 10.0 ** rng.uniform(-6, np.log10(60.0), n)
+    fwd = -eye / np.linalg.norm(eye)
+    near = eye + z[:, None] * fwd + rng.normal(0, 1, (n, 3)) * (0.05 * z)[:, None]
+    means = np.concatenate([base.means3D.astype(np.float64), near])
+    scales = np.concatenate([base.scales.astype(np.float64), (0.01 * z)[:, None] * rng.uniform(0.5, 1.5, (n, 3))])
+    extra = Cloud(near.astype(np.float32), scales[-n:].astype(np.float32), _random_quats(rng, n),
+                  rng.uniform(0.02, 0.3, (n, 1)).astype(np.float32), _sh3(rng, n), 3)
+    rot = np.concatenate([base.rotations, extra.rotations])
+    opac = np.concatenate([base.opacities, extra.opacities])
+    shs = np.concatenate([base.shs, extra.shs])
+    target = np.zeros(3)
+    if kind == "translate":
+        t = factor * np.array([1.0, -0.5, 1.0 / 3.0])
+        means, eye, target = means + t, eye + t, target + t
+    elif kind == "scale":
+        means, scales, eye = means * factor, scales * factor, eye * factor
+    else:
+        raise ValueError(kind)
+    cam = look_at_camera(eye, target, (0, -1, 0), 240, 160, fovx_deg=55.0)
+    return Cloud(means.astype(np.float32), scales.astype(np.float32), rot, opac, shs, 3), cam
+
+
 CONFIGS = {
     # name: (P, sh_degree, W, H)
     "c1": dict(P=10_000, sh_degree=0, W=256, H=256),

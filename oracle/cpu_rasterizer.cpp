@@ -74,13 +74,23 @@ template <typename F> M3<F> transpose(const M3<F>& A) {
 // fp64 and rounds once on return; both variants here do the same.
 template <typename F> F ndc2Pix(F v, int S) { return (F)((((double)v + 1.0) * S - 1.0) * 0.5); }
 
-// auxiliary.h:46-56 (float -> int conversions truncate toward zero)
+// float -> int as the GPU converts (cvt.rzi.s32.f32): truncation toward zero, saturating at INT_MIN / INT_MAX, NaN -> 0.
+// A plain (int) cast of an out-of-range or NaN value is undefined in C++ and gives INT_MIN on x86; the reference's CUDA
+// build sees a saturated radius (a splat over the whole grid) where such a cast would see a negative one.
+template <typename F> int to_int_rz(F v) {
+  if (std::isnan(v)) return 0;
+  if (v >= (F)2147483648.0) return INT32_MAX;
+  if (v <= (F)-2147483648.0) return INT32_MIN;
+  return (int)v;
+}
+
+// auxiliary.h:46-56 (float -> int conversions truncate toward zero and saturate, to_int_rz)
 template <typename F>
 void getRect(F px, F py, int max_radius, int gx, int gy, uint32_t* rmin, uint32_t* rmax) {
-  rmin[0] = (uint32_t)std::min(gx, std::max(0, (int)((px - max_radius) / BLOCK_X)));
-  rmin[1] = (uint32_t)std::min(gy, std::max(0, (int)((py - max_radius) / BLOCK_Y)));
-  rmax[0] = (uint32_t)std::min(gx, std::max(0, (int)((px + max_radius + BLOCK_X - 1) / BLOCK_X)));
-  rmax[1] = (uint32_t)std::min(gy, std::max(0, (int)((py + max_radius + BLOCK_Y - 1) / BLOCK_Y)));
+  rmin[0] = (uint32_t)std::min(gx, std::max(0, to_int_rz<F>((px - max_radius) / BLOCK_X)));
+  rmin[1] = (uint32_t)std::min(gy, std::max(0, to_int_rz<F>((py - max_radius) / BLOCK_Y)));
+  rmax[0] = (uint32_t)std::min(gx, std::max(0, to_int_rz<F>((px + max_radius + BLOCK_X - 1) / BLOCK_X)));
+  rmax[1] = (uint32_t)std::min(gy, std::max(0, to_int_rz<F>((py + max_radius + BLOCK_Y - 1) / BLOCK_Y)));
 }
 
 // auxiliary.h:58-77
@@ -129,8 +139,8 @@ void cov2D_setup(V3<F> mean, F focal_x, F focal_y, F tan_fovx, F tan_fovy, const
   c.limy = (F)1.3f * tan_fovy;
   c.txtz = c.t.x / c.t.z;
   c.tytz = c.t.y / c.t.z;
-  c.t.x = std::min(c.limx, std::max(-c.limx, c.txtz)) * c.t.z;
-  c.t.y = std::min(c.limy, std::max(-c.limy, c.tytz)) * c.t.z;
+  c.t.x = std::fmin(c.limx, std::fmax(-c.limx, c.txtz)) * c.t.z;
+  c.t.y = std::fmin(c.limy, std::fmax(-c.limy, c.tytz)) * c.t.z;
   M3<F>& J = c.J;
   J.m[0][0] = focal_x / c.t.z; J.m[0][1] = 0; J.m[0][2] = -(focal_x * c.t.x) / (c.t.z * c.t.z);
   J.m[1][0] = 0; J.m[1][1] = focal_y / c.t.z; J.m[1][2] = -(focal_y * c.t.y) / (c.t.z * c.t.z);
@@ -229,13 +239,13 @@ template <typename F> void preprocess(const Params& p, Geom<F>& g) {
     F det_inv = (F)1 / det;
     F conic[3] = {cz * det_inv, -cy * det_inv, cx * det_inv};
     F mid = (F)0.5f * (cx + cz);
-    F lambda1 = mid + std::sqrt(std::max((F)0.1f, mid * mid - det));
-    F lambda2 = mid - std::sqrt(std::max((F)0.1f, mid * mid - det));
-    F my_radius = std::ceil((F)3 * std::sqrt(std::max(lambda1, lambda2)));
+    F lambda1 = mid + std::sqrt(std::fmax((F)0.1f, mid * mid - det));
+    F lambda2 = mid - std::sqrt(std::fmax((F)0.1f, mid * mid - det));
+    F my_radius = std::ceil((F)3 * std::sqrt(std::fmax(lambda1, lambda2)));
     F pix = ndc2Pix<F>(projx, p.W);
     F piy = ndc2Pix<F>(projy, p.H);
     uint32_t rmin[2], rmax[2];
-    getRect<F>(pix, piy, (int)my_radius, gx, gy, rmin, rmax);
+    getRect<F>(pix, piy, to_int_rz<F>(my_radius), gx, gy, rmin, rmax);
     if ((rmax[0] - rmin[0]) * (rmax[1] - rmin[1]) == 0) continue;
     if (!p.colors_precomp) {
       // forward.cu:20-71 computeColorFromSH
@@ -252,11 +262,11 @@ template <typename F> void preprocess(const Params& p, Geom<F>& g) {
         for (int k = 0; k < nb; k++) res = (k == 0) ? b[0] * (F)sh[ch] : res + b[k] * (F)sh[3 * k + ch];
         res += (F)0.5f;
         g.clamped[3 * (size_t)idx + ch] = res < 0;
-        g.rgb[3 * (size_t)idx + ch] = std::max(res, (F)0);
+        g.rgb[3 * (size_t)idx + ch] = std::fmax(res, (F)0);
       }
     }
     g.depths[idx] = p_view.z;
-    g.radii[idx] = (int)my_radius;
+    g.radii[idx] = to_int_rz<F>(my_radius);
     g.means2D[2 * (size_t)idx] = pix; g.means2D[2 * (size_t)idx + 1] = piy;
     g.conic_opacity[4 * (size_t)idx + 0] = conic[0]; g.conic_opacity[4 * (size_t)idx + 1] = conic[1];
     g.conic_opacity[4 * (size_t)idx + 2] = conic[2]; g.conic_opacity[4 * (size_t)idx + 3] = p.opacities[idx];
@@ -370,7 +380,7 @@ void render_forward(const Params& p, const Geom<F>& g, const Binning& b, Image<F
           F power = (F)-0.5f * (co[0] * dx * dx + co[2] * dy * dy) - co[1] * dx * dy;
           pairs++;
           if (power > 0) continue;
-          F alpha = std::min((F)0.99f, co[3] * std::exp(power));
+          F alpha = std::fmin((F)0.99f, co[3] * std::exp(power));
           if (alpha < (F)(1.0f / 255.0f)) continue;
           F test_T = T * (1 - alpha);
           if (test_T < (F)0.0001f) break;  // done = true
@@ -438,7 +448,7 @@ void render_backward(const Params& p, const Geom<F>& g, const Binning& b, const 
             F power = (F)-0.5f * (co[0] * dx * dx + co[2] * dy * dy) - co[1] * dx * dy;
             if (power > 0) continue;
             F G = std::exp(power);
-            F alpha = std::min((F)0.99f, co[3] * G);
+            F alpha = std::fmin((F)0.99f, co[3] * G);
             if (alpha < (F)(1.0f / 255.0f)) continue;
             T = T / ((F)1 - alpha);
             F dchannel_dcolor = alpha * T;
@@ -810,7 +820,7 @@ ORACLE_API void oracle_apply_weights(void* h, float* weights, int32_t* cnt, cons
           const float* co = &g.conic_opacity[4 * (size_t)id];
           float power = -0.5f * (co[0] * dx * dx + co[2] * dy * dy) - co[1] * dx * dy;
           if (power > 0.0f) continue;
-          float alpha = std::min(0.99f, co[3] * std::exp(power));
+          float alpha = std::fmin(0.99f, co[3] * std::exp(power));
           if (alpha < 1.0f / 255.0f) continue;
           float test_T = T * (1 - alpha);
           if (test_T < 0.0001f) break;

@@ -144,13 +144,10 @@ __attribute__((visibility("default"))) void subblock_scene(int P, const float* m
       const float x = means2D[2 * i], y = means2D[2 * i + 1];
       const float4 q0 = make_float4(x, y, conic_opacity[4 * i], conic_opacity[4 * i + 1]);
       const float4 q1 = make_float4(conic_opacity[4 * i + 2], conic_opacity[4 * i + 3], 0.f, 0.f);
-      const int rr = radii[i];
-      const int x0 = std::min(gx, std::max(0, (int)((x - rr) / gsr::TILE)));
-      const int y0 = std::min(gy, std::max(0, (int)((y - rr) / gsr::TILE)));
-      const int x1 = std::min(gx, std::max(0, (int)((x + rr + gsr::TILE - 1) / gsr::TILE)));
-      const int y1 = std::min(gy, std::max(0, (int)((y + rr + gsr::TILE - 1) / gsr::TILE)));
-      for (int ty = y0; ty < y1; ty++)
-        for (int tx = x0; tx < x1; tx++) check_tile_any(term_ulps, q0, q1, tx, ty, W, H, c);
+      uint2 rmin, rmax;  // the kernels' own rectangle (saturating conversions: a radius of INT_MAX covers the grid)
+      gsr::tile_rect(x, y, radii[i], gx, gy, rmin, rmax);
+      for (int ty = (int)rmin.y; ty < (int)rmax.y; ty++)
+        for (int tx = (int)rmin.x; tx < (int)rmax.x; tx++) check_tile_any(term_ulps, q0, q1, tx, ty, W, H, c);
     }
 #pragma omp critical
     add(total, c);

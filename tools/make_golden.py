@@ -13,6 +13,8 @@ are what pins the CPU oracle and our kernels to the reference's actual outputs w
                                   by   python tools/make_golden.py OUT_DIR camera_models
   * tile_grid_reference.npz       (goes to tests/golden/parity/) the same for tests/test_tile_grid.py, written alone by
                                   python tools/make_golden.py OUT_DIR tile_grid
+  * magnitudes_reference.npz      (goes to tests/golden/parity/) the same for tests/test_magnitudes.py, written alone by
+                                  python tools/make_golden.py OUT_DIR magnitudes
 """
 import os
 import sys
@@ -76,6 +78,14 @@ def main():
         import test_camera_models as CM
         np.savez_compressed(os.path.join(OUT, "camera_models_reference.npz"),
                             **record((CM.test_forward_mark_visible_apply_weights_match_reference,)))
+        print("golden written to", OUT)
+        return
+    if sys.argv[2:] == ["magnitudes"]:
+        import test_magnitudes as MG
+        np.savez_compressed(os.path.join(OUT, "magnitudes_reference.npz"),
+                            **record((MG.test_forward_bit_exact_every_variant, MG.test_backward_against_reference,
+                                      MG.test_translated_patch_matches_reference,
+                                      MG.test_mark_visible_and_apply_weights_bit_exact)))
         print("golden written to", OUT)
         return
     if sys.argv[2:] == ["tile_grid"]:
